@@ -13,6 +13,8 @@
  *   check_tx_sigs_batch        the per-HTLC loop of channeld/channeld.c:2215-2232 (one shared key,
  *                              n sighashes, n signatures) as one launch
  *
+ *   bolt12_check_signature     common/bolt12.h           (common/bolt12.c:80-92) — same signature; the TLV Merkle root
+ *                              and sighash are computed on the device
  *   check_tx_sig               bitcoin/signature.h:120   (bitcoin/signature.c:194-221) — same signature; the BIP143
  *                              sighash (bitcoin_tx_hash_for_sig :120-151 -> libwally tx_io.c:660-765) is computed
  *                              on the device from the wally_tx fields
@@ -98,6 +100,13 @@ struct wally_tx {
 struct chainparams;
 struct wally_psbt;
 struct bitcoin_tx { struct wally_tx *wtx; const struct chainparams *chainparams; struct wally_psbt *psbt; }; /* bitcoin/tx.h:32-40 */
+struct tlv_record_type;
+struct tlv_field {                         /* wire/tlvstream.h:16-27 */
+    const struct tlv_record_type *meta;
+    uint64_t numtype;
+    size_t length;
+    u8 *value;
+};
 #endif
 
 /* Optional: choose the CUDA device (default: $CLN_SIGVERIFY_DEVICE or 0).  The context is created
@@ -121,6 +130,15 @@ bool check_tx_sig(const struct bitcoin_tx *tx, size_t input_num, const u8 *redee
                   const struct pubkey *key, const struct bitcoin_signature *sig);
 void cln_sigverify_set_tx_hooks(size_t (*script_bytelen)(const void *tal_script),
                                 uint64_t (*input_amount_sat)(const struct bitcoin_tx *tx, size_t input_num));
+
+/* common/bolt12.h: bolt12_check_signature (common/bolt12.c:80-92).  fields is a tal array (its length comes from
+ * tal_bytelen(fields) / sizeof(struct tlv_field), through the same weak tal_bytelen reference or hook as check_tx_sig);
+ * the fields are serialised in array order into one TLV stream and sent to sv_verify_bolt12_host, which builds the
+ * Merkle root and sighash on the device.  CLN only passes strictly ascending arrays (fromwire_tlv and tlv_update_fields
+ * produce them), and for those the result is CLN's.  An array that is not strictly ascending by type, or is empty (merkle_tlv
+ * asserts on that), is not a stream CLN's parser produces: the function returns false for it. */
+bool bolt12_check_signature(const struct tlv_field *fields, const char *messagename, const char *fieldname,
+                            const struct pubkey *key, const struct bip340sig *sig);
 
 /* channeld HTLC loop: ok[i] = check_signed_hash(&hashes[i], &sigs[i].s, key) for one shared key. */
 void check_tx_sigs_batch(const struct sha256_double *hashes, const struct bitcoin_signature *sigs,

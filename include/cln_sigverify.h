@@ -16,6 +16,12 @@
  *                                           with a BIP143 preimage as the span, check_tx_sig()
  *                                           bitcoin/signature.c:194-221 (the per-HTLC loop of
  *                                           channeld/channeld.c:2215-2232)
+ *   sv_verify_bolt12_host(...)              bolt12_check_signature()     common/bolt12.c:80-92: merkle_tlv()
+ *                                           common/bolt12_merkle.c:160-194 over the fields fromwire_tlv()
+ *                                           wire/tlvstream.c:144-300 parses, sighash_from_merkle() :210-220,
+ *                                           check_schnorr_sig(); callers plugins/offers_invreq_hook.c:634-637,
+ *                                           plugins/offers_inv_hook.c:177-179, plugins/fetchinvoice.c:256-260,
+ *                                           :1501-1507, lightningd/offer.c:88-89, devtools/bolt12-cli.c:319-321
  *   sv_sha256d_host(...)                    sha256_double()              bitcoin/shadouble.c:7-11
  *   sv_pubkey_parse_host(...)               pubkey_from_der()            bitcoin/pubkey.c:14-24
  *   sv_enqueue_* / sv_flush                 the deferral queue a batching caller (gossipd ingest,
@@ -176,6 +182,23 @@ typedef struct {
 int sv_verify_tx_host(sv_ctx *ctx, int kind, const sv_tx *txs, const uint8_t *scripts, size_t scripts_len,
                       const uint8_t *key, const uint8_t *sig64, size_t n, uint8_t *verdicts, uint8_t *sighash32_out);
 
+/* ---- BOLT12 signatures with the message hash computed ON THE DEVICE: bolt12_check_signature (common/bolt12.c:80-92)
+ *      for n TLV streams.  Stream i is blob[off[i] .. off[i]+len[i]), the raw TLV bytes of an offer, invoice_request or
+ *      invoice (signature fields included: they are outside the Merkle tree).  The device parses each stream as
+ *      fromwire_tlv with any type allowed does (wire/tlvstream.c:144-300: minimal BigSize type and length, strictly
+ *      increasing types, no length past the end), builds merkle_tlv's root (common/bolt12_merkle.c:160-194), hashes it
+ *      with the tag "lightning" || messagename || fieldname (sighash_from_merkle, :210-220) and verifies BIP-340 exactly as
+ *      sv_verify_host(SV_KIND_SCHNORR) does: xonly32[i] is the key's x coordinate (check_schnorr_sig drops the parity,
+ *      bitcoin/signature.c:412-423), sig64[i] the signature.
+ *      status[i] = 1  bolt12_check_signature would return true;
+ *                  0  it would return false (including an x that is not on the curve, r >= p, s >= n);
+ *                 -1  the stream is not one CLN's TLV parser produces fields from, or it is empty.
+ *      sighash32_out (optional, n x 32) returns the sighashes, zeros where status is -1.  No bound on fields per stream or
+ *      value length beyond the 32-bit span length.  Spans out of range or NULL required pointers: SV_ERR_ARG. ---- */
+int sv_verify_bolt12_host(sv_ctx *ctx, const char *messagename, const char *fieldname, const uint8_t *blob,
+                          size_t blob_len, const uint64_t *off, const uint32_t *len, const uint8_t *xonly32,
+                          const uint8_t *sig64, size_t n, int *status, uint8_t *sighash32_out);
+
 /* ---- DEVICE buffers (same SoA layout, device pointers); asynchronous on `stream`
  *      (a cudaStream_t passed as void*; NULL = the context's own stream).  d_verdicts[n] bytes;
  *      d_bitmap, if non-NULL, receives ceil(n/32) little-endian 32-bit words, bit i%32 of word i/32. ---- */
@@ -263,6 +286,8 @@ int sv_get_info(const sv_ctx *ctx, sv_info *info);
  * around the scalar-side and curve-side kernels; read them back after synchronising. */
 int sv_set_profiling(sv_ctx *ctx, int on);
 int sv_get_last_timing(sv_ctx *ctx, float *prep_ms, float *main_ms);
+/* the same for the last sv_verify_bolt12_host call: parse + Merkle + sighash kernels, then the verification kernels */
+int sv_get_last_bolt12_timing(sv_ctx *ctx, float *merkle_ms, float *verify_ms);
 
 /* integer-pipe roofline probe: runs a dependent-chain IMAD.WIDE.U32 microbenchmark and returns the
  * achieved 32x32->64 multiply-accumulates per second on this device (the roofline denominator

@@ -5,6 +5,7 @@ Everything is built IN-TREE, so the package and the tests run from the source tr
   tests/host_emul/libemul.so           kernel headers compiled for the host, tests only [g++]
   oracle/libsecp_port.so               the plain-C restatement oracle                 [gcc]
   oracle/_ref/libsecp_ref.so           the unmodified reference, from the Core Lightning tree at $CLN_SRC or /root/reference [gcc]
+  oracle/_ref/libcln_ref.so, libcln_bolt12.so   CLN's own plumbing and BOLT12 Merkle code from the same tree [gcc]
 """
 import os
 import shutil
@@ -83,11 +84,11 @@ def build_engine(force=False, verbose=False, extra_flags=()):
 
 
 def build_host_emul(force=False):
-    src = os.path.join(ROOT, "tests", "host_emul", "emul.cpp")
-    srcs = _sources(CSRC, (".cuh",)) + [src]
+    src = [os.path.join(ROOT, "tests", "host_emul", f) for f in ("emul.cpp", "bolt12_emul.cpp")]
+    srcs = _sources(CSRC, (".cuh",)) + src
     if not force and _newer(EMUL, srcs):
         return EMUL
-    cmd = ["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-pthread", "-Wall", "-Wno-unused-function", "-o", EMUL, src]
+    cmd = ["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-pthread", "-Wall", "-Wno-unused-function", "-o", EMUL] + src
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("g++ (host_emul) failed:\n" + r.stdout + r.stderr)
@@ -99,6 +100,11 @@ def build_oracle():
                        stdin=subprocess.DEVNULL, timeout=900)
     if r.returncode != 0:
         raise RuntimeError("oracle build failed:\n" + r.stdout + r.stderr)
+    # the reference's BOLT12 Merkle code, linked against the library above
+    r = subprocess.run(["make", "-C", os.path.join(ROOT, "oracle"), "-f", "bolt12.mk", "all"], capture_output=True, text=True,
+                       stdin=subprocess.DEVNULL, timeout=900)
+    if r.returncode != 0:
+        raise RuntimeError("oracle build (bolt12.mk) failed:\n" + r.stdout + r.stderr)
 
 
 def build_all(force=False, verbose=False):

@@ -214,6 +214,45 @@ bool check_tx_sig(const struct bitcoin_tx *tx, size_t input_num, const u8 *redee
     return v == 1;
 }
 
+/* ---- bolt12_check_signature (common/bolt12.c:80-92): the fields go back to wire form (towire_tlvstream_raw's layout:
+ * BigSize type, BigSize length, value), the device does merkle_tlv, sighash_from_merkle and check_schnorr_sig ---- */
+static size_t put_bigsize(u8 *p, uint64_t v) { /* common/bigsize.c bigsize_put */
+    size_t n = v < 0xfd ? 1 : v <= 0xffff ? 3 : v <= 0xffffffffu ? 5 : 9;
+    if (n == 1) { p[0] = (u8)v; return 1; }
+    p[0] = n == 3 ? 0xfd : n == 5 ? 0xfe : 0xff;
+    for (size_t i = 1; i < n; i++) p[i] = (u8)(v >> (8 * (n - 1 - i)));
+    return n;
+}
+
+bool bolt12_check_signature(const struct tlv_field *fields, const char *messagename, const char *fieldname,
+                            const struct pubkey *key, const struct bip340sig *sig) {
+    size_t bytes;
+    if (g_bytelen) bytes = fields ? g_bytelen(fields) : 0;
+    else if (tal_bytelen) bytes = fields ? tal_bytelen(fields) : 0;
+    else die("bolt12_check_signature: no tal_bytelen (cln_sigverify_set_tx_hooks)", -4);
+    size_t nf = bytes / sizeof(struct tlv_field), total = 0;
+    for (size_t i = 0; i < nf; i++) total += 18 + fields[i].length;
+    if (total > 0xffffffffu) die("bolt12_check_signature: stream longer than 4 GiB", -4);
+    u8 *blob = (u8 *)malloc(total ? total : 1);
+    if (!blob) die("malloc", -3);
+    size_t n = 0;
+    for (size_t i = 0; i < nf; i++) {
+        n += put_bigsize(blob + n, fields[i].numtype);
+        n += put_bigsize(blob + n, fields[i].length);
+        if (fields[i].length) memcpy(blob + n, fields[i].value, fields[i].length);
+        n += fields[i].length;
+    }
+    uint64_t off = 0;
+    uint32_t len = (uint32_t)n;
+    u8 xy[64];
+    int status = 0;
+    pubkey_to_xy(xy, &key->pubkey); /* x-only: the first 32 bytes */
+    int rc = sv_verify_bolt12_host(ctx(), messagename, fieldname, blob, n, &off, &len, xy, sig->u8, 1, &status, NULL);
+    free(blob);
+    if (rc != SV_OK) die("sv_verify_bolt12_host", rc);
+    return status == 1;
+}
+
 void check_tx_sigs_batch(const struct sha256_double *hashes, const struct bitcoin_signature *sigs,
                          const struct pubkey *key, size_t n, bool *ok) {
     if (n == 0) return;

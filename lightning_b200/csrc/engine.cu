@@ -13,6 +13,7 @@
 //       k_small<kind>                    one-launch latency path for small batches (5 warps per 32 verifications)
 //       k_main_shared, k_dedup_*, k_sharedkey_build_many   one multiples table per distinct key (same-key / gossip batches)
 //       k_gossip_slice / _status, k_bip143, k_mixed_*       callers' data formats on the device (rows N1, N2, C3)
+//       k_b12_*                          BOLT12 streams: TLV parse, Merkle root (one warp per stream), tagged sighash
 //       k_sb_* (batch.cu)                BIP-340 batch verification by random linear combination
 //       k_pack_bitmap                    verdict bytes -> 1 bit per verification (ballot)
 //       k_pubkey_parse                   batched pubkey_from_der
@@ -30,6 +31,7 @@
 
 #include "../../include/cln_sigverify.h"
 #include "verify.cuh"
+#include "bolt12.cuh"
 #include "selftest.cuh"
 #include "batch.cuh"  // constants and the host-testable stages; the kernels themselves are in batch.cu
 
@@ -500,6 +502,157 @@ __global__ void __launch_bounds__(128) k_gossip_status(const u8* blob, const u64
     status[m] = st;
 }
 
+// ---- BOLT12 signatures (bolt12.cuh): the message hash of bolt12_check_signature on the device -----------------------
+// k_b12_count: one thread per stream walks its BigSize headers (bytes only): field count, or 0 if the parse fails
+__global__ void __launch_bounds__(128) k_b12_count(const u8* blob, const u64* off, const u32* len, size_t n, u32* cnt) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    long long c = b12_count(blob + off[i], len[i]);
+    cnt[i] = c < 0 ? 0u : (u32)c;
+}
+// exclusive prefix sum of the field counts (u64): block-local scan, scan of the block totals, add-back.  sums[nb] = total.
+#define SV_B12_SCAN 1024
+__device__ __forceinline__ u64 b12_block_scan(u64 v, u64* total) {
+    __shared__ u64 warp_sums[SV_B12_SCAN / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    u64 x = v;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        u64 y = __shfl_up_sync(0xFFFFFFFFu, x, d);
+        if (lane >= d) x += y;
+    }
+    if (lane == 31) warp_sums[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        u64 s = lane < (int)(blockDim.x >> 5) ? warp_sums[lane] : 0;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            u64 y = __shfl_up_sync(0xFFFFFFFFu, s, d);
+            if (lane >= d) s += y;
+        }
+        warp_sums[lane] = s;
+    }
+    __syncthreads();
+    u64 excl = x - v + (warp ? warp_sums[warp - 1] : 0);
+    *total = warp_sums[(blockDim.x >> 5) - 1];
+    __syncthreads();
+    return excl;
+}
+__global__ void __launch_bounds__(SV_B12_SCAN) k_b12_scan_local(const u32* cnt, size_t n, u64* base, u64* sums) {
+    size_t i = (size_t)blockIdx.x * SV_B12_SCAN + threadIdx.x;
+    u64 total;
+    u64 e = b12_block_scan(i < n ? cnt[i] : 0, &total);
+    if (i < n) base[i] = e;
+    if (threadIdx.x == 0) sums[blockIdx.x] = total;
+}
+__global__ void __launch_bounds__(SV_B12_SCAN) k_b12_scan_sums(u64* sums, size_t nb) {
+    u64 carry = 0;
+    for (size_t c = 0; c < nb; c += SV_B12_SCAN) {
+        size_t i = c + threadIdx.x;
+        u64 total;
+        u64 e = b12_block_scan(i < nb ? sums[i] : 0, &total);
+        if (i < nb) sums[i] = carry + e;
+        carry += total;
+    }
+    if (threadIdx.x == 0) sums[nb] = carry;
+}
+__global__ void __launch_bounds__(SV_B12_SCAN) k_b12_scan_add(u64* base, size_t n, const u64* sums) {
+    size_t i = (size_t)blockIdx.x * SV_B12_SCAN + threadIdx.x;
+    if (i < n) base[i] += sums[blockIdx.x];
+}
+__global__ void k_b12_tags(const u8* sigtag, u32 sigtag_len, b12_tags* tags) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) b12_make_tags(tags, sigtag, sigtag_len);
+}
+// k_b12_merkle: one warp per stream.  Lane 0 walks the headers into the field records; the lanes hash one field each
+// (leaf, nonce, leaf pair; strided past 32 fields); signature-range fields drop out by ballot / popc compaction; then the
+// tree is reduced one level per step (neighbours paired, an odd last node carried up: merkle_tlv's power-of-two split);
+// lane 0 hashes the root into the sighash.  Failed parses get a zero sighash (they are never verified as signed).
+#define SV_B12_WARPS 4
+__global__ void __launch_bounds__(32 * SV_B12_WARPS) k_b12_merkle(const u8* blob, const u64* off, const u32* len, size_t n,
+                                                                  const u32* cnt, const u64* fbase, const b12_tags* tags,
+                                                                  b12_field* recs, u32* nodes, u8* msg32) {
+    const size_t i = (size_t)blockIdx.x * SV_B12_WARPS + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (i >= n) return;  // whole warps leave together
+    const u32 F = cnt[i];
+    if (F == 0) {
+        msg32[32 * i + lane] = 0;
+        return;
+    }
+    const u8* p = blob + off[i];
+    const u32 L = len[i];
+    b12_field* rec = recs + fbase[i];
+    u32* node = nodes + 8 * fbase[i];
+    __shared__ b12_tags s_tags[SV_B12_WARPS];  // one copy per warp: warps leave early, so no CTA-wide barrier
+    u32 nm[8];
+    if (lane == 0) {
+        u32 pos = 0;
+        u64 prev = 0;
+        for (u32 j = 0; j < F; j++) {
+            b12_field f;
+            b12_next(p, L, &pos, j == 0, prev, &f);  // cannot fail: k_b12_count walked the same bytes
+            prev = f.type;
+            rec[j] = f;
+        }
+        b12_nonce_mid(nm, p + rec[0].off, rec[0].len);
+    }
+#pragma unroll
+    for (int k = 0; k < 8; k++) nm[k] = __shfl_sync(0xFFFFFFFFu, nm[k], 0);
+    b12_tags& t = s_tags[threadIdx.x >> 5];
+    if (lane < 24) reinterpret_cast<u32*>(&t)[lane] = reinterpret_cast<const u32*>(tags)[lane];
+    __syncwarp();
+    u32 m = 0;  // non-signature fields so far
+    for (u32 j0 = 0; j0 < F; j0 += 32) {
+        const u32 j = j0 + lane;
+        b12_field f;
+        bool leaf = false;
+        if (j < F) {
+            f = rec[j];
+            leaf = !b12_is_signature(f.type);
+        }
+        u32 h[8];
+        if (leaf) b12_leaf_pair(h, &t, nm, p, f);
+        const unsigned b = __ballot_sync(0xFFFFFFFFu, leaf);
+        if (leaf) {
+            u32* d = node + 8 * (m + __popc(b & ((1u << lane) - 1u)));
+#pragma unroll
+            for (int k = 0; k < 8; k++) d[k] = h[k];
+        }
+        m += __popc(b);
+    }
+    __syncwarp();
+    while (m > 1) {
+        const u32 up = (m + 1) / 2;
+        for (u32 k0 = 0; k0 < up; k0 += 32) {
+            const u32 k = k0 + lane;
+            u32 h[8];
+            if (2 * k + 1 < m) b12_branch(h, t.branch, node + 16 * k, node + 16 * k + 8);
+            else if (k < up) {
+#pragma unroll
+                for (int q = 0; q < 8; q++) h[q] = node[16 * k + q];
+            }
+            __syncwarp();  // every lane has read its pair before any lane of this round overwrites a slot
+            if (k < up) {
+#pragma unroll
+                for (int q = 0; q < 8; q++) node[8 * k + q] = h[q];
+            }
+            __syncwarp();
+        }
+        m = up;
+    }
+    if (lane == 0) {
+        u32 root[8];
+#pragma unroll
+        for (int q = 0; q < 8; q++) root[q] = m ? node[q] : 0u;  // no non-signature field: merkle_tlv's all-zero root
+        b12_sighash(msg32 + 32 * i, &t, root);
+    }
+}
+// status[i] = verdict where the stream parsed, -1 where it did not
+__global__ void __launch_bounds__(256) k_b12_status(const u32* cnt, const u8* verdict, size_t n, int* status) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) status[i] = cnt[i] ? (int)verdict[i] : -1;
+}
+
 static_assert(sizeof(sv_jac) == sizeof(sv_work), "R is parked in place of the work record");
 __global__ void __launch_bounds__(64) k_final_schnorr(const sv_work* work, const u8* sig, size_t n, u8* verdict) {
     size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -889,8 +1042,12 @@ struct sv_ctx {
     // gossip ingest scratch (grow-only)
     u8* g_buf;
     size_t g_cap;
+    // BOLT12 field records and tree nodes (grow-only, sized by the counting pass)
+    u8* b12_buf;
+    size_t b12_cap;
     int profiling;
     cudaEvent_t ev[3];  // before prep, between prep and main, after main (profiling mode only)
+    cudaEvent_t b12_ev[2];  // around the BOLT12 parse / Merkle / sighash kernels (profiling mode only)
     unsigned long long launches;
     std::vector<sv_queue_item> queue;
     std::string err;
@@ -1013,8 +1170,11 @@ extern "C" int sv_create(sv_ctx** out, int device) {
     ctx->launches = 0;
     ctx->g_buf = nullptr;
     ctx->g_cap = 0;
+    ctx->b12_buf = nullptr;
+    ctx->b12_cap = 0;
     ctx->profiling = 0;
     ctx->ev[0] = ctx->ev[1] = ctx->ev[2] = nullptr;
+    ctx->b12_ev[0] = ctx->b12_ev[1] = nullptr;
     ctx->stream = ctx->stream2 = ctx->copy_stream = nullptr;
     for (int i = 0; i < 8; i++) ctx->h2d_ev[i] = nullptr;
     cudaDeviceProp prop;
@@ -1104,8 +1264,9 @@ extern "C" void sv_destroy(sv_ctx* ctx) {
         if (ctx->slot[i].done) cudaEventDestroy(ctx->slot[i].done);
     }
     cudaFree(ctx->d_msg); cudaFree(ctx->d_key); cudaFree(ctx->d_sig); cudaFree(ctx->d_verdict);
-    cudaFree(ctx->d_data); cudaFree(ctx->d_off); cudaFree(ctx->d_len); cudaFree(ctx->g_buf);
+    cudaFree(ctx->d_data); cudaFree(ctx->d_off); cudaFree(ctx->d_len); cudaFree(ctx->g_buf); cudaFree(ctx->b12_buf);
     for (int i = 0; i < 3; i++) if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
+    for (int i = 0; i < 2; i++) if (ctx->b12_ev[i]) cudaEventDestroy(ctx->b12_ev[i]);
     for (int i = 0; i < 8; i++) if (ctx->h2d_ev[i]) cudaEventDestroy(ctx->h2d_ev[i]);
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
     if (ctx->stream2) cudaStreamDestroy(ctx->stream2);
@@ -1343,7 +1504,16 @@ extern "C" int sv_set_profiling(sv_ctx* ctx, int on) {
     CK(dg__.enter(ctx->device));
     if (on && !ctx->ev[0])
         for (int i = 0; i < 3; i++) CK(cudaEventCreate(&ctx->ev[i]));
+    if (on && !ctx->b12_ev[0])
+        for (int i = 0; i < 2; i++) CK(cudaEventCreate(&ctx->b12_ev[i]));
     ctx->profiling = on ? 1 : 0;
+    return SV_OK;
+}
+// device time of the last sv_verify_bolt12_host call: parse + Merkle + sighash kernels, then the verification kernels
+extern "C" int sv_get_last_bolt12_timing(sv_ctx* ctx, float* merkle_ms, float* verify_ms) {
+    if (!ctx || !ctx->profiling || !merkle_ms || !verify_ms) return SV_ERR_ARG;
+    CK(cudaEventElapsedTime(merkle_ms, ctx->b12_ev[0], ctx->b12_ev[1]));
+    CK(cudaEventElapsedTime(verify_ms, ctx->ev[0], ctx->ev[2]));
     return SV_OK;
 }
 // device time of the last sv_verify_* launch pair (call after the stream has been synchronised)
@@ -1771,6 +1941,81 @@ extern "C" int sv_verify_mixed_host(sv_ctx* ctx, const uint8_t* kinds, const uin
     rc = mixed_device(ctx, d_kinds, d_m, d_k, d_s, n, d_o, reinterpret_cast<u32*>(ctx->g_buf), st);
     if (rc) return rc;
     CK(cudaMemcpyAsync(verdicts, d_o, n, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return SV_OK;
+}
+
+// ---- BOLT12: bolt12_check_signature (common/bolt12.c:80-92) for n TLV streams -------------------------------------------
+// The host copies bytes only.  The device parses every stream, builds its Merkle root and sighash (k_b12_*), verifies the
+// sighashes through the ordinary BIP-340 path (launch_verify) and folds parse status and verdict into one int.  One host
+// synchronisation in the middle: the total field count sizes the record / node scratch.
+extern "C" int sv_verify_bolt12_host(sv_ctx* ctx, const char* messagename, const char* fieldname, const uint8_t* blob,
+                                     size_t blob_len, const uint64_t* off, const uint32_t* len, const uint8_t* xonly32,
+                                     const uint8_t* sig64, size_t n, int* status, uint8_t* sighash32_out) {
+    if (!ctx || !messagename || !fieldname || (n && (!blob || !off || !len || !xonly32 || !sig64 || !status))) return SV_ERR_ARG;
+    if (n == 0) return SV_OK;
+    dev_guard dg__;
+    CK(dg__.enter(ctx->device));
+    int rc = ensure_staging(ctx, n);
+    if (rc) return rc;
+    rc = stage_spans(ctx, blob, blob_len, off, len, n);
+    if (rc) return rc;
+    // bip340_sighash_init(sctx, "lightning", messagename, fieldname): the tag is the three strings back to back
+    std::string tag = std::string("lightning") + messagename + fieldname;
+    if (tag.size() > 0xFFFFFFFFu) return fail(ctx, SV_ERR_ARG, "tag too long", cudaSuccess);
+    const size_t nb = (n + SV_B12_SCAN - 1) / SV_B12_SCAN;
+    // per-call scratch in the auxiliary slab: [cnt u32 n][base u64 n][block sums u64 nb+1][status int n][tags][tag bytes]
+    auto up16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
+    const size_t o_base = up16(4 * n), o_sums = o_base + 8 * n, o_status = up16(o_sums + 8 * (nb + 1)),
+                 o_tags = up16(o_status + 4 * n), o_tag = o_tags + up16(sizeof(b12_tags)), need = o_tag + tag.size() + 64;
+    rc = ensure_gbuf(ctx, need);
+    if (rc) return rc;
+    u32* d_cnt = reinterpret_cast<u32*>(ctx->g_buf);
+    u64* d_base = reinterpret_cast<u64*>(ctx->g_buf + o_base);
+    u64* d_sums = reinterpret_cast<u64*>(ctx->g_buf + o_sums);
+    int* d_status = reinterpret_cast<int*>(ctx->g_buf + o_status);
+    b12_tags* d_tags = reinterpret_cast<b12_tags*>(ctx->g_buf + o_tags);
+    u8* d_tag = ctx->g_buf + o_tag;
+    cudaStream_t st = ctx->stream;
+    CK(cudaMemcpyAsync(ctx->d_key, xonly32, 32 * n, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(ctx->d_sig, sig64, 64 * n, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_tag, tag.data(), tag.size(), cudaMemcpyHostToDevice, st));
+    if (ctx->profiling) cudaEventRecord(ctx->b12_ev[0], st);
+    k_b12_tags<<<1, 32, 0, st>>>(d_tag, (u32)tag.size(), d_tags);
+    k_b12_count<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(ctx->d_data, ctx->d_off, ctx->d_len, n, d_cnt);
+    k_b12_scan_local<<<(unsigned)nb, SV_B12_SCAN, 0, st>>>(d_cnt, n, d_base, d_sums);
+    k_b12_scan_sums<<<1, SV_B12_SCAN, 0, st>>>(d_sums, nb);
+    k_b12_scan_add<<<(unsigned)nb, SV_B12_SCAN, 0, st>>>(d_base, n, d_sums);
+    ctx->launches += 5;
+    CK(cudaGetLastError());
+    u64 total = 0;
+    CK(cudaMemcpyAsync(&total, d_sums + nb, sizeof total, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    const size_t per_field = sizeof(b12_field) + 32;
+    if (total > ((size_t)-1) / per_field) return fail(ctx, SV_ERR_NOMEM, "BOLT12 field scratch", cudaSuccess);
+    const size_t need_f = (size_t)total * per_field;
+    if (need_f > ctx->b12_cap) {
+        size_t want = ctx->b12_cap ? ctx->b12_cap : (1u << 20);
+        while (want < need_f) want *= 2;
+        cudaFree(ctx->b12_buf); ctx->b12_buf = nullptr; ctx->b12_cap = 0;
+        CK(cudaMalloc(&ctx->b12_buf, want));
+        ctx->b12_cap = want;
+    }
+    b12_field* d_recs = reinterpret_cast<b12_field*>(ctx->b12_buf);
+    u32* d_nodes = reinterpret_cast<u32*>(ctx->b12_buf + (size_t)total * sizeof(b12_field));
+    k_b12_merkle<<<(unsigned)((n + SV_B12_WARPS - 1) / SV_B12_WARPS), 32 * SV_B12_WARPS, 0, st>>>(
+        ctx->d_data, ctx->d_off, ctx->d_len, n, d_cnt, d_base, d_tags, d_recs, d_nodes, ctx->d_msg);
+    ctx->launches += 1;
+    if (ctx->profiling) cudaEventRecord(ctx->b12_ev[1], st);
+    CK(cudaGetLastError());
+    // the sighashes are ordinary BIP-340 messages from here on: small-batch kernel or the throughput kernels
+    rc = launch_verify(ctx, SV_KIND_SCHNORR, ctx->d_msg, ctx->d_key, ctx->d_sig, n, ctx->d_verdict, nullptr, st);
+    if (rc) return rc;
+    k_b12_status<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_cnt, ctx->d_verdict, n, d_status);
+    ctx->launches += 1;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(status, d_status, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+    if (sighash32_out) CK(cudaMemcpyAsync(sighash32_out, ctx->d_msg, 32 * n, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     return SV_OK;
 }

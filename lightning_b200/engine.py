@@ -61,6 +61,8 @@ def load_library():
     lib.sv_verify_gossip_host.argtypes = [vp, vp, sz, vp, vp, sz, vp, vp]
     lib.sv_verify_tx_host.argtypes = [vp, i, vp, vp, sz, vp, vp, sz, vp, vp]
     lib.sv_verify_samekey_host.argtypes = [vp, i, vp, vp, vp, sz, vp]
+    lib.sv_verify_bolt12_host.argtypes = [vp, ctypes.c_char_p, ctypes.c_char_p, vp, sz, vp, vp, vp, vp, sz, vp, vp]
+    lib.sv_get_last_bolt12_timing.argtypes = [vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float)]
     lib.sv_sync.argtypes = [vp, vp]
     lib.sv_get_stream.argtypes = [vp]
     lib.sv_set_profiling.argtypes = [vp, i]
@@ -213,6 +215,42 @@ class SigVerifier:
                                                key.ctypes.data, sig64.ctypes.data, n, out.ctypes.data,
                                                sh.ctypes.data if want_sighash else None), "sv_verify_tx_host")
         return (out[:n], sh[:n]) if want_sighash else out[:n]
+
+    def verify_bolt12(self, messagename, fieldname, streams, xonly, sig, want_sighash=False):
+        """bolt12_check_signature (common/bolt12.c:80) for n raw TLV streams, Merkle root and sighash computed on the
+        device.  streams: sequence of bytes-like; xonly (n, 32); sig (n, 64).  Returns int32 statuses (1 valid, 0 invalid,
+        -1 not a TLV stream CLN parses, or empty), and with want_sighash also the (n, 32) sighashes (zeros where -1)."""
+        lens = np.array([len(s) for s in streams], dtype=np.uint32)
+        offs = np.zeros(len(streams), dtype=np.uint64)
+        if len(streams) > 1:
+            offs[1:] = np.cumsum(lens[:-1], dtype=np.uint64)
+        blob = np.frombuffer(b"".join(bytes(s) for s in streams), dtype=np.uint8)
+        return self.verify_bolt12_spans(messagename, fieldname, blob, offs, lens, xonly, sig, want_sighash)
+
+    def verify_bolt12_spans(self, messagename, fieldname, blob, off, length, xonly, sig, want_sighash=False):
+        """verify_bolt12 with the streams already laid out: stream i = blob[off[i]:off[i]+length[i]]."""
+        blob = np.ascontiguousarray(blob, dtype=np.uint8).reshape(-1)
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        length = np.ascontiguousarray(length, dtype=np.uint32)
+        xonly, sig = _u8(xonly, 32), _u8(sig, 64)
+        n = off.shape[0]
+        if length.shape[0] != n or xonly.shape[0] != n or sig.shape[0] != n:
+            raise ValueError("length mismatch")
+        status =np.zeros(max(n, 1), dtype=np.int32)
+        sh = np.zeros((max(n, 1), 32), dtype=np.uint8)
+        mn = messagename.encode() if isinstance(messagename, str) else bytes(messagename)
+        fn = fieldname.encode() if isinstance(fieldname, str) else bytes(fieldname)
+        self._check(self.lib.sv_verify_bolt12_host(self._ctx, mn, fn, blob.ctypes.data, blob.size, off.ctypes.data,
+                                                   length.ctypes.data, xonly.ctypes.data, sig.ctypes.data, n,
+                                                   status.ctypes.data, sh.ctypes.data if want_sighash else None),
+                    "sv_verify_bolt12_host")
+        return (status[:n], sh[:n]) if want_sighash else status[:n]
+
+    def last_bolt12_timing(self):
+        """(merkle_ms, verify_ms) device time of the last verify_bolt12 call; needs set_profiling(True)."""
+        a, b = ctypes.c_float(), ctypes.c_float()
+        self._check(self.lib.sv_get_last_bolt12_timing(self._ctx, ctypes.byref(a), ctypes.byref(b)), "sv_get_last_bolt12_timing")
+        return a.value, b.value
 
     def sha256_double(self, data, off, length):
         data = np.ascontiguousarray(data, dtype=np.uint8).reshape(-1)
