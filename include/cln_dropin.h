@@ -114,6 +114,24 @@ struct tlv_field {                         /* wire/tlvstream.h:16-27 */
 void cln_sigverify_init(int device);
 void cln_sigverify_shutdown(void);
 
+/* CLIENT MODE: share one GPU process (the verifier subdaemon cln_sigverifyd) instead of opening an engine context here.
+ * It is on when $CLN_SIGVERIFYD_SOCKET names the daemon's unix socket (connected on the first check; a failed connect
+ * aborts), or after one of these calls succeeds (0; -1 and errno when the socket cannot be reached):
+ *   cln_sigverify_connect(path)   connect to the daemon's socket
+ *   cln_sigverify_connect_fd(fd)  use an already-connected socket, e.g. a socketpair end inherited from the parent, the way
+ *                                 lightningd hands fds to its subdaemons (the daemon side: cln_sigverifyd --fd N)
+ * In client mode these functions send one request over one blocking connection per process and wait for the reply;
+ * they never create a context:
+ *   check_signed_hash, check_signed_hash_nodeid, check_schnorr_sig, check_tx_sigs_batch   (sigverifyd_verify)
+ *   bolt12_check_signature                                                              (sigverifyd_bolt12)
+ *   sigcheck_channel_announcement_batch / _node_announcement_batch / _channel_update_batch (sigverifyd_gossip)
+ * The daemon verifies the requests of all its clients together.  A lost daemon, a short read, an error reply or a reply
+ * to another request abort() (an internal error, never a bad signature).  check_tx_sig, check_tx_sigs_bip143_batch,
+ * sha256_double and pubkey_from_der have no subdaemon message: they keep using an in-process context, created on their
+ * first use.  Without the variable and the calls, nothing changes. */
+int cln_sigverify_connect(const char *socket_path);
+int cln_sigverify_connect_fd(int fd);
+
 bool check_signed_hash(const struct sha256_double *hash, const secp256k1_ecdsa_signature *signature,
                        const struct pubkey *key);
 bool check_signed_hash_nodeid(const struct sha256_double *hash, const secp256k1_ecdsa_signature *signature,

@@ -22,6 +22,8 @@
  *                                           check_schnorr_sig(); callers plugins/offers_invreq_hook.c:634-637,
  *                                           plugins/offers_inv_hook.c:177-179, plugins/fetchinvoice.c:256-260,
  *                                           :1501-1507, lightningd/offer.c:88-89, devtools/bolt12-cli.c:319-321
+ *   sv_verify_bolt12_tagged_host(...)       the same checks, many callers' tags in one batch (the verifier
+ *                                           subdaemon serves the plugins' bolt12_check_signature calls with it)
  *   sv_sha256d_host(...)                    sha256_double()              bitcoin/shadouble.c:7-11
  *   sv_pubkey_parse_host(...)               pubkey_from_der()            bitcoin/pubkey.c:14-24
  *   sv_enqueue_* / sv_flush                 the deferral queue a batching caller (gossipd ingest,
@@ -198,6 +200,15 @@ int sv_verify_tx_host(sv_ctx *ctx, int kind, const sv_tx *txs, const uint8_t *sc
 int sv_verify_bolt12_host(sv_ctx *ctx, const char *messagename, const char *fieldname, const uint8_t *blob,
                           size_t blob_len, const uint64_t *off, const uint32_t *len, const uint8_t *xonly32,
                           const uint8_t *sig64, size_t n, int *status, uint8_t *sighash32_out);
+/* ---- the same for streams signed under DIFFERENT tags, in one pass (one launch sequence): stream i is hashed with the
+ *      tag "lightning" || messagenames[tag_of[i]] || fieldnames[tag_of[i]].  Callers that collect checks of several kinds
+ *      (the verifier subdaemon: invoice and invoice_request signatures of many clients) verify them together.  status and
+ *      sighash32_out as for sv_verify_bolt12_host.  No bound on ntags or on the length of a name.  SV_ERR_ARG also when
+ *      ntags == 0 with n > 0, a tag_of[i] >= ntags, or a NULL name. ---- */
+int sv_verify_bolt12_tagged_host(sv_ctx *ctx, size_t ntags, const char *const *messagenames, const char *const *fieldnames,
+                                 const uint32_t *tag_of, const uint8_t *blob, size_t blob_len, const uint64_t *off,
+                                 const uint32_t *len, const uint8_t *xonly32, const uint8_t *sig64, size_t n,
+                                 int *status, uint8_t *sighash32_out);
 
 /* ---- DEVICE buffers (same SoA layout, device pointers); asynchronous on `stream`
  *      (a cudaStream_t passed as void*; NULL = the context's own stream).  d_verdicts[n] bytes;

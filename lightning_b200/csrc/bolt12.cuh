@@ -27,7 +27,7 @@ struct b12_field {
 struct b12_tags {
     u32 leaf[8];     // "LnLeaf"
     u32 branch[8];   // "LnBranch"
-    u32 sighash[8];  // "lightning" || messagename || fieldname
+    u32 sighash[8];  // "lightning" || messagename || fieldname (one tag; the kernels keep a table of these, one per tag)
 };
 
 // bigsize_get (common/bigsize.c): bytes consumed, 0 if truncated or not minimally encoded
@@ -116,12 +116,17 @@ SV_HD void b12_tag_mid(u32 mid[8], const u8* pre, u32 prelen, const u8* p, u64 l
     sha256_compress(mid, blk);
 }
 
-// the batch's three tag midstates; sigtag = "lightning" || messagename || fieldname (bip340_sighash_init)
-SV_HD void b12_make_tags(b12_tags* t, const u8* sigtag, u32 sigtag_len) {
+// the two tree midstates, the same for every sighash tag
+SV_HD void b12_make_tree_tags(b12_tags* t) {
     const u8 leaf[6] = {'L', 'n', 'L', 'e', 'a', 'f'};
     const u8 branch[8] = {'L', 'n', 'B', 'r', 'a', 'n', 'c', 'h'};
     b12_tag_mid(t->leaf, leaf, 6, leaf, 0);
     b12_tag_mid(t->branch, branch, 8, branch, 0);
+}
+
+// the batch's three tag midstates; sigtag = "lightning" || messagename || fieldname (bip340_sighash_init)
+SV_HD void b12_make_tags(b12_tags* t, const u8* sigtag, u32 sigtag_len) {
+    b12_make_tree_tags(t);
     b12_tag_mid(t->sighash, sigtag, sigtag_len, sigtag, 0);
 }
 
@@ -164,10 +169,10 @@ SV_HD void b12_leaf_pair(u32 out[8], const b12_tags* t, const u32 nonce_mid[8], 
     b12_branch(out, t->branch, leaf, nonce);
 }
 
-// sighash_from_merkle: H(sighash tag, root), big-endian bytes out
-SV_HD void b12_sighash(u8 out32[32], const b12_tags* t, const u32 root[8]) {
+// sighash_from_merkle: H(sighash tag, root) from the tag's midstate, big-endian bytes out
+SV_HD void b12_sighash_mid(u8 out32[32], const u32 mid[8], const u32 root[8]) {
     u32 st[8], blk[16];
-    for (int i = 0; i < 8; i++) { st[i] = t->sighash[i]; blk[i] = root[i]; }
+    for (int i = 0; i < 8; i++) { st[i] = mid[i]; blk[i] = root[i]; }
     blk[8] = 0x80000000u;
     for (int i = 9; i < 15; i++) blk[i] = 0;
     blk[15] = (64 + 32) * 8;
@@ -177,3 +182,4 @@ SV_HD void b12_sighash(u8 out32[32], const b12_tags* t, const u32 root[8]) {
         out32[4 * i + 2] = (u8)(st[i] >> 8); out32[4 * i + 3] = (u8)st[i];
     }
 }
+SV_HD void b12_sighash(u8 out32[32], const b12_tags* t, const u32 root[8]) { b12_sighash_mid(out32, t->sighash, root); }

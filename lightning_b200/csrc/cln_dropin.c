@@ -2,13 +2,23 @@
  * cln_dropin.c — host side of the drop-in (plain C, as the reference's bitcoin/signature.c is).
  * It only marshals bytes: opaque libsecp256k1 structs -> wire form, wire messages -> (span, key,
  * signature) items, and calls the batch C ABI.  No arithmetic happens on the host.
+ *
+ * Client mode: with $CLN_SIGVERIFYD_SOCKET set, or after cln_sigverify_connect() / cln_sigverify_connect_fd(), the
+ * functions the verifier subdaemon has a message for send a request to it and block for the reply instead of creating an
+ * engine context of their own (see cln_dropin.h).
  */
+#define _GNU_SOURCE
 #include "../../include/cln_dropin.h"
 #include "../../include/cln_sigverify.h"
+#include "sigverifyd_wiregen.h"
 
+#include <errno.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <sys/socket.h>
+#include <sys/un.h>
+#include <unistd.h>
 
 #if !defined(__BYTE_ORDER__) || __BYTE_ORDER__ != __ORDER_LITTLE_ENDIAN__
 #error "opaque-struct conversion below assumes a little-endian 64-bit libsecp256k1 build"
@@ -20,6 +30,112 @@ static int g_device = -1;
 static void die(const char *what, int rc) {
     fprintf(stderr, "cln_sigverify: %s failed (%d): %s\n", what, rc, sv_last_error(g_ctx));
     abort(); /* internal error is fatal (CLN convention); never reported as "bad signature" */
+}
+
+/* ---- client mode: one blocking connection to cln_sigverifyd per process ---- */
+static int g_sock = -1;
+static int g_env_done;
+static uint64_t g_req_id;
+
+static void die_daemon(const char *what) {
+    fprintf(stderr, "cln_sigverify: verifier subdaemon: %s\n", what);
+    abort(); /* a lost daemon is an internal error too: never reported as "bad signature" */
+}
+
+int cln_sigverify_connect(const char *socket_path) {
+    struct sockaddr_un addr;
+    if (!socket_path || strlen(socket_path) >= sizeof addr.sun_path) return -1;
+    int fd = socket(AF_UNIX, SOCK_STREAM | SOCK_CLOEXEC, 0);
+    if (fd < 0) return -1;
+    memset(&addr, 0, sizeof addr);
+    addr.sun_family = AF_UNIX;
+    memcpy(addr.sun_path, socket_path, strlen(socket_path));
+    if (connect(fd, (struct sockaddr *)&addr, sizeof addr) < 0) {
+        close(fd);
+        return -1;
+    }
+    return cln_sigverify_connect_fd(fd);
+}
+
+int cln_sigverify_connect_fd(int fd) {
+    if (fd < 0) return -1;
+    if (g_sock >= 0) close(g_sock);
+    g_sock = fd;
+    g_env_done = 1;
+    return 0;
+}
+
+/* true when the checks go to the subdaemon; the first call looks at $CLN_SIGVERIFYD_SOCKET */
+static bool client(void) {
+    if (!g_env_done) {
+        g_env_done = 1;
+        const char *path = getenv("CLN_SIGVERIFYD_SOCKET");
+        if (path && *path && cln_sigverify_connect(path) < 0) {
+            fprintf(stderr, "cln_sigverify: cannot connect to %s: %s\n", path, strerror(errno));
+            abort();
+        }
+    }
+    return g_sock >= 0;
+}
+
+static void send_all(const u8 *p, size_t n) {
+    while (n) {
+        ssize_t w = send(g_sock, p, n, MSG_NOSIGNAL);
+        if (w < 0 && errno == EINTR) continue;
+        if (w <= 0) die_daemon("write failed");
+        p += w;
+        n -= (size_t)w;
+    }
+}
+static void recv_all(u8 *p, size_t n) {
+    while (n) {
+        ssize_t r = read(g_sock, p, n);
+        if (r < 0 && errno == EINTR) continue;
+        if (r <= 0) die_daemon(r == 0 ? "connection closed" : "read failed");
+        p += r;
+        n -= (size_t)r;
+    }
+}
+
+/* frame[4..4+len) holds a request (CLN framing: the be32 length goes in frame[0..4)); returns the reply message, which
+ * the caller frees.  A sigverifyd_error reply, or a reply to another request, is fatal. */
+static u8 *roundtrip(u8 *frame, size_t len, uint64_t req_id, size_t *reply_len) {
+    wire_put(frame, len, 4);
+    send_all(frame, 4 + len);
+    u8 hdr[4];
+    recv_all(hdr, 4);
+    size_t rl = wire_be32(hdr);
+    u8 *r = (u8 *)malloc(rl ? rl : 1);
+    if (!r) die("malloc", -3);
+    recv_all(r, rl);
+    struct sigverifyd_error e;
+    if (fromwire_sigverifyd_error(r, rl, &e)) {
+        fprintf(stderr, "cln_sigverify: verifier subdaemon refused request %llu (code %u)\n", (unsigned long long)e.req_id, e.code);
+        abort();
+    }
+    if (rl < 10 || wire_be(r + 2, 8) != req_id) die_daemon("reply to another request");
+    *reply_len = rl;
+    return r;
+}
+
+/* n verifications of one kind through sigverifyd_verify; verdicts[n] 0/1 */
+static void remote_verify(int kind, const u8 *msg32, const u8 *key, const u8 *sig64, size_t n, u8 *verdicts) {
+    const size_t ks = sv_key_size(kind), chunk = 1u << 16; /* well inside the daemon's frame limit */
+    for (size_t s = 0; s < n; s += chunk) {
+        uint32_t m = (uint32_t)(n - s < chunk ? n - s : chunk);
+        size_t len = 2 + 8 + 1 + 4 + 32 * (size_t)m + 4 + ks * m + 64 * (size_t)m, rl;
+        u8 *f = (u8 *)malloc(4 + len);
+        if (!f) die("malloc", -3);
+        uint64_t id = ++g_req_id;
+        towire_sigverifyd_verify(f + 4, len, id, (uint8_t)kind, m, msg32 + 32 * s, (uint32_t)(ks * m), key + ks * s,
+                                 sig64 + 64 * s);
+        u8 *r = roundtrip(f, len, id, &rl);
+        struct sigverifyd_verify_reply v;
+        if (!fromwire_sigverifyd_verify_reply(r, rl, &v) || v.n != m) die_daemon("malformed verify reply");
+        memcpy(verdicts + s, v.verdicts, m);
+        free(r);
+        free(f);
+    }
 }
 
 static sv_ctx *ctx(void) {
@@ -45,6 +161,8 @@ void cln_sigverify_init(int device) {
 void cln_sigverify_shutdown(void) {
     if (g_ctx) sv_destroy(g_ctx);
     g_ctx = NULL;
+    if (g_sock >= 0) close(g_sock);
+    g_sock = -1;
 }
 
 /* libsecp256k1's opaque structs hold r,s / x,y as 4x64-bit little-endian limbs on 64-bit little-endian
@@ -68,6 +186,10 @@ bool check_signed_hash(const struct sha256_double *hash, const secp256k1_ecdsa_s
     u8 sig[64], xy[64], v = 0;
     sig_to_wire(sig, signature);
     pubkey_to_xy(xy, &key->pubkey);
+    if (client()) {
+        remote_verify(SV_KIND_ECDSA_XY, hash->sha.u.u8, xy, sig, 1, &v);
+        return v == 1;
+    }
     int rc = sv_verify_host(ctx(), SV_KIND_ECDSA_XY, hash->sha.u.u8, xy, sig, 1, &v);
     if (rc != SV_OK) die("sv_verify_host", rc);
     return v == 1;
@@ -77,6 +199,10 @@ bool check_signed_hash_nodeid(const struct sha256_double *hash, const secp256k1_
                               const struct node_id *id) {
     u8 sig[64], v = 0;
     sig_to_wire(sig, signature);
+    if (client()) {
+        remote_verify(SV_KIND_ECDSA33, hash->sha.u.u8, id->k, sig, 1, &v);
+        return v == 1;
+    }
     int rc = sv_verify_host(ctx(), SV_KIND_ECDSA33, hash->sha.u.u8, id->k, sig, 1, &v);
     if (rc != SV_OK) die("sv_verify_host", rc);
     return v == 1;
@@ -86,6 +212,10 @@ bool check_schnorr_sig(const struct sha256 *hash, const secp256k1_pubkey *pubkey
     /* signature.c:412-423: serialize compressed, drop the parity byte -> x-only key */
     u8 xy[64], v = 0;
     pubkey_to_xy(xy, pubkey);
+    if (client()) {
+        remote_verify(SV_KIND_SCHNORR, hash->u.u8, xy, sig->u8, 1, &v);
+        return v == 1;
+    }
     int rc = sv_verify_host(ctx(), SV_KIND_SCHNORR, hash->u.u8, xy, sig->u8, 1, &v);
     if (rc != SV_OK) die("sv_verify_host", rc);
     return v == 1;
@@ -224,6 +354,28 @@ static size_t put_bigsize(u8 *p, uint64_t v) { /* common/bigsize.c bigsize_put *
     return n;
 }
 
+/* one stream through sigverifyd_bolt12: its status (1, 0 or -1) */
+static int remote_bolt12(const char *messagename, const char *fieldname, const u8 *stream, size_t len, const u8 *xonly32,
+                         const u8 *sig64) {
+    size_t mnl = strlen(messagename), fnl = strlen(fieldname);
+    if (mnl > 0xffff || fnl > 0xffff || len > 0xffffffffu) die("bolt12_check_signature: tag or stream too long", -4);
+    size_t mlen = 2 + 8 + 2 + mnl + 2 + fnl + 4 + 4 + 4 + len + 32 + 64 + 1, rl;
+    u8 *f = (u8 *)malloc(4 + mlen);
+    if (!f) die("malloc", -3);
+    u8 len_be[4];
+    wire_put(len_be, len, 4);
+    uint64_t id = ++g_req_id;
+    towire_sigverifyd_bolt12(f + 4, mlen, id, (uint16_t)mnl, (const u8 *)messagename, (uint16_t)fnl, (const u8 *)fieldname, 1,
+                             len_be, (uint32_t)len, stream, xonly32, sig64, 0);
+    u8 *r = roundtrip(f, mlen, id, &rl);
+    struct sigverifyd_bolt12_reply b;
+    if (!fromwire_sigverifyd_bolt12_reply(r, rl, &b) || b.n != 1) die_daemon("malformed bolt12 reply");
+    int st = b.status[0] == 255 ? -1 : b.status[0];
+    free(r);
+    free(f);
+    return st;
+}
+
 bool bolt12_check_signature(const struct tlv_field *fields, const char *messagename, const char *fieldname,
                             const struct pubkey *key, const struct bip340sig *sig) {
     size_t bytes;
@@ -247,6 +399,11 @@ bool bolt12_check_signature(const struct tlv_field *fields, const char *messagen
     u8 xy[64];
     int status = 0;
     pubkey_to_xy(xy, &key->pubkey); /* x-only: the first 32 bytes */
+    if (client()) {
+        status = remote_bolt12(messagename, fieldname, blob, n, xy, sig->u8);
+        free(blob);
+        return status == 1;
+    }
     int rc = sv_verify_bolt12_host(ctx(), messagename, fieldname, blob, n, &off, &len, xy, sig->u8, 1, &status, NULL);
     free(blob);
     if (rc != SV_OK) die("sv_verify_bolt12_host", rc);
@@ -265,9 +422,17 @@ void check_tx_sigs_batch(const struct sha256_double *hashes, const struct bitcoi
         memcpy(msg + 32 * i, hashes[i].sha.u.u8, 32);
         sig_to_wire(sig + 64 * i, &sigs[i].s);
     }
-    /* one key for the whole loop: its multiples table is built once on the device */
-    int rc = sv_verify_samekey_host(ctx(), SV_KIND_ECDSA_XY, xy, msg, sig, n, v);
-    if (rc != SV_OK) die("sv_verify_samekey_host", rc);
+    if (client()) { /* per-item keys of one kind: the daemon coalesces them with every other client's */
+        u8 *keys = (u8 *)malloc(64 * n);
+        if (!keys) die("malloc", -3);
+        for (size_t i = 0; i < n; i++) memcpy(keys + 64 * i, xy, 64);
+        remote_verify(SV_KIND_ECDSA_XY, msg, keys, sig, n, v);
+        free(keys);
+    } else {
+        /* one key for the whole loop: its multiples table is built once on the device */
+        int rc = sv_verify_samekey_host(ctx(), SV_KIND_ECDSA_XY, xy, msg, sig, n, v);
+        if (rc != SV_OK) die("sv_verify_samekey_host", rc);
+    }
     for (size_t i = 0; i < n; i++) ok[i] = v[i] == 1;
     free(buf);
 }
@@ -297,6 +462,29 @@ void check_tx_sigs_bip143_batch(const void *sv_tx_array, const u8 *scripts, size
     free(buf);
 }
 
+/* gossip messages through sigverifyd_gossip, in requests of at most 65536 messages and 64 MiB; status 255 -> -1 */
+static void remote_gossip(const u8 *blob, const uint32_t *len, size_t n, const u8 *cu_signers33, int *status) {
+    size_t s = 0, bo = 0;
+    while (s < n) {
+        size_t m = 0, bytes = 0;
+        while (s + m < n && m < 65536 && (m == 0 || bytes + len[s + m] <= (64u << 20))) bytes += len[s + m++];
+        size_t mlen = 2 + 8 + 4 + 4 * m + 33 * m + 4 + bytes, rl;
+        u8 *f = (u8 *)malloc(4 + mlen), *lens = (u8 *)malloc(4 * m), *sg = (u8 *)calloc(m ? m : 1, 33);
+        if (!f || !lens || !sg) die("malloc", -3);
+        for (size_t i = 0; i < m; i++) wire_put(lens + 4 * i, len[s + i], 4);
+        if (cu_signers33) memcpy(sg, cu_signers33 + 33 * s, 33 * m);
+        uint64_t id = ++g_req_id;
+        towire_sigverifyd_gossip(f + 4, mlen, id, (uint32_t)m, lens, sg, (uint32_t)bytes, blob + bo);
+        u8 *r = roundtrip(f, mlen, id, &rl);
+        struct sigverifyd_gossip_reply g;
+        if (!fromwire_sigverifyd_gossip_reply(r, rl, &g) || g.n != m) die_daemon("malformed gossip reply");
+        for (size_t i = 0; i < m; i++) status[s + i] = g.status[i] == 255 ? -1 : g.status[i];
+        free(r); free(f); free(lens); free(sg);
+        s += m;
+        bo += bytes;
+    }
+}
+
 /* ---- gossip: the raw wire messages go to the device as one blob; the DEVICE slices them the way
  * gossipd/sigcheck.c does (k_gossip_slice), hashes the signed regions and verifies (sv_verify_gossip_host) ---- */
 static void gossip_batch(const u8 *const *msgs, const size_t *lens, size_t n, const struct node_id *signers,
@@ -315,8 +503,12 @@ static void gossip_batch(const u8 *const *msgs, const size_t *lens, size_t n, co
         memcpy(blob + t, msgs[i], lens[i]);
         t += lens[i];
     }
-    int rc = sv_verify_gossip_host(ctx(), blob, total, off, len, n, signers ? signers[0].k : NULL, status);
-    if (rc != SV_OK) die("sv_verify_gossip_host", rc);
+    if (client()) {
+        remote_gossip(blob, len, n, signers ? signers[0].k : NULL, status);
+    } else {
+        int rc = sv_verify_gossip_host(ctx(), blob, total, off, len, n, signers ? signers[0].k : NULL, status);
+        if (rc != SV_OK) die("sv_verify_gossip_host", rc);
+    }
     for (size_t i = 0; i < n; i++) /* this entry point is typed: a message of another kind is malformed here */
         if (lens[i] < 2 || (uint16_t)((msgs[i][0] << 8) | msgs[i][1]) != want_type) status[i] = -1;
     free(blob); free(off); free(len);

@@ -560,16 +560,23 @@ __global__ void __launch_bounds__(SV_B12_SCAN) k_b12_scan_add(u64* base, size_t 
     size_t i = (size_t)blockIdx.x * SV_B12_SCAN + threadIdx.x;
     if (i < n) base[i] += sums[blockIdx.x];
 }
-__global__ void k_b12_tags(const u8* sigtag, u32 sigtag_len, b12_tags* tags) {
-    if (blockIdx.x == 0 && threadIdx.x == 0) b12_make_tags(tags, sigtag, sigtag_len);
+// k_b12_tags: thread t < ntags computes the sighash midstate of tag t (tag bytes tagbytes[tagoff[t] .. +taglen[t])), thread
+// ntags the leaf and branch midstates every tag shares
+__global__ void k_b12_tags(const u8* tagbytes, const u64* tagoff, const u32* taglen, size_t ntags, b12_tags* tags,
+                           u32* sigmid) {
+    const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < ntags) b12_tag_mid(sigmid + 8 * t, tagbytes + tagoff[t], taglen[t], tagbytes, 0);
+    else if (t == ntags) b12_make_tree_tags(tags);
 }
 // k_b12_merkle: one warp per stream.  Lane 0 walks the headers into the field records; the lanes hash one field each
 // (leaf, nonce, leaf pair; strided past 32 fields); signature-range fields drop out by ballot / popc compaction; then the
 // tree is reduced one level per step (neighbours paired, an odd last node carried up: merkle_tlv's power-of-two split);
-// lane 0 hashes the root into the sighash.  Failed parses get a zero sighash (they are never verified as signed).
+// lane 0 hashes the root into the sighash under the stream's tag (sigmid[tag_of[i]]; tag_of NULL: tag 0).  Failed parses
+// get a zero sighash (they are never verified as signed).
 #define SV_B12_WARPS 4
 __global__ void __launch_bounds__(32 * SV_B12_WARPS) k_b12_merkle(const u8* blob, const u64* off, const u32* len, size_t n,
                                                                   const u32* cnt, const u64* fbase, const b12_tags* tags,
+                                                                  const u32* sigmid, const u32* tag_of,
                                                                   b12_field* recs, u32* nodes, u8* msg32) {
     const size_t i = (size_t)blockIdx.x * SV_B12_WARPS + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
@@ -599,7 +606,7 @@ __global__ void __launch_bounds__(32 * SV_B12_WARPS) k_b12_merkle(const u8* blob
 #pragma unroll
     for (int k = 0; k < 8; k++) nm[k] = __shfl_sync(0xFFFFFFFFu, nm[k], 0);
     b12_tags& t = s_tags[threadIdx.x >> 5];
-    if (lane < 24) reinterpret_cast<u32*>(&t)[lane] = reinterpret_cast<const u32*>(tags)[lane];
+    if (lane < 16) reinterpret_cast<u32*>(&t)[lane] = reinterpret_cast<const u32*>(tags)[lane];  // leaf, branch
     __syncwarp();
     u32 m = 0;  // non-signature fields so far
     for (u32 j0 = 0; j0 < F; j0 += 32) {
@@ -644,7 +651,7 @@ __global__ void __launch_bounds__(32 * SV_B12_WARPS) k_b12_merkle(const u8* blob
         u32 root[8];
 #pragma unroll
         for (int q = 0; q < 8; q++) root[q] = m ? node[q] : 0u;  // no non-signature field: merkle_tlv's all-zero root
-        b12_sighash(msg32 + 32 * i, &t, root);
+        b12_sighash_mid(msg32 + 32 * i, sigmid + 8 * (size_t)(tag_of ? tag_of[i] : 0u), root);
     }
 }
 // status[i] = verdict where the stream parsed, -1 where it did not
@@ -1949,25 +1956,41 @@ extern "C" int sv_verify_mixed_host(sv_ctx* ctx, const uint8_t* kinds, const uin
 // The host copies bytes only.  The device parses every stream, builds its Merkle root and sighash (k_b12_*), verifies the
 // sighashes through the ordinary BIP-340 path (launch_verify) and folds parse status and verdict into one int.  One host
 // synchronisation in the middle: the total field count sizes the record / node scratch.
-extern "C" int sv_verify_bolt12_host(sv_ctx* ctx, const char* messagename, const char* fieldname, const uint8_t* blob,
-                                     size_t blob_len, const uint64_t* off, const uint32_t* len, const uint8_t* xonly32,
-                                     const uint8_t* sig64, size_t n, int* status, uint8_t* sighash32_out) {
-    if (!ctx || !messagename || !fieldname || (n && (!blob || !off || !len || !xonly32 || !sig64 || !status))) return SV_ERR_ARG;
-    if (n == 0) return SV_OK;
+//
+// One pass over n streams under ntags sighash tags: tag t is "lightning" || messagenames[t] || fieldnames[t]
+// (bip340_sighash_init(sctx, "lightning", messagename, fieldname): the three strings back to back), stream i is hashed
+// under tag tag_of[i] (tag_of NULL: every stream under tag 0).  The arguments are checked by the callers.
+static int bolt12_pass(sv_ctx* ctx, size_t ntags, const char* const* messagenames, const char* const* fieldnames,
+                       const uint32_t* tag_of, const uint8_t* blob, size_t blob_len, const uint64_t* off, const uint32_t* len,
+                       const uint8_t* xonly32, const uint8_t* sig64, size_t n, int* status, uint8_t* sighash32_out) {
     dev_guard dg__;
     CK(dg__.enter(ctx->device));
     int rc = ensure_staging(ctx, n);
     if (rc) return rc;
     rc = stage_spans(ctx, blob, blob_len, off, len, n);
     if (rc) return rc;
-    // bip340_sighash_init(sctx, "lightning", messagename, fieldname): the tag is the three strings back to back
-    std::string tag = std::string("lightning") + messagename + fieldname;
-    if (tag.size() > 0xFFFFFFFFu) return fail(ctx, SV_ERR_ARG, "tag too long", cudaSuccess);
-    const size_t nb = (n + SV_B12_SCAN - 1) / SV_B12_SCAN;
-    // per-call scratch in the auxiliary slab: [cnt u32 n][base u64 n][block sums u64 nb+1][status int n][tags][tag bytes]
     auto up16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
+    // the tag table travels in one copy: [tag offsets u64 ntags][tag lengths u32 ntags][tag_of u32 n][tag bytes]
+    const size_t t_len = up16(8 * ntags), t_of = t_len + up16(4 * ntags), t_bytes = t_of + (tag_of ? up16(4 * n) : 0);
+    std::vector<u8> tab(t_bytes);
+    for (size_t t = 0; t < ntags; t++) {
+        const u64 o = tab.size() - t_bytes;
+        const size_t a = strlen(messagenames[t]), b = strlen(fieldnames[t]);
+        if (9 + a + b > 0xFFFFFFFFu) return fail(ctx, SV_ERR_ARG, "tag too long", cudaSuccess);
+        const u32 l = (u32)(9 + a + b);
+        memcpy(tab.data() + 8 * t, &o, 8);
+        memcpy(tab.data() + t_len + 4 * t, &l, 4);
+        tab.insert(tab.end(), "lightning", "lightning" + 9);
+        tab.insert(tab.end(), messagenames[t], messagenames[t] + a);
+        tab.insert(tab.end(), fieldnames[t], fieldnames[t] + b);
+    }
+    if (tag_of) memcpy(tab.data() + t_of, tag_of, 4 * n);
+    const size_t nb = (n + SV_B12_SCAN - 1) / SV_B12_SCAN;
+    // per-call scratch in the auxiliary slab: [cnt u32 n][base u64 n][block sums u64 nb+1][status int n][tree tags]
+    // [sighash midstates 32 x ntags][tag table]
     const size_t o_base = up16(4 * n), o_sums = o_base + 8 * n, o_status = up16(o_sums + 8 * (nb + 1)),
-                 o_tags = up16(o_status + 4 * n), o_tag = o_tags + up16(sizeof(b12_tags)), need = o_tag + tag.size() + 64;
+                 o_tags = up16(o_status + 4 * n), o_mid = o_tags + up16(sizeof(b12_tags)), o_tab = o_mid + 32 * ntags,
+                 need = o_tab + tab.size() + 64;
     rc = ensure_gbuf(ctx, need);
     if (rc) return rc;
     u32* d_cnt = reinterpret_cast<u32*>(ctx->g_buf);
@@ -1975,13 +1998,15 @@ extern "C" int sv_verify_bolt12_host(sv_ctx* ctx, const char* messagename, const
     u64* d_sums = reinterpret_cast<u64*>(ctx->g_buf + o_sums);
     int* d_status = reinterpret_cast<int*>(ctx->g_buf + o_status);
     b12_tags* d_tags = reinterpret_cast<b12_tags*>(ctx->g_buf + o_tags);
-    u8* d_tag = ctx->g_buf + o_tag;
+    u32* d_mid = reinterpret_cast<u32*>(ctx->g_buf + o_mid);
+    u8* d_tab = ctx->g_buf + o_tab;
     cudaStream_t st = ctx->stream;
     CK(cudaMemcpyAsync(ctx->d_key, xonly32, 32 * n, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->d_sig, sig64, 64 * n, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_tag, tag.data(), tag.size(), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_tab, tab.data(), tab.size(), cudaMemcpyHostToDevice, st));
     if (ctx->profiling) cudaEventRecord(ctx->b12_ev[0], st);
-    k_b12_tags<<<1, 32, 0, st>>>(d_tag, (u32)tag.size(), d_tags);
+    k_b12_tags<<<(unsigned)((ntags + 1 + 63) / 64), 64, 0, st>>>(d_tab + t_bytes, reinterpret_cast<const u64*>(d_tab),
+                                                              reinterpret_cast<const u32*>(d_tab + t_len), ntags, d_tags, d_mid);
     k_b12_count<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(ctx->d_data, ctx->d_off, ctx->d_len, n, d_cnt);
     k_b12_scan_local<<<(unsigned)nb, SV_B12_SCAN, 0, st>>>(d_cnt, n, d_base, d_sums);
     k_b12_scan_sums<<<1, SV_B12_SCAN, 0, st>>>(d_sums, nb);
@@ -2004,7 +2029,8 @@ extern "C" int sv_verify_bolt12_host(sv_ctx* ctx, const char* messagename, const
     b12_field* d_recs = reinterpret_cast<b12_field*>(ctx->b12_buf);
     u32* d_nodes = reinterpret_cast<u32*>(ctx->b12_buf + (size_t)total * sizeof(b12_field));
     k_b12_merkle<<<(unsigned)((n + SV_B12_WARPS - 1) / SV_B12_WARPS), 32 * SV_B12_WARPS, 0, st>>>(
-        ctx->d_data, ctx->d_off, ctx->d_len, n, d_cnt, d_base, d_tags, d_recs, d_nodes, ctx->d_msg);
+        ctx->d_data, ctx->d_off, ctx->d_len, n, d_cnt, d_base, d_tags, d_mid,
+        tag_of ? reinterpret_cast<const u32*>(d_tab + t_of) : nullptr, d_recs, d_nodes, ctx->d_msg);
     ctx->launches += 1;
     if (ctx->profiling) cudaEventRecord(ctx->b12_ev[1], st);
     CK(cudaGetLastError());
@@ -2018,6 +2044,29 @@ extern "C" int sv_verify_bolt12_host(sv_ctx* ctx, const char* messagename, const
     if (sighash32_out) CK(cudaMemcpyAsync(sighash32_out, ctx->d_msg, 32 * n, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     return SV_OK;
+}
+extern "C" int sv_verify_bolt12_host(sv_ctx* ctx, const char* messagename, const char* fieldname, const uint8_t* blob,
+                                     size_t blob_len, const uint64_t* off, const uint32_t* len, const uint8_t* xonly32,
+                                     const uint8_t* sig64, size_t n, int* status, uint8_t* sighash32_out) {
+    if (!ctx || !messagename || !fieldname || (n && (!blob || !off || !len || !xonly32 || !sig64 || !status))) return SV_ERR_ARG;
+    if (n == 0) return SV_OK;
+    return bolt12_pass(ctx, 1, &messagename, &fieldname, nullptr, blob, blob_len, off, len, xonly32, sig64, n, status,
+                       sighash32_out);
+}
+// the same with a tag per stream: the whole batch is one pass (one launch sequence) whatever the number of tags
+extern "C" int sv_verify_bolt12_tagged_host(sv_ctx* ctx, size_t ntags, const char* const* messagenames,
+                                            const char* const* fieldnames, const uint32_t* tag_of, const uint8_t* blob,
+                                            size_t blob_len, const uint64_t* off, const uint32_t* len, const uint8_t* xonly32,
+                                            const uint8_t* sig64, size_t n, int* status, uint8_t* sighash32_out) {
+    if (!ctx || (ntags && (!messagenames || !fieldnames))) return SV_ERR_ARG;
+    for (size_t t = 0; t < ntags; t++)
+        if (!messagenames[t] || !fieldnames[t]) return SV_ERR_ARG;
+    if (n && (!ntags || !tag_of || !blob || !off || !len || !xonly32 || !sig64 || !status)) return SV_ERR_ARG;
+    for (size_t i = 0; i < n; i++)
+        if (tag_of[i] >= ntags) return fail(ctx, SV_ERR_ARG, "tag_of out of range", cudaSuccess);
+    if (n == 0) return SV_OK;
+    return bolt12_pass(ctx, ntags, messagenames, fieldnames, tag_of, blob, blob_len, off, len, xonly32, sig64, n, status,
+                       sighash32_out);
 }
 
 // ---- BIP-340 batch verification, host entry (batch.cuh) --------------------------------------------------------------

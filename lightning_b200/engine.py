@@ -62,6 +62,7 @@ def load_library():
     lib.sv_verify_tx_host.argtypes = [vp, i, vp, vp, sz, vp, vp, sz, vp, vp]
     lib.sv_verify_samekey_host.argtypes = [vp, i, vp, vp, vp, sz, vp]
     lib.sv_verify_bolt12_host.argtypes = [vp, ctypes.c_char_p, ctypes.c_char_p, vp, sz, vp, vp, vp, vp, sz, vp, vp]
+    lib.sv_verify_bolt12_tagged_host.argtypes = [vp, sz, vp, vp, vp, vp, sz, vp, vp, vp, vp, sz, vp, vp]
     lib.sv_get_last_bolt12_timing.argtypes = [vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float)]
     lib.sv_sync.argtypes = [vp, vp]
     lib.sv_get_stream.argtypes = [vp]
@@ -244,6 +245,29 @@ class SigVerifier:
                                                    length.ctypes.data, xonly.ctypes.data, sig.ctypes.data, n,
                                                    status.ctypes.data, sh.ctypes.data if want_sighash else None),
                     "sv_verify_bolt12_host")
+        return (status[:n], sh[:n]) if want_sighash else status[:n]
+
+    def verify_bolt12_tagged(self, tags, tag_of, blob, off, length, xonly, sig, want_sighash=False):
+        """verify_bolt12_spans with a tag per stream, in one pass: tags is a sequence of (messagename, fieldname) pairs,
+        stream i is hashed under tags[tag_of[i]]."""
+        blob = np.ascontiguousarray(blob, dtype=np.uint8).reshape(-1)
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        length = np.ascontiguousarray(length, dtype=np.uint32)
+        tag_of = np.ascontiguousarray(tag_of, dtype=np.uint32)
+        xonly, sig = _u8(xonly, 32), _u8(sig, 64)
+        n = off.shape[0]
+        if length.shape[0] != n or tag_of.shape[0] != n or xonly.shape[0] != n or sig.shape[0] != n:
+            raise ValueError("length mismatch")
+        enc = [(s.encode() if isinstance(s, str) else bytes(s)) for pair in tags for s in pair]  # alive through the call
+        mn = (ctypes.c_char_p * max(len(tags), 1))(*enc[0::2])
+        fn = (ctypes.c_char_p * max(len(tags), 1))(*enc[1::2])
+        status = np.zeros(max(n, 1), dtype=np.int32)
+        sh = np.zeros((max(n, 1), 32), dtype=np.uint8)
+        self._check(self.lib.sv_verify_bolt12_tagged_host(self._ctx, len(tags), mn, fn, tag_of.ctypes.data, blob.ctypes.data,
+                                                          blob.size, off.ctypes.data, length.ctypes.data, xonly.ctypes.data,
+                                                          sig.ctypes.data, n, status.ctypes.data,
+                                                          sh.ctypes.data if want_sighash else None),
+                    "sv_verify_bolt12_tagged_host")
         return (status[:n], sh[:n]) if want_sighash else status[:n]
 
     def last_bolt12_timing(self):
