@@ -268,6 +268,82 @@ static size_t put_output(u8 *p, const struct wally_tx_output *o) {
     return n + o->script_len;
 }
 
+#define DAEMON_MAX_FRAME (32u + (1u << 20) * 161u) /* the largest message cln_sigverifyd reads (MAX_FRAME of sigverifyd.c) */
+
+/* the bytes of t's spans sv_verify_tx_host reads: witness script, outputs and, for a multi-input transaction, outpoints
+ * and sequences; a span outside scripts[0 .. scripts_len) aborts, as the in-process call's SV_ERR_ARG does */
+static uint64_t tx_span_bytes(const sv_tx *t, size_t scripts_len) {
+    const bool in = (t->flags & SV_TX_INPUTS_SERIALIZED) != 0;
+    if ((uint64_t)t->script_off + t->script_len > scripts_len || (uint64_t)t->out_script_off + t->out_script_len > scripts_len ||
+        (in && ((uint64_t)t->prevouts_off + t->prevouts_len > scripts_len ||
+                (uint64_t)t->sequences_off + t->sequences_len > scripts_len)))
+        die("sv_tx: script span out of range", SV_ERR_ARG);
+    return (uint64_t)t->script_len + t->out_script_len + (in ? (uint64_t)t->prevouts_len + t->sequences_len : 0);
+}
+
+/* n transaction checks by one key through sigverifyd_tx, in requests of at most 65536 transactions and 64 MiB of spans
+ * (a single larger transaction goes alone, and aborts if it does not fit in a frame); verdicts[n] as sv_verify_tx_host
+ * gives them.  Each transaction's spans are copied out of scripts back to back: the daemon derives the offsets. */
+static void remote_tx(int kind, const u8 *key, const sv_tx *txs, const u8 *scripts, size_t scripts_len, const u8 *sig64,
+                      size_t n, u8 *verdicts) {
+    const size_t ks = sv_key_size(kind), per_tx = 6 * 4 + 32 + 2 * 8 + 4 * 4 + 64;
+    size_t s = 0;
+    while (s < n) {
+        size_t m = 0;
+        uint64_t bytes = 0;
+        while (s + m < n && m < 65536) {
+            uint64_t b = tx_span_bytes(&txs[s + m], scripts_len);
+            if (m && bytes + b > (64u << 20)) break;
+            bytes += b;
+            m++;
+        }
+        uint64_t mlen64 = 2 + 8 + 1 + 4 + ks + 4 + per_tx * m + 4 + bytes + 1;
+        if (mlen64 > DAEMON_MAX_FRAME) die_daemon("transaction too large for one request");
+        size_t mlen = (size_t)mlen64, rl;
+        u8 *f = (u8 *)malloc(4 + mlen), *a = (u8 *)malloc((6 * 4 + 32 + 2 * 8 + 4 * 4) * m + bytes + 1);
+        if (!f || !a) die("malloc", -3);
+        u8 *ver = a, *lock = ver + 4 * m, *seq = lock + 4 * m, *sht = seq + 4 * m, *pidx = sht + 4 * m, *flg = pidx + 4 * m;
+        u8 *txid = flg + 4 * m, *iamt = txid + 32 * m, *oamt = iamt + 8 * m, *sl = oamt + 8 * m, *ol = sl + 4 * m;
+        u8 *pl = ol + 4 * m, *ql = pl + 4 * m, *blob = ql + 4 * m;
+        size_t bo = 0;
+        for (size_t i = 0; i < m; i++) {
+            const sv_tx *t = &txs[s + i];
+            const bool in = (t->flags & SV_TX_INPUTS_SERIALIZED) != 0;
+            const uint32_t plen = in ? t->prevouts_len : 0, qlen = in ? t->sequences_len : 0;
+            wire_put(ver + 4 * i, t->version, 4);
+            wire_put(lock + 4 * i, t->locktime, 4);
+            wire_put(seq + 4 * i, t->sequence, 4);
+            wire_put(sht + 4 * i, t->sighash_type, 4);
+            wire_put(pidx + 4 * i, t->prev_index, 4);
+            wire_put(flg + 4 * i, t->flags, 4);
+            memcpy(txid + 32 * i, t->prev_txid, 32);
+            wire_put(iamt + 8 * i, t->input_amount, 8);
+            wire_put(oamt + 8 * i, t->output_amount, 8);
+            wire_put(sl + 4 * i, t->script_len, 4);
+            wire_put(ol + 4 * i, t->out_script_len, 4);
+            wire_put(pl + 4 * i, plen, 4);
+            wire_put(ql + 4 * i, qlen, 4);
+            if (t->script_len) memcpy(blob + bo, scripts + t->script_off, t->script_len);
+            bo += t->script_len;
+            if (t->out_script_len) memcpy(blob + bo, scripts + t->out_script_off, t->out_script_len);
+            bo += t->out_script_len;
+            if (plen) memcpy(blob + bo, scripts + t->prevouts_off, plen);
+            bo += plen;
+            if (qlen) memcpy(blob + bo, scripts + t->sequences_off, qlen);
+            bo += qlen;
+        }
+        uint64_t id = ++g_req_id;
+        towire_sigverifyd_tx(f + 4, mlen, id, (uint8_t)kind, (uint32_t)ks, key, (uint32_t)m, ver, lock, seq, sht, pidx, flg,
+                             txid, iamt, oamt, sl, ol, pl, ql, (uint32_t)bytes, blob, sig64 + 64 * s, 0);
+        u8 *r = roundtrip(f, mlen, id, &rl);
+        struct sigverifyd_tx_reply x;
+        if (!fromwire_sigverifyd_tx_reply(r, rl, &x) || x.n != m) die_daemon("malformed tx reply");
+        memcpy(verdicts + s, x.verdicts, m);
+        free(r); free(f); free(a);
+        s += m;
+    }
+}
+
 bool check_tx_sig(const struct bitcoin_tx *tx, size_t input_num, const u8 *redeemscript, const u8 *witness_script,
                   const struct pubkey *key, const struct bitcoin_signature *sig) {
     const u8 *script = witness_script ? witness_script : redeemscript;
@@ -338,6 +414,11 @@ bool check_tx_sig(const struct bitcoin_tx *tx, size_t input_num, const u8 *redee
     u8 xy[64], s64[64], v = 0;
     pubkey_to_xy(xy, &key->pubkey);
     sig_to_wire(s64, &sig->s);
+    if (client()) {
+        remote_tx(SV_KIND_ECDSA_XY, xy, &t, blob, n, s64, 1, &v);
+        free(blob);
+        return v == 1;
+    }
     int rc = sv_verify_tx_host(ctx(), SV_KIND_ECDSA_XY, &t, blob, n, xy, s64, 1, &v, NULL);
     free(blob);
     if (rc != SV_OK) die("sv_verify_tx_host", rc);
@@ -450,8 +531,12 @@ void check_tx_sigs_bip143_batch(const void *sv_tx_array, const u8 *scripts, size
         pubkey_to_xy(xy + 64 * i, &key->pubkey);
         sig_to_wire(sig + 64 * i, &sigs[i].s);
     }
-    int rc = sv_verify_tx_host(ctx(), SV_KIND_ECDSA_XY, txs, scripts, scripts_len, xy, sig, n, v, NULL);
-    if (rc != SV_OK) die("sv_verify_tx_host", rc);
+    if (client()) { /* one key for the batch: the daemon coalesces it with every other client's transactions */
+        remote_tx(SV_KIND_ECDSA_XY, xy, txs, scripts, scripts_len, sig, n, v);
+    } else {
+        int rc = sv_verify_tx_host(ctx(), SV_KIND_ECDSA_XY, txs, scripts, scripts_len, xy, sig, n, v, NULL);
+        if (rc != SV_OK) die("sv_verify_tx_host", rc);
+    }
     for (size_t i = 0; i < n; i++) {
         /* check_tx_sig's gate (signature.c:206-211); a witness script is always present on this path */
         bool type_ok = sigs[i].sighash_type == SIGHASH_ALL ||
