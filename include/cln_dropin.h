@@ -126,12 +126,15 @@ void cln_sigverify_shutdown(void);
  *   bolt12_check_signature                                                              (sigverifyd_bolt12)
  *   check_tx_sig, check_tx_sigs_bip143_batch                                            (sigverifyd_tx)
  *   sigcheck_channel_announcement_batch / _node_announcement_batch / _channel_update_batch (sigverifyd_gossip)
+ *   sha256_double                                                                       (sigverifyd_sha256d)
+ *   pubkey_from_der                                                                     (sigverifyd_pubkey)
  * check_tx_sig gates the sighash type before it sends anything; the BIP143 sighash is built on the daemon's device.
- * check_tx_sigs_bip143_batch sends requests of at most 65536 transactions and 64 MiB of scripts each.  The daemon verifies
- * the requests of all its clients together.  A lost daemon, a short read, an error reply, a reply to another request or
- * a transaction too large for one request abort() (an internal error, never a bad signature).  sha256_double and
- * pubkey_from_der have no subdaemon message: they keep using an in-process context, created on their first use.  Without
- * the variable and the calls, nothing changes. */
+ * check_tx_sigs_bip143_batch sends requests of at most 65536 transactions and 64 MiB of scripts each.  pubkey_from_der
+ * returns false for a length other than 33 without sending anything.  The daemon serves the requests of all its clients
+ * together.  A lost daemon, a short read, an error reply, a reply to another request or a transaction or buffer too large
+ * for one request abort() (an internal error, never a bad signature).  No function of this header opens a context in
+ * client mode; cln_sigverify_init(), which creates one on purpose, is for the in-process variant.  Without the variable
+ * and the calls, nothing changes. */
 int cln_sigverify_connect(const char *socket_path);
 int cln_sigverify_connect_fd(int fd);
 

@@ -37,6 +37,8 @@ static int g_sock = -1;
 static int g_env_done;
 static uint64_t g_req_id;
 
+#define DAEMON_MAX_FRAME (32u + (1u << 20) * 161u) /* the largest message cln_sigverifyd reads (MAX_FRAME of sigverifyd.c) */
+
 static void die_daemon(const char *what) {
     fprintf(stderr, "cln_sigverify: verifier subdaemon: %s\n", what);
     abort(); /* a lost daemon is an internal error too: never reported as "bad signature" */
@@ -221,10 +223,46 @@ bool check_schnorr_sig(const struct sha256 *hash, const secp256k1_pubkey *pubkey
     return v == 1;
 }
 
+/* one buffer through sigverifyd_sha256d; a buffer too large for one frame aborts */
+static void remote_sha256d(const u8 *p, size_t len, u8 out32[32]) {
+    if (len > DAEMON_MAX_FRAME - (2 + 8 + 4 + 4 + 4)) die_daemon("buffer too large for one request");
+    size_t mlen = 2 + 8 + 4 + 4 + 4 + len, rl;
+    u8 *f = (u8 *)malloc(4 + mlen);
+    if (!f) die("malloc", -3);
+    u8 len_be[4];
+    wire_put(len_be, len, 4);
+    uint64_t id = ++g_req_id;
+    towire_sigverifyd_sha256d(f + 4, mlen, id, 1, len_be, (uint32_t)len, p);
+    u8 *r = roundtrip(f, mlen, id, &rl);
+    struct sigverifyd_sha256d_reply h;
+    if (!fromwire_sigverifyd_sha256d_reply(r, rl, &h) || h.n != 1) die_daemon("malformed sha256d reply");
+    memcpy(out32, h.hashes, 32);
+    free(r);
+    free(f);
+}
+
+/* one 33-byte key through sigverifyd_pubkey: ok and x || y as sv_pubkey_parse_host gives them */
+static void remote_pubkey(const u8 *der33, u8 xy[64], u8 *ok) {
+    size_t mlen = 2 + 8 + 4 + 33, rl;
+    u8 f[4 + 2 + 8 + 4 + 33];
+    uint64_t id = ++g_req_id;
+    towire_sigverifyd_pubkey(f + 4, mlen, id, 1, der33);
+    u8 *r = roundtrip(f, mlen, id, &rl);
+    struct sigverifyd_pubkey_reply k;
+    if (!fromwire_sigverifyd_pubkey_reply(r, rl, &k) || k.n != 1) die_daemon("malformed pubkey reply");
+    *ok = k.ok[0];
+    memcpy(xy, k.xy, 64);
+    free(r);
+}
+
 void sha256_double(struct sha256_double *shadouble, const void *p, size_t len) {
     uint64_t off = 0;
     uint32_t l = (uint32_t)len;
     u8 dummy = 0;
+    if (client()) {
+        remote_sha256d(len ? (const u8 *)p : &dummy, len, shadouble->sha.u.u8);
+        return;
+    }
     int rc = sv_sha256d_host(ctx(), len ? (const u8 *)p : &dummy, len, &off, &l, 1, shadouble->sha.u.u8);
     if (rc != SV_OK) die("sv_sha256d_host", rc);
 }
@@ -232,8 +270,12 @@ void sha256_double(struct sha256_double *shadouble, const void *p, size_t len) {
 bool pubkey_from_der(const u8 *der, size_t len, struct pubkey *key) {
     if (len != 33) return false; /* PUBKEY_CMPR_LEN, bitcoin/pubkey.c:16 */
     u8 xy[64], ok = 0;
-    int rc = sv_pubkey_parse_host(ctx(), der, 1, xy, &ok);
-    if (rc != SV_OK) die("sv_pubkey_parse_host", rc);
+    if (client()) {
+        remote_pubkey(der, xy, &ok);
+    } else {
+        int rc = sv_pubkey_parse_host(ctx(), der, 1, xy, &ok);
+        if (rc != SV_OK) die("sv_pubkey_parse_host", rc);
+    }
     if (!ok) return false;
     rev32(key->pubkey.data, xy);
     rev32(key->pubkey.data + 32, xy + 32);
@@ -267,8 +309,6 @@ static size_t put_output(u8 *p, const struct wally_tx_output *o) {
     if (o->script_len) memcpy(p + n, o->script, o->script_len);
     return n + o->script_len;
 }
-
-#define DAEMON_MAX_FRAME (32u + (1u << 20) * 161u) /* the largest message cln_sigverifyd reads (MAX_FRAME of sigverifyd.c) */
 
 /* the bytes of t's spans sv_verify_tx_host reads: witness script, outputs and, for a multi-input transaction, outpoints
  * and sequences; a span outside scripts[0 .. scripts_len) aborts, as the in-process call's SV_ERR_ARG does */
