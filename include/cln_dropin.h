@@ -126,6 +126,7 @@ void cln_sigverify_shutdown(void);
  *   bolt12_check_signature                                                              (sigverifyd_bolt12)
  *   check_tx_sig, check_tx_sigs_bip143_batch                                            (sigverifyd_tx)
  *   sigcheck_channel_announcement_batch / _node_announcement_batch / _channel_update_batch (sigverifyd_gossip)
+ *   sigcheck_gossip_batch                                                               (sigverifyd_gossip_burst)
  *   sha256_double                                                                       (sigverifyd_sha256d)
  *   pubkey_from_der                                                                     (sigverifyd_pubkey)
  * check_tx_sig gates the sighash type before it sends anything; the BIP143 sighash is built on the daemon's device.
@@ -186,6 +187,17 @@ void sigcheck_node_announcement_batch(const u8 *const *msgs, const size_t *lens,
 /* channel_update is signed by the node found in the gossmap: the caller supplies it. */
 void sigcheck_channel_update_batch(const u8 *const *msgs, const size_t *lens, const struct node_id *signers,
                                    size_t n, int *status);
+
+/* gossipd's signature gate over a burst of raw gossip messages of any types (sv_verify_gossip_burst_host in
+ * cln_sigverify.h): a channel_update's signer comes from the batch's own channel_announcements (signer_kind[i] 0), from
+ * signers[i] (1: the node the caller's gossmap gives), or from the batch with signers[i] as the source peer's fallback
+ * (2).  status[i]: 0 ok, 1..4 first bad signature, 5 verified under the source peer, -1 malformed, -2 no channel, -3
+ * another chain than chain_hash32, -4 node ids out of order.  signer_kind == NULL means all 0; signers may be NULL only
+ * when no channel_update has kind 1 or 2.  The batch is never split (an update may resolve against any announcement
+ * before it): in client mode it travels as ONE sigverifyd_gossip_burst request, and a batch too large for one frame
+ * aborts. */
+void sigcheck_gossip_batch(const u8 *chain_hash32, const u8 *const *msgs, const size_t *lens, size_t n, const u8 *signer_kind,
+                           const struct node_id *signers, int *status);
 
 #ifdef __cplusplus
 }

@@ -24,6 +24,10 @@
  *                                           :1501-1507, lightningd/offer.c:88-89, devtools/bolt12-cli.c:319-321
  *   sv_verify_bolt12_tagged_host(...)       the same checks, many callers' tags in one batch (the verifier
  *                                           subdaemon serves the plugins' bolt12_check_signature calls with it)
+ *   sv_verify_gossip_burst_host(...)        gossipd's signature gate over a burst: parse, node-id order and chain
+ *                                           gates gossipd/gossmap_manage.c:659-670, :1048-1051, sigcheck_*, and the
+ *                                           pending map that gives a channel_update its signer (:695-703,
+ *                                           :1060-1097), or the source peer's private-update check (:1099-1110)
  *   sv_sha256d_host(...)                    sha256_double()              bitcoin/shadouble.c:7-11
  *   sv_pubkey_parse_host(...)               pubkey_from_der()            bitcoin/pubkey.c:14-24
  *   sv_enqueue_* / sv_flush                 the deferral queue a batching caller (gossipd ingest,
@@ -119,6 +123,35 @@ int sv_verify_host_raw(sv_ctx *ctx, int kind, const uint8_t *data, size_t data_l
  *      MESSAGE, ignored for other types; NULL if the batch has no channel_update). ---- */
 int sv_verify_gossip_host(sv_ctx *ctx, const uint8_t *blob, size_t blob_len, const uint64_t *msg_off,
                           const uint32_t *msg_len, size_t n_msgs, const uint8_t *cu_signers33, int *status);
+
+/* ---- gossip BURST: a batch of raw gossip messages of any mix of types (a peer's channel_announcement followed by its
+ *      channel_updates, as initial sync and query_short_channel_ids deliver them), where an update's signer may be found
+ *      among the batch's own announcements.  status[m] is what gossipd's signature gate decides:
+ *        channel_announcement / node_announcement: as sv_verify_gossip_host (0, 1..4, -1), and for a channel_announcement
+ *          -4 if node_id_1 is not below node_id_2 (gossipd/gossmap_manage.c:659-663), else -3 if its chain_hash is not
+ *          chain_hash32 (:669-670).  A message the wire parser refuses is -1 before either gate, as in gossipd.  A gated
+ *          announcement reports no signature verdict.
+ *        channel_update: -1 as sv_verify_gossip_host, else -3 if its chain_hash is not chain_hash32 (:1048-1051), else by
+ *          signer_kind[m]:
+ *          1  signers33[m] is the node the caller's gossmap gives for the update's direction (sv_verify_gossip_host's
+ *             meaning; the batch is not consulted): 0 or 1.
+ *          0  the channel is the FIRST channel_announcement at an index j < m with the same short_channel_id whose final
+ *             status is 0 (gossipd's pending map, :695-703, :1060-1097: an announcement that fails sigcheck is never
+ *             added, a later one of the same scid can be, an update that arrives first finds no channel).  The signer is
+ *             its node_id_1 if channel_flags & 1 == 0, else its node_id_2: 0 or 1.  No such announcement: -2.
+ *          2  as 0; if no announcement resolves, signers33[m] is the source peer and the update is checked as gossipd's
+ *             private-update path does (:1099-1110): 5 if it verifies under the peer, -2 otherwise.
+ *      Every channel_announcement reports its own signatures, duplicates included.  Not decided here (policy, not
+ *      signatures): timestamp_reasonable, txout confirmation, node_announcements of nodes without channels.
+ *      signer_kind == NULL means all 0; signers33 (33 bytes per MESSAGE) may be NULL only when no channel_update has kind 1
+ *      or 2; a signer_kind above 2 (any message) is SV_ERR_ARG.  Resolution never reaches outside the call.  On the device:
+ *      an scid table of the gated announcements, one resolve thread per update and ONE verification launch for all
+ *      items; only when an update's candidate announcement itself fails does a second, small round run
+ *      (sv_last_gossip_repairs reports how many updates it took). ---- */
+int sv_verify_gossip_burst_host(sv_ctx *ctx, const uint8_t chain_hash32[32], const uint8_t *blob, size_t blob_len,
+                                const uint64_t *msg_off, const uint32_t *msg_len, size_t n_msgs, const uint8_t *signer_kind,
+                                const uint8_t *signers33, int *status);
+unsigned sv_last_gossip_repairs(const sv_ctx *ctx);
 
 /* L2 residency hint for the throughput kernels (default on): the G comb table and the per-thread multiples tables are
  * marked persisting through a stream access-policy window, the rest of the stream's traffic streaming.  0 switches it off

@@ -649,3 +649,50 @@ void sigcheck_channel_update_batch(const u8 *const *msgs, const size_t *lens, co
                                    size_t n, int *status) {
     gossip_batch(msgs, lens, n, signers, 258, status); /* struct node_id is exactly 33 bytes: signers[] is the packed array */
 }
+
+/* a burst through ONE sigverifyd_gossip_burst request: updates resolve against the whole batch, so it is never split;
+ * statuses 255..252 -> -1..-4 */
+static void remote_gossip_burst(const u8 *chain_hash32, const u8 *blob, size_t bytes, const size_t *len, size_t n,
+                                const u8 *signer_kind, const u8 *signers33, int *status) {
+    uint64_t mlen64 = 2 + 8 + 32 + 4 + (uint64_t)n * (4 + 1 + 33) + 4 + bytes;
+    if (n > (1u << 20) || bytes > 0xffffffffu || mlen64 > DAEMON_MAX_FRAME) die_daemon("gossip burst too large for one request");
+    size_t mlen = (size_t)mlen64, rl;
+    u8 *f = (u8 *)malloc(4 + mlen), *lens = (u8 *)malloc(4 * n + 1), *kinds = (u8 *)calloc(n + 1, 1), *sg = (u8 *)calloc(n + 1, 33);
+    if (!f || !lens || !kinds || !sg) die("malloc", -3);
+    for (size_t i = 0; i < n; i++) wire_put(lens + 4 * i, len[i], 4);
+    if (signer_kind) memcpy(kinds, signer_kind, n);
+    if (signers33) memcpy(sg, signers33, 33 * n);
+    uint64_t id = ++g_req_id;
+    towire_sigverifyd_gossip_burst(f + 4, mlen, id, chain_hash32, (uint32_t)n, lens, kinds, sg, (uint32_t)bytes, blob);
+    u8 *r = roundtrip(f, mlen, id, &rl);
+    struct sigverifyd_gossip_burst_reply g;
+    if (!fromwire_sigverifyd_gossip_burst_reply(r, rl, &g) || g.n != n) die_daemon("malformed gossip burst reply");
+    for (size_t i = 0; i < n; i++) status[i] = g.status[i] >= 252 ? (int)g.status[i] - 256 : g.status[i];
+    free(r); free(f); free(lens); free(kinds); free(sg);
+}
+
+void sigcheck_gossip_batch(const u8 *chain_hash32, const u8 *const *msgs, const size_t *lens, size_t n, const u8 *signer_kind,
+                           const struct node_id *signers, int *status) {
+    if (n == 0) return;
+    size_t total = 0;
+    for (size_t i = 0; i < n; i++) total += lens[i];
+    u8 *blob = (u8 *)malloc(total ? total : 1);
+    uint64_t *off = (uint64_t *)malloc(n * sizeof(uint64_t));
+    uint32_t *len = (uint32_t *)malloc(n * sizeof(uint32_t));
+    if (!blob || !off || !len) die("malloc", -3);
+    size_t t = 0;
+    for (size_t i = 0; i < n; i++) {
+        off[i] = t;
+        len[i] = (uint32_t)lens[i];
+        memcpy(blob + t, msgs[i], lens[i]);
+        t += lens[i];
+    }
+    if (client()) {
+        remote_gossip_burst(chain_hash32, blob, total, lens, n, signer_kind, signers ? signers[0].k : NULL, status);
+    } else {
+        int rc = sv_verify_gossip_burst_host(ctx(), chain_hash32, blob, total, off, len, n, signer_kind,
+                                             signers ? signers[0].k : NULL, status);
+        if (rc != SV_OK) die("sv_verify_gossip_burst_host", rc);
+    }
+    free(blob); free(off); free(len);
+}

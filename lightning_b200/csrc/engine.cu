@@ -426,9 +426,15 @@ __global__ void k_mask_verdicts(u8* verdict, const u8* ok, size_t n) {
 // gossipd/sigcheck.c:9-43 (channel_update), 45-115 (channel_announcement), 118-164 (node_announcement).
 // item_base[m] is the first item slot of message m (4 slots for a channel_announcement, 1 otherwise, host-computed
 // from the 2-byte type).  Writes span (off,len), key33, sig64 per item; status[m] = -1 if malformed.
+// Burst mode (chain32 != nullptr, sv_verify_gossip_burst_host): gossipd's gates after the parse
+// (gossipd/gossmap_manage.c:659-670, :1048-1051) set status[m] = -4 (channel_announcement whose node_id_1 is not below
+// node_id_2) or -3 (chain_hash other than chain32); the items are still sliced, because a signature encoding or
+// bitcoin_key the wire parser refuses makes the message -1 first.  A channel_update takes signers33[m] only where
+// kinds[m] == 1; the other updates get their key from k_gossip_resolve.
 __global__ void __launch_bounds__(128) k_gossip_slice(const u8* blob, const u64* msg_off, const u32* msg_len,
                                                       const u32* item_base, const u8* signers33, size_t n_msgs,
-                                                      u64* span_off, u32* span_len, u8* key33, u8* sig64, int* status) {
+                                                      u64* span_off, u32* span_len, u8* key33, u8* sig64, int* status,
+                                                      const u8* chain32, const u8* kinds) {
     size_t m = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (m >= n_msgs) return;
     const u8* p = blob + msg_off[m];
@@ -463,41 +469,158 @@ __global__ void __launch_bounds__(128) k_gossip_slice(const u8* blob, const u64*
         // signature(64) chain_hash(32) short_channel_id(8) timestamp(4) message_flags(1) channel_flags(1)
         // cltv_expiry_delta(2) htlc_minimum_msat(8) fee_base_msat(4) fee_proportional_millionths(4)
         // htlc_maximum_msat(8) = 138 bytes with the type (wire/peer_wire.csv:366-377; htlc_maximum_msat is mandatory)
-        if (len < 138 || signers33 == nullptr) st = -1;
+        if (len < 138 || (signers33 == nullptr && chain32 == nullptr)) st = -1;
     } else {
         st = -1;
     }
+    int gate = 0;
+    if (chain32 && st == 0 && type != 257) {
+        const u8* ch = p + ((type == 256) ? keys - 40 : 66);
+        for (int b = 0; b < 32; b++) gate |= ch[b] ^ chain32[b];
+        gate = gate ? -3 : 0;
+        if (type == 256) {
+            int c = 0;  // node_id_cmp: memcmp of the 33 bytes
+            for (int b = 0; b < 33 && c == 0; b++) c = (int)p[keys + b] - (int)p[keys + 33 + b];
+            if (c >= 0) gate = -4;
+        }
+    }
+    const bool cu_key = !chain32 || (kinds[m] == 1);
     for (int k = 0; k < nitems; k++) {
         u32 it = base + k;
         bool ok = (st == 0);
         span_off[it] = msg_off[m] + (ok ? hoff : 0);
         span_len[it] = ok ? (len - hoff) : 0;
         const u8* kp = (type == 258) ? (signers33 ? signers33 + 33 * m : p) : (p + keys + 33 * k);
-        for (int b = 0; b < 33; b++) key33[33 * (size_t)it + b] = ok ? kp[b] : 0;  // an all-zero key never verifies
+        const bool kok = ok && (type != 258 || cu_key);
+        for (int b = 0; b < 33; b++) key33[33 * (size_t)it + b] = kok ? kp[b] : 0;  // an all-zero key never verifies
         const u8* sp = p + 2 + 64 * k;
         for (int b = 0; b < 64; b++) sig64[64 * (size_t)it + b] = ok ? sp[b] : 0;
     }
-    status[m] = st;
+    status[m] = st ? st : gate;
+}
+
+// ---- gossip bursts: a channel_update's signer found among the batch's own channel_announcements ------------------
+// The scid table is exact open addressing keyed by the 8 scid bytes (k_dedup_insert's pattern): a slot holds a message
+// index, the bytes are compared in the blob, and atomicMin keeps the LOWEST index of each scid (a slot only ever changes
+// to another index of the same scid, so a concurrent probe still compares the right bytes).
+#define SV_SCID_EMPTY 0xFFFFFFFFu
+__device__ __forceinline__ const u8* gossip_scid(const u8* p) {
+    // channel_announcement: after 4 signatures, features, chain_hash; channel_update: after signature and chain_hash
+    return (p[1] == 0) ? p + 260 + (((u32)p[258] << 8) | p[259]) + 32 : p + 98;
+}
+__device__ __forceinline__ u32 scid_hash(const u8* s) {
+    u32 h = 2166136261u;
+    for (int b = 0; b < 8; b++) h = (h ^ s[b]) * 16777619u;
+    return h ^ (h >> 15);
+}
+__device__ __forceinline__ bool scid_same(const u8* a, const u8* b) {
+    bool same = true;
+    for (int k = 0; k < 8; k++) same = same && (a[k] == b[k]);
+    return same;
+}
+// every channel_announcement whose status is 0 goes in: after k_gossip_slice these are the well-formed, right-chain,
+// ordered ones; after k_gossip_status the ones whose four signatures verify
+__global__ void __launch_bounds__(256) k_scid_insert(const u8* blob, const u64* msg_off, const u32* msg_len, const int* status,
+                                                     size_t n_msgs, u32* slots, u32 mask) {
+    size_t m = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (m >= n_msgs || status[m] != 0 || msg_len[m] < 2) return;
+    const u8* p = blob + msg_off[m];
+    if (p[0] != 1 || p[1] != 0) return;
+    const u8* s = gossip_scid(p);
+    u32 slot = scid_hash(s) & mask;
+    for (;;) {
+        u32 old = atomicCAS(&slots[slot], SV_SCID_EMPTY, (u32)m);
+        if (old == SV_SCID_EMPTY) return;
+        if (scid_same(gossip_scid(blob + msg_off[old]), s)) { atomicMin(&slots[slot], (u32)m); return; }
+        slot = (slot + 1) & mask;
+    }
+}
+// One thread per channel_update that takes its signer from the batch (kinds 0 and 2, status 0 after the slice).  The
+// candidate is the lowest-index announcement of the scid in the table; it counts only if it comes before the update.
+// cand[m] = its index (the key is its node_id_1 or node_id_2 by channel_flags & 1, byte 111) or SV_SCID_EMPTY (the key
+// is signers33[m] for kind 2, all zero otherwise).  list == nullptr: every message, item slot item_base[m].  list = the
+// repair list ([count, m...]): update list[1 + t] moves to item slot tail + t, with its hash and signature.
+__global__ void __launch_bounds__(128) k_gossip_resolve(const u8* blob, const u64* msg_off, const u32* msg_len, u32* item_base,
+                                                        const int* status, const u8* kinds, const u8* signers33,
+                                                        size_t n, const u32* slots, u32 mask, u32* cand, const u32* list,
+                                                        u32 tail, u8* msg32, u8* key33, u8* sig64) {
+    size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    size_t m = list ? list[1 + t] : t;
+    if (!list) {
+        if (status[m] != 0 || kinds[m] == 1 || msg_len[m] < 2) return;
+        const u8* q = blob + msg_off[m];
+        if (q[0] != 1 || q[1] != 2) return;
+    }
+    const u8* p = blob + msg_off[m];
+    u32 it = item_base[m];
+    if (list) {
+        u32 to = tail + (u32)t;
+        for (int b = 0; b < 32; b++) msg32[32 * (size_t)to + b] = msg32[32 * (size_t)it + b];
+        for (int b = 0; b < 64; b++) sig64[64 * (size_t)to + b] = sig64[64 * (size_t)it + b];
+        item_base[m] = it = to;
+    }
+    const u8* s = p + 98;
+    u32 slot = scid_hash(s) & mask, j;
+    for (;;) {
+        j = slots[slot];
+        if (j == SV_SCID_EMPTY || scid_same(gossip_scid(blob + msg_off[j]), s)) break;
+        slot = (slot + 1) & mask;
+    }
+    const u8* kp = nullptr;
+    if (j != SV_SCID_EMPTY && j < m) {
+        const u8* a = blob + msg_off[j];
+        kp = gossip_scid(a) + 8 + 33 * (p[111] & 1);
+    } else {
+        j = SV_SCID_EMPTY;
+        if (kinds[m] == 2) kp = signers33 + 33 * m;
+    }
+    cand[m] = j;
+    for (int b = 0; b < 33; b++) key33[33 * (size_t)it + b] = kp ? kp[b] : 0;
 }
 // status[m] = 1 + index of the first failing signature (the reference's order), 0 if all verify
 // -1 also when CLN's wire parser would refuse the message: a signature with r >= n or s >= n
 // (fromwire_secp256k1_ecdsa_signature, wire/fromwire.c:188-199) or an undecodable bitcoin_key (fromwire_pubkey,
 // bitcoin/pubkey.c:102-113).  node_ids are raw bytes on the wire (common/node_id.c:54) and only fail the signature.
-__global__ void __launch_bounds__(128) k_gossip_status(const u8* blob, const u64* msg_off, const u32* msg_len,
-                                                       const u32* item_base, size_t n_msgs, const u8* verdict,
-                                                       const u8* aux, int* status) {
-    size_t m = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (m >= n_msgs || status[m] != 0) return;
-    const u8* p = blob + msg_off[m];
-    u32 type = ((u32)p[0] << 8) | p[1];
+__device__ __forceinline__ int gossip_items_status(u32 type, u32 base, const u8* verdict, const u8* aux) {
     int nitems = (type == 256) ? 4 : 1;
     int st = 0;
     for (int k = nitems - 1; k >= 0; k--)
-        if (!verdict[item_base[m] + k]) st = k + 1;
+        if (!verdict[base + k]) st = k + 1;
     for (int k = 0; k < nitems; k++) {
-        u32 it = item_base[m] + k;
+        u32 it = base + k;
         if (!(aux[it] & 2u)) st = -1;                           // r or s >= n: the wire parser refuses the message
         if (type == 256 && k >= 2 && !(aux[it] & 1u)) st = -1;  // undecodable bitcoin_key
+    }
+    return st;
+}
+// Burst mode (kinds != nullptr): a gated message (-3, -4) keeps its gate unless the parse refuses it (-1).  A
+// channel_update resolved from the batch (cand[m], k_gossip_resolve) is settled from its candidate's own item verdicts:
+// if the candidate verifies, the update's own verdict stands; if not, the update goes on the repair list ([count, m...])
+// and keeps status 0 for the repair round (which runs this kernel again with repair == nullptr).  No candidate: -2, or
+// for kind 2 (the source peer's private-update check, gossmap_manage.c:1099-1110) 5 if it verifies under the peer.
+__global__ void __launch_bounds__(128) k_gossip_status(const u8* blob, const u64* msg_off, const u32* msg_len,
+                                                       const u32* item_base, size_t n_msgs, const u8* verdict,
+                                                       const u8* aux, int* status, const u8* kinds, const u32* cand,
+                                                       u32* repair) {
+    size_t m = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (m >= n_msgs) return;
+    const int st0 = status[m];
+    if (st0 != 0 && !(kinds && (st0 == -3 || st0 == -4))) return;
+    const u8* p = blob + msg_off[m];
+    u32 type = ((u32)p[0] << 8) | p[1];
+    int st = gossip_items_status(type, item_base[m], verdict, aux);
+    if (kinds && st != -1) {
+        if (st0 != 0) return;
+        if (type == 258 && kinds[m] != 1) {
+            u32 j = cand[m];
+            if (j == SV_SCID_EMPTY) {
+                st = (kinds[m] == 2 && st == 0) ? 5 : -2;
+            } else if (repair && gossip_items_status(256, item_base[j], verdict, aux) != 0) {
+                repair[1 + atomicAdd(repair, 1u)] = (u32)m;
+                return;
+            }
+        }
     }
     status[m] = st;
 }
@@ -1036,6 +1159,7 @@ struct sv_ctx {
     int dedup;  // gossip batches: look for repeated keys (sv_set_dedup; default on)
     int nosqrt; // compressed-key ECDSA through the flow without the square root (default on; env SV_NOSQRT=0: measurement aid)
     u32 last_distinct;
+    u32 last_repair;  // updates the last gossip burst re-resolved in its repair round
     // growable device staging for the host-buffer entry points
     size_t cap;  // items
     u8 *d_msg, *d_key, *d_sig, *d_verdict;
@@ -1168,6 +1292,7 @@ extern "C" int sv_create(sv_ctx** out, int device) {
     ctx->nosqrt = 1;
     if (const char* e = getenv("SV_NOSQRT")) ctx->nosqrt = atoi(e) != 0;
     ctx->last_distinct = 0;
+    ctx->last_repair = 0;
     ctx->small_cap = SV_SMALL_CAP;
     ctx->small_max = SV_SMALL_MAX_DEFAULT;
     if (const char* e = getenv("SV_SMALL_MAX")) ctx->small_max = (size_t)strtoull(e, nullptr, 10);
@@ -1683,23 +1808,45 @@ extern "C" int sv_pubkey_parse_host(sv_ctx* ctx, const uint8_t* key33, size_t n,
     return SV_OK;
 }
 
+// the ECDSA33 verification of a gossip batch's items: with key de-duplication when it is on and pays
+static int gossip_verify_items(sv_ctx* ctx, u8* d_msg, u8* d_key, u8* d_sig, size_t n, u8* d_verdict, cudaStream_t st,
+                               u8* d_keyok, u32* distinct_out) {
+    // node keys repeat heavily inside a gossip batch (every channel of a node, its updates, its announcement)
+    int rc = ctx->dedup ? launch_verify_dedup(ctx, SV_KIND_ECDSA33, d_msg, d_key, d_sig, n, d_verdict, st, d_keyok, distinct_out) : 0;
+    if (rc == 0) rc = launch_verify(ctx, SV_KIND_ECDSA33, d_msg, d_key, d_sig, n, d_verdict, nullptr, st, d_keyok);
+    else if (rc == 1) rc = SV_OK;
+    return rc;
+}
+
 // gossip ingest with device-side slicing: blob = concatenated wire messages, msg_off/msg_len locate them.
-extern "C" int sv_verify_gossip_host(sv_ctx* ctx, const uint8_t* blob, size_t blob_len, const uint64_t* msg_off,
-                                     const uint32_t* msg_len, size_t n_msgs, const uint8_t* cu_signers33, int* status) {
+// chain32 == nullptr: sv_verify_gossip_host (signers from the caller).  Otherwise sv_verify_gossip_burst_host: kinds
+// (n_msgs bytes, or nullptr for all 0) says where each channel_update's signer comes from.
+static int gossip_run(sv_ctx* ctx, const uint8_t* chain32, const uint8_t* blob, size_t blob_len, const uint64_t* msg_off,
+                      const uint32_t* msg_len, size_t n_msgs, const uint8_t* kinds, const uint8_t* cu_signers33, int* status) {
     if (!ctx || (n_msgs && (!blob || !msg_off || !msg_len || !status))) return SV_ERR_ARG;
     if (n_msgs == 0) return SV_OK;
+    const bool burst = chain32 != nullptr;
     dev_guard dg__;
     CK(dg__.enter(ctx->device));
     // the host only reads the 2-byte type of each message to lay out the item slots
     std::vector<u32> base(n_msgs);
-    size_t items = 0;
+    size_t items = 0, n_ca = 0, n_cu = 0;
     for (size_t m = 0; m < n_msgs; m++) {
         if (msg_off[m] > blob_len || msg_len[m] > blob_len - msg_off[m]) return fail(ctx, SV_ERR_ARG, "message out of range", cudaSuccess);
         u32 type = msg_len[m] >= 2 ? (((u32)blob[msg_off[m]] << 8) | blob[msg_off[m] + 1]) : 0;
         base[m] = (u32)items;
         items += (type == 256) ? 4 : ((type == 257 || type == 258) ? 1 : 0);
+        if (burst) {
+            u8 k = kinds ? kinds[m] : 0;
+            if (k > 2) return fail(ctx, SV_ERR_ARG, "signer_kind above 2", cudaSuccess);
+            if (type == 258 && k != 0 && !cu_signers33) return fail(ctx, SV_ERR_ARG, "signer_kind 1 or 2 without signers33", cudaSuccess);
+            n_ca += type == 256;
+            n_cu += type == 258;
+        }
     }
-    size_t cap = items ? items : 1;
+    if (items + n_cu > 0xFFFFFFFFu) return fail(ctx, SV_ERR_ARG, "too many signatures in one gossip batch", cudaSuccess);
+    // burst: item slots [items, items + n_cu) take the updates of a repair round
+    size_t cap = items + n_cu ? items + n_cu : 1;
     int rc = ensure_staging(ctx, cap);
     if (rc) return rc;
     if (blob_len > ctx->data_cap) {
@@ -1714,8 +1861,14 @@ extern "C" int sv_verify_gossip_host(sv_ctx* ctx, const uint8_t* blob, size_t bl
         CK(cudaMalloc(&ctx->d_len, need * sizeof(u32)));
         ctx->span_cap = need;
     }
-    // one grow-only slab: [msg_off u64][msg_len u32][item_base u32][status int][signers 33B][keyok 1B per item]
-    size_t need_g = n_msgs * (8 + 4 + 4 + 4 + 33) + cap + 64;
+    // one grow-only slab: [msg_off u64][msg_len u32][item_base u32][status int][signers 33B][keyok 1B per item], and for a
+    // burst [kinds 1B][cand u32][repair list u32 (count, then indices)][chain_hash 32B][scid table u32], 16-byte aligned
+    auto a16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
+    u32 tcap = 64;
+    while (tcap < 2 * n_ca) tcap <<= 1;
+    const size_t ex = a16(n_msgs * (8 + 4 + 4 + 4 + 33) + cap), ex_cand = ex + a16(n_msgs), ex_rep = ex_cand + a16(4 * n_msgs),
+                 ex_chain = ex_rep + a16(4 * (n_msgs + 1)), ex_slots = ex_chain + 32;
+    size_t need_g = burst ? ex_slots + (size_t)tcap * 4 : n_msgs * (8 + 4 + 4 + 4 + 33) + cap + 64;
     if (need_g > ctx->g_cap) {
         CK(cudaDeviceSynchronize());
         size_t gcap = ctx->g_cap ? ctx->g_cap : (1u << 16);
@@ -1730,6 +1883,11 @@ extern "C" int sv_verify_gossip_host(sv_ctx* ctx, const uint8_t* blob, size_t bl
     int* d_status = reinterpret_cast<int*>(d_base + n_msgs);
     u8* d_signers = reinterpret_cast<u8*>(d_status + n_msgs);
     u8* d_keyok = d_signers + 33 * n_msgs;
+    u8* d_kinds = burst ? ctx->g_buf + ex : nullptr;
+    u32* d_cand = reinterpret_cast<u32*>(ctx->g_buf + ex_cand);
+    u32* d_repair = reinterpret_cast<u32*>(ctx->g_buf + ex_rep);
+    u8* d_chain = burst ? ctx->g_buf + ex_chain : nullptr;
+    u32* d_slots = reinterpret_cast<u32*>(ctx->g_buf + ex_slots);
     if (!cu_signers33) d_signers = nullptr;
     cudaStream_t st = ctx->stream;
     CK(cudaMemcpyAsync(ctx->d_data, blob, blob_len, cudaMemcpyHostToDevice, st));
@@ -1737,29 +1895,77 @@ extern "C" int sv_verify_gossip_host(sv_ctx* ctx, const uint8_t* blob, size_t bl
     CK(cudaMemcpyAsync(d_mlen, msg_len, n_msgs * sizeof(u32), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_base, base.data(), n_msgs * sizeof(u32), cudaMemcpyHostToDevice, st));
     if (cu_signers33) CK(cudaMemcpyAsync(d_signers, cu_signers33, n_msgs * 33, cudaMemcpyHostToDevice, st));
+    if (burst) {
+        if (kinds) CK(cudaMemcpyAsync(d_kinds, kinds, n_msgs, cudaMemcpyHostToDevice, st));
+        else CK(cudaMemsetAsync(d_kinds, 0, n_msgs, st));
+        CK(cudaMemcpyAsync(d_chain, chain32, 32, cudaMemcpyHostToDevice, st));
+        CK(cudaMemsetAsync(d_repair, 0, 4, st));
+    }
     unsigned gm = (unsigned)((n_msgs + 127) / 128);
     k_gossip_slice<<<gm, 128, 0, st>>>(ctx->d_data, d_moff, d_mlen, d_base, d_signers, n_msgs, ctx->d_off, ctx->d_len,
-                                       ctx->d_key, ctx->d_sig, d_status);
+                                       ctx->d_key, ctx->d_sig, d_status, d_chain, d_kinds);
     ctx->launches += 1;
+    if (burst && n_cu) {
+        // each update's signer from the first gated announcement of its scid, written into its item slot before hashing
+        CK(cudaMemsetAsync(d_slots, 0xFF, (size_t)tcap * 4, st));
+        k_scid_insert<<<(unsigned)((n_msgs + 255) / 256), 256, 0, st>>>(ctx->d_data, d_moff, d_mlen, d_status, n_msgs, d_slots, tcap - 1);
+        k_gossip_resolve<<<gm, 128, 0, st>>>(ctx->d_data, d_moff, d_mlen, d_base, d_status, d_kinds, d_signers, n_msgs, d_slots,
+                                             tcap - 1, d_cand, nullptr, 0, ctx->d_msg, ctx->d_key, ctx->d_sig);
+        ctx->launches += 2;
+    }
     if (items) {
         k_sha256d<<<(unsigned)((items + 127) / 128), 128, 0, st>>>(ctx->d_data, ctx->d_off, ctx->d_len, items, ctx->d_msg);
         ctx->launches += 1;
-        // node keys repeat heavily inside a gossip batch (every channel of a node, its updates, its announcement)
-        rc = ctx->dedup ? launch_verify_dedup(ctx, SV_KIND_ECDSA33, ctx->d_msg, ctx->d_key, ctx->d_sig, items, ctx->d_verdict, st, d_keyok,
-                                              &ctx->last_distinct) : 0;
-        if (rc == 0) rc = launch_verify(ctx, SV_KIND_ECDSA33, ctx->d_msg, ctx->d_key, ctx->d_sig, items, ctx->d_verdict, nullptr, st, d_keyok);
-        else if (rc == 1) rc = SV_OK;
+        rc = gossip_verify_items(ctx, ctx->d_msg, ctx->d_key, ctx->d_sig, items, ctx->d_verdict, st, d_keyok, &ctx->last_distinct);
         if (rc == SV_OK) {
-            k_gossip_status<<<gm, 128, 0, st>>>(ctx->d_data, d_moff, d_mlen, d_base, n_msgs, ctx->d_verdict, d_keyok, d_status);
+            k_gossip_status<<<gm, 128, 0, st>>>(ctx->d_data, d_moff, d_mlen, d_base, n_msgs, ctx->d_verdict, d_keyok, d_status,
+                                                d_kinds, d_cand, burst ? d_repair : nullptr);
             ctx->launches += 1;
         }
     }
+    u32 n_repair = 0;
     cudaError_t ce = cudaMemcpyAsync(status, d_status, n_msgs * sizeof(int), cudaMemcpyDeviceToHost, st);
+    if (ce == cudaSuccess && burst) ce = cudaMemcpyAsync(&n_repair, d_repair, 4, cudaMemcpyDeviceToHost, st);
     if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
     if (rc) return rc;
     if (ce != cudaSuccess) return fail(ctx, SV_ERR_CUDA, "gossip ingest", ce);
+    if (n_repair) {
+        // Repair round: some updates resolved to an announcement whose own signatures fail.  The right one is the first
+        // announcement before the update whose status is 0 (every such status is final now), else the source peer (kind
+        // 2), else none.  The table is rebuilt from those announcements only, the updates move to the spare item slots
+        // [items, items + n_repair) and are verified again; k_gossip_status then settles them (and recomputes the rest
+        // to the same values).  Nothing it resolves to can fail, so one round is enough.
+        CK(cudaMemsetAsync(d_slots, 0xFF, (size_t)tcap * 4, st));
+        k_scid_insert<<<(unsigned)((n_msgs + 255) / 256), 256, 0, st>>>(ctx->d_data, d_moff, d_mlen, d_status, n_msgs, d_slots, tcap - 1);
+        k_gossip_resolve<<<(n_repair + 127) / 128, 128, 0, st>>>(ctx->d_data, d_moff, d_mlen, d_base, d_status, d_kinds, d_signers,
+                                                                 n_repair, d_slots, tcap - 1, d_cand, d_repair, (u32)items,
+                                                                 ctx->d_msg, ctx->d_key, ctx->d_sig);
+        ctx->launches += 2;
+        rc = gossip_verify_items(ctx, ctx->d_msg + 32 * items, ctx->d_key + 33 * items, ctx->d_sig + 64 * items, n_repair,
+                                 ctx->d_verdict + items, st, d_keyok + items, nullptr);
+        if (rc) return rc;
+        k_gossip_status<<<gm, 128, 0, st>>>(ctx->d_data, d_moff, d_mlen, d_base, n_msgs, ctx->d_verdict, d_keyok, d_status,
+                                            d_kinds, d_cand, nullptr);
+        ctx->launches += 1;
+        CK(cudaMemcpyAsync(status, d_status, n_msgs * sizeof(int), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+    }
+    ctx->last_repair = n_repair;
     return SV_OK;
 }
+
+extern "C" int sv_verify_gossip_host(sv_ctx* ctx, const uint8_t* blob, size_t blob_len, const uint64_t* msg_off,
+                                     const uint32_t* msg_len, size_t n_msgs, const uint8_t* cu_signers33, int* status) {
+    return gossip_run(ctx, nullptr, blob, blob_len, msg_off, msg_len, n_msgs, nullptr, cu_signers33, status);
+}
+
+extern "C" int sv_verify_gossip_burst_host(sv_ctx* ctx, const uint8_t chain_hash32[32], const uint8_t* blob, size_t blob_len,
+                                           const uint64_t* msg_off, const uint32_t* msg_len, size_t n_msgs,
+                                           const uint8_t* signer_kind, const uint8_t* signers33, int* status) {
+    if (!chain_hash32) return SV_ERR_ARG;
+    return gossip_run(ctx, chain_hash32, blob, blob_len, msg_off, msg_len, n_msgs, signer_kind, signers33, status);
+}
+extern "C" unsigned sv_last_gossip_repairs(const sv_ctx* ctx) { return ctx ? ctx->last_repair : 0; }
 
 // n ECDSA signatures by ONE key (channeld's HTLC loop): table of the key built once, ladder-only kernel
 extern "C" int sv_verify_samekey_host(sv_ctx* ctx, int kind, const uint8_t* key, const uint8_t* msg32, const uint8_t* sig64,

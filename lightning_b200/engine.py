@@ -59,6 +59,9 @@ def load_library():
     lib.sv_verify_host_raw.argtypes = [vp, i, vp, sz, vp, vp, vp, vp, sz, vp]
     lib.sv_verify_device.argtypes = [vp, i, vp, vp, vp, sz, vp, vp, vp]
     lib.sv_verify_gossip_host.argtypes = [vp, vp, sz, vp, vp, sz, vp, vp]
+    lib.sv_verify_gossip_burst_host.argtypes = [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp]
+    lib.sv_last_gossip_repairs.argtypes = [vp]
+    lib.sv_last_gossip_repairs.restype = ctypes.c_uint
     lib.sv_verify_tx_host.argtypes = [vp, i, vp, vp, sz, vp, vp, sz, vp, vp]
     lib.sv_verify_samekey_host.argtypes = [vp, i, vp, vp, vp, sz, vp]
     lib.sv_verify_bolt12_host.argtypes = [vp, ctypes.c_char_p, ctypes.c_char_p, vp, sz, vp, vp, vp, vp, sz, vp, vp]
@@ -190,6 +193,35 @@ class SigVerifier:
                                                    sg.ctypes.data if sg is not None else None, status.ctypes.data),
                     "sv_verify_gossip_host")
         return status[:n]
+
+    def verify_gossip_burst(self, msgs, chain_hash, signer_kind=None, signers=None):
+        """A burst of raw gossip messages of any types; a channel_update's signer comes from the batch's own
+        channel_announcements (signer_kind 0), from signers[m] (1), or from the batch with signers[m] as the source peer's
+        fallback (2).  Returns int32 statuses: 0 ok, 1..4 first bad signature, 5 verified under the source peer, -1
+        malformed, -2 no channel, -3 other chain, -4 node ids out of order (cln_sigverify.h)."""
+        n = len(msgs)
+        lens = np.array([len(m) for m in msgs], dtype=np.uint32)
+        offs = np.concatenate([[0], np.cumsum(lens[:-1], dtype=np.uint64)]).astype(np.uint64) if n else np.zeros(0, np.uint64)
+        blob = np.frombuffer(b"".join(bytes(m) for m in msgs), dtype=np.uint8)
+        chain = np.frombuffer(bytes(chain_hash), dtype=np.uint8)
+        if chain.size != 32:
+            raise ValueError("chain_hash must be 32 bytes")
+        kinds = None if signer_kind is None else np.ascontiguousarray(signer_kind, dtype=np.uint8).reshape(-1)
+        if kinds is not None and kinds.size != n:
+            raise ValueError("signer_kind: one byte per message")
+        sg = None if signers is None else _u8(signers, 33)
+        if sg is not None and sg.shape[0] != n:
+            raise ValueError("signers: one 33-byte key per message")
+        status = np.zeros(max(n, 1), dtype=np.int32)
+        self._check(self.lib.sv_verify_gossip_burst_host(
+            self._ctx, chain.ctypes.data, blob.ctypes.data, blob.size, offs.ctypes.data, lens.ctypes.data, n,
+            kinds.ctypes.data if kinds is not None else None, sg.ctypes.data if sg is not None else None,
+            status.ctypes.data), "sv_verify_gossip_burst_host")
+        return status[:n]
+
+    def last_gossip_repairs(self):
+        """updates the last gossip burst re-resolved in its repair round (their first candidate announcement failed)"""
+        return int(self.lib.sv_last_gossip_repairs(self._ctx))
 
     def verify_samekey(self, kind, key, msg32, sig64):
         """n ECDSA signatures by ONE key (channeld's HTLC loop): the key's table is built once on the device."""
