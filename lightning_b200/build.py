@@ -25,6 +25,9 @@ NVCC_FLAGS = [
     # in the ladder one barrier every 2 windows (tools/variants.py compares the other spacings)
     "-DSV_FE_INLINE", "-DSV_MAIN_SYNC", "-DSV_SYNC_LEVEL=1", "-DSV_SYNC_WINDOWS=2",
 ]
+# gcc flags of the plain-C parts: the drop-in (linked into the library) and the verifier subdaemon
+DROPIN_CFLAGS = ["-O2", "-fPIC", "-Wall", "-Wextra", "-std=c11"]
+DAEMON_CFLAGS = ["-O2", "-Wall", "-Wextra", "-std=c11"]
 
 
 def _newer(target, sources):
@@ -53,8 +56,7 @@ def build_engine(force=False, verbose=False, extra_flags=()):
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     # host side of the drop-in is plain C (as the reference's bitcoin/signature.c), compiled by gcc
     dropin_o = os.path.join(CSRC, "cln_dropin.o")
-    r = subprocess.run(["gcc", "-O2", "-fPIC", "-Wall", "-Wextra", "-std=c11", "-c", os.path.join(CSRC, "cln_dropin.c"),
-                        "-o", dropin_o], capture_output=True, text=True)
+    r = subprocess.run(["gcc"] + DROPIN_CFLAGS + ["-c", os.path.join(CSRC, "cln_dropin.c"), "-o", dropin_o], capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("gcc (cln_dropin.c) failed:\n" + r.stdout + r.stderr)
     # the batch-verification kernels are a translation unit of their own, compiled with the field multiplier as real
@@ -75,7 +77,7 @@ def build_engine(force=False, verbose=False, extra_flags=()):
     if r.returncode != 0:
         raise RuntimeError("nvcc failed:\n" + r.stdout + r.stderr)
     # verifier subdaemon (row N4): plain C, links the engine
-    r = subprocess.run(["gcc", "-O2", "-Wall", "-Wextra", "-std=c11", os.path.join(CSRC, "sigverifyd.c"), "-o", DAEMON,
+    r = subprocess.run(["gcc"] + DAEMON_CFLAGS + [os.path.join(CSRC, "sigverifyd.c"), "-o", DAEMON,
                         "-L" + os.path.dirname(LIB), "-lcln_sigverify", "-Wl,-rpath,$ORIGIN"], capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("gcc (sigverifyd.c) failed:\n" + r.stdout + r.stderr)

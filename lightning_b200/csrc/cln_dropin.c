@@ -10,6 +10,7 @@
 #define _GNU_SOURCE
 #include "../../include/cln_dropin.h"
 #include "../../include/cln_sigverify.h"
+#include "sigverifyd_proto.h"
 #include "sigverifyd_wiregen.h"
 
 #include <errno.h>
@@ -36,8 +37,6 @@ static void die(const char *what, int rc) {
 static int g_sock = -1;
 static int g_env_done;
 static uint64_t g_req_id;
-
-#define DAEMON_MAX_FRAME (32u + (1u << 20) * 161u) /* the largest message cln_sigverifyd reads (MAX_FRAME of sigverifyd.c) */
 
 static void die_daemon(const char *what) {
     fprintf(stderr, "cln_sigverify: verifier subdaemon: %s\n", what);
@@ -183,49 +182,43 @@ static void pubkey_to_xy(u8 out[64], const secp256k1_pubkey *p) {
     rev32(out + 32, p->data + 32);
 }
 
+/* one verification of this kind: through the daemon in client mode, else in process */
+static bool verify_one(int kind, const u8 *msg32, const u8 *key, const u8 *sig64) {
+    u8 v = 0;
+    if (client()) {
+        remote_verify(kind, msg32, key, sig64, 1, &v);
+    } else {
+        int rc = sv_verify_host(ctx(), kind, msg32, key, sig64, 1, &v);
+        if (rc != SV_OK) die("sv_verify_host", rc);
+    }
+    return v == 1;
+}
+
 bool check_signed_hash(const struct sha256_double *hash, const secp256k1_ecdsa_signature *signature,
                        const struct pubkey *key) {
-    u8 sig[64], xy[64], v = 0;
+    u8 sig[64], xy[64];
     sig_to_wire(sig, signature);
     pubkey_to_xy(xy, &key->pubkey);
-    if (client()) {
-        remote_verify(SV_KIND_ECDSA_XY, hash->sha.u.u8, xy, sig, 1, &v);
-        return v == 1;
-    }
-    int rc = sv_verify_host(ctx(), SV_KIND_ECDSA_XY, hash->sha.u.u8, xy, sig, 1, &v);
-    if (rc != SV_OK) die("sv_verify_host", rc);
-    return v == 1;
+    return verify_one(SV_KIND_ECDSA_XY, hash->sha.u.u8, xy, sig);
 }
 
 bool check_signed_hash_nodeid(const struct sha256_double *hash, const secp256k1_ecdsa_signature *signature,
                               const struct node_id *id) {
-    u8 sig[64], v = 0;
+    u8 sig[64];
     sig_to_wire(sig, signature);
-    if (client()) {
-        remote_verify(SV_KIND_ECDSA33, hash->sha.u.u8, id->k, sig, 1, &v);
-        return v == 1;
-    }
-    int rc = sv_verify_host(ctx(), SV_KIND_ECDSA33, hash->sha.u.u8, id->k, sig, 1, &v);
-    if (rc != SV_OK) die("sv_verify_host", rc);
-    return v == 1;
+    return verify_one(SV_KIND_ECDSA33, hash->sha.u.u8, id->k, sig);
 }
 
 bool check_schnorr_sig(const struct sha256 *hash, const secp256k1_pubkey *pubkey, const struct bip340sig *sig) {
     /* signature.c:412-423: serialize compressed, drop the parity byte -> x-only key */
-    u8 xy[64], v = 0;
+    u8 xy[64];
     pubkey_to_xy(xy, pubkey);
-    if (client()) {
-        remote_verify(SV_KIND_SCHNORR, hash->u.u8, xy, sig->u8, 1, &v);
-        return v == 1;
-    }
-    int rc = sv_verify_host(ctx(), SV_KIND_SCHNORR, hash->u.u8, xy, sig->u8, 1, &v);
-    if (rc != SV_OK) die("sv_verify_host", rc);
-    return v == 1;
+    return verify_one(SV_KIND_SCHNORR, hash->u.u8, xy, sig->u8);
 }
 
 /* one buffer through sigverifyd_sha256d; a buffer too large for one frame aborts */
 static void remote_sha256d(const u8 *p, size_t len, u8 out32[32]) {
-    if (len > DAEMON_MAX_FRAME - (2 + 8 + 4 + 4 + 4)) die_daemon("buffer too large for one request");
+    if (len > MAX_FRAME - (2 + 8 + 4 + 4 + 4)) die_daemon("buffer too large for one request");
     size_t mlen = 2 + 8 + 4 + 4 + 4 + len, rl;
     u8 *f = (u8 *)malloc(4 + mlen);
     if (!f) die("malloc", -3);
@@ -295,6 +288,15 @@ void cln_sigverify_set_tx_hooks(size_t (*script_bytelen)(const void *), uint64_t
     g_input_sat = input_amount_sat;
 }
 
+/* the byte length of a tal array (NULL: 0), through the hook or CLN's own tal_bytelen; `who` names the caller in the
+ * abort when neither is there */
+static size_t tal_len(const void *p, const char *who) {
+    if (g_bytelen) return p ? g_bytelen(p) : 0;
+    if (tal_bytelen) return p ? tal_bytelen(p) : 0;
+    die(who, -4);
+    return 0;
+}
+
 static size_t put_varint(u8 *p, uint64_t v) { /* Bitcoin CompactSize */
     if (v < 0xfd) { p[0] = (u8)v; return 1; }
     if (v <= 0xffff) { p[0] = 0xfd; p[1] = (u8)v; p[2] = (u8)(v >> 8); return 3; }
@@ -338,7 +340,7 @@ static void remote_tx(int kind, const u8 *key, const sv_tx *txs, const u8 *scrip
             m++;
         }
         uint64_t mlen64 = 2 + 8 + 1 + 4 + ks + 4 + per_tx * m + 4 + bytes + 1;
-        if (mlen64 > DAEMON_MAX_FRAME) die_daemon("transaction too large for one request");
+        if (mlen64 > MAX_FRAME) die_daemon("transaction too large for one request");
         size_t mlen = (size_t)mlen64, rl;
         u8 *f = (u8 *)malloc(4 + mlen), *a = (u8 *)malloc((6 * 4 + 32 + 2 * 8 + 4 * 4) * m + bytes + 1);
         if (!f || !a) die("malloc", -3);
@@ -397,11 +399,8 @@ bool check_tx_sig(const struct bitcoin_tx *tx, size_t input_num, const u8 *redee
         fprintf(stderr, "cln_sigverify: check_tx_sig: input %zu of %zu\n", input_num, w->num_inputs);
         abort();
     }
-    size_t script_len;
+    size_t script_len = tal_len(script, "check_tx_sig: no tal_bytelen (cln_sigverify_set_tx_hooks)");
     uint64_t amount;
-    if (g_bytelen) script_len = script ? g_bytelen(script) : 0;
-    else if (tal_bytelen) script_len = script ? tal_bytelen(script) : 0;
-    else die("check_tx_sig: no tal_bytelen (cln_sigverify_set_tx_hooks)", -4);
     if (g_input_sat) amount = g_input_sat(tx, input_num);
     else if (psbt_input_get_amount) amount = psbt_input_get_amount(tx->psbt, input_num).satoshis;
     else die("check_tx_sig: no psbt_input_get_amount (cln_sigverify_set_tx_hooks)", -4);
@@ -491,7 +490,7 @@ static int remote_bolt12(const char *messagename, const char *fieldname, const u
     u8 *r = roundtrip(f, mlen, id, &rl);
     struct sigverifyd_bolt12_reply b;
     if (!fromwire_sigverifyd_bolt12_reply(r, rl, &b) || b.n != 1) die_daemon("malformed bolt12 reply");
-    int st = b.status[0] == 255 ? -1 : b.status[0];
+    int st = status_from_wire(b.status[0]);
     free(r);
     free(f);
     return st;
@@ -499,11 +498,8 @@ static int remote_bolt12(const char *messagename, const char *fieldname, const u
 
 bool bolt12_check_signature(const struct tlv_field *fields, const char *messagename, const char *fieldname,
                             const struct pubkey *key, const struct bip340sig *sig) {
-    size_t bytes;
-    if (g_bytelen) bytes = fields ? g_bytelen(fields) : 0;
-    else if (tal_bytelen) bytes = fields ? tal_bytelen(fields) : 0;
-    else die("bolt12_check_signature: no tal_bytelen (cln_sigverify_set_tx_hooks)", -4);
-    size_t nf = bytes / sizeof(struct tlv_field), total = 0;
+    size_t nf = tal_len(fields, "bolt12_check_signature: no tal_bytelen (cln_sigverify_set_tx_hooks)") / sizeof(struct tlv_field);
+    size_t total = 0;
     for (size_t i = 0; i < nf; i++) total += 18 + fields[i].length;
     if (total > 0xffffffffu) die("bolt12_check_signature: stream longer than 4 GiB", -4);
     u8 *blob = (u8 *)malloc(total ? total : 1);
@@ -587,7 +583,7 @@ void check_tx_sigs_bip143_batch(const void *sv_tx_array, const u8 *scripts, size
     free(buf);
 }
 
-/* gossip messages through sigverifyd_gossip, in requests of at most 65536 messages and 64 MiB; status 255 -> -1 */
+/* gossip messages through sigverifyd_gossip, in requests of at most 65536 messages and 64 MiB */
 static void remote_gossip(const u8 *blob, const uint32_t *len, size_t n, const u8 *cu_signers33, int *status) {
     size_t s = 0, bo = 0;
     while (s < n) {
@@ -603,11 +599,31 @@ static void remote_gossip(const u8 *blob, const uint32_t *len, size_t n, const u
         u8 *r = roundtrip(f, mlen, id, &rl);
         struct sigverifyd_gossip_reply g;
         if (!fromwire_sigverifyd_gossip_reply(r, rl, &g) || g.n != m) die_daemon("malformed gossip reply");
-        for (size_t i = 0; i < m; i++) status[s + i] = g.status[i] == 255 ? -1 : g.status[i];
+        for (size_t i = 0; i < m; i++) status[s + i] = status_from_wire(g.status[i]);
         free(r); free(f); free(lens); free(sg);
         s += m;
         bo += bytes;
     }
+}
+
+/* the n messages back to back in one blob (returned, with its length in *total), their offsets and 32-bit lengths in *off
+ * and *len; the caller frees all three */
+static u8 *concat_msgs(const u8 *const *msgs, const size_t *lens, size_t n, size_t *total, uint64_t **off, uint32_t **len) {
+    size_t t = 0;
+    for (size_t i = 0; i < n; i++) t += lens[i];
+    u8 *blob = (u8 *)malloc(t ? t : 1);
+    *off = (uint64_t *)malloc(n * sizeof(uint64_t));
+    *len = (uint32_t *)malloc(n * sizeof(uint32_t));
+    if (!blob || !*off || !*len) die("malloc", -3);
+    *total = t;
+    t = 0;
+    for (size_t i = 0; i < n; i++) {
+        (*off)[i] = t;
+        (*len)[i] = (uint32_t)lens[i];
+        memcpy(blob + t, msgs[i], lens[i]);
+        t += lens[i];
+    }
+    return blob;
 }
 
 /* ---- gossip: the raw wire messages go to the device as one blob; the DEVICE slices them the way
@@ -615,19 +631,10 @@ static void remote_gossip(const u8 *blob, const uint32_t *len, size_t n, const u
 static void gossip_batch(const u8 *const *msgs, const size_t *lens, size_t n, const struct node_id *signers,
                          uint16_t want_type, int *status) {
     if (n == 0) return;
-    size_t total = 0;
-    for (size_t i = 0; i < n; i++) total += lens[i];
-    u8 *blob = (u8 *)malloc(total ? total : 1);
-    uint64_t *off = (uint64_t *)malloc(n * sizeof(uint64_t));
-    uint32_t *len = (uint32_t *)malloc(n * sizeof(uint32_t));
-    if (!blob || !off || !len) die("malloc", -3);
-    size_t t = 0;
-    for (size_t i = 0; i < n; i++) {
-        off[i] = t;
-        len[i] = (uint32_t)lens[i];
-        memcpy(blob + t, msgs[i], lens[i]);
-        t += lens[i];
-    }
+    uint64_t *off;
+    uint32_t *len;
+    size_t total;
+    u8 *blob = concat_msgs(msgs, lens, n, &total, &off, &len);
     if (client()) {
         remote_gossip(blob, len, n, signers ? signers[0].k : NULL, status);
     } else {
@@ -650,12 +657,11 @@ void sigcheck_channel_update_batch(const u8 *const *msgs, const size_t *lens, co
     gossip_batch(msgs, lens, n, signers, 258, status); /* struct node_id is exactly 33 bytes: signers[] is the packed array */
 }
 
-/* a burst through ONE sigverifyd_gossip_burst request: updates resolve against the whole batch, so it is never split;
- * statuses 255..252 -> -1..-4 */
+/* a burst through ONE sigverifyd_gossip_burst request: updates resolve against the whole batch, so it is never split */
 static void remote_gossip_burst(const u8 *chain_hash32, const u8 *blob, size_t bytes, const size_t *len, size_t n,
                                 const u8 *signer_kind, const u8 *signers33, int *status) {
     uint64_t mlen64 = 2 + 8 + 32 + 4 + (uint64_t)n * (4 + 1 + 33) + 4 + bytes;
-    if (n > (1u << 20) || bytes > 0xffffffffu || mlen64 > DAEMON_MAX_FRAME) die_daemon("gossip burst too large for one request");
+    if (n > MAX_ITEMS || bytes > 0xffffffffu || mlen64 > MAX_FRAME) die_daemon("gossip burst too large for one request");
     size_t mlen = (size_t)mlen64, rl;
     u8 *f = (u8 *)malloc(4 + mlen), *lens = (u8 *)malloc(4 * n + 1), *kinds = (u8 *)calloc(n + 1, 1), *sg = (u8 *)calloc(n + 1, 33);
     if (!f || !lens || !kinds || !sg) die("malloc", -3);
@@ -667,26 +673,17 @@ static void remote_gossip_burst(const u8 *chain_hash32, const u8 *blob, size_t b
     u8 *r = roundtrip(f, mlen, id, &rl);
     struct sigverifyd_gossip_burst_reply g;
     if (!fromwire_sigverifyd_gossip_burst_reply(r, rl, &g) || g.n != n) die_daemon("malformed gossip burst reply");
-    for (size_t i = 0; i < n; i++) status[i] = g.status[i] >= 252 ? (int)g.status[i] - 256 : g.status[i];
+    for (size_t i = 0; i < n; i++) status[i] = status_from_wire(g.status[i]);
     free(r); free(f); free(lens); free(kinds); free(sg);
 }
 
 void sigcheck_gossip_batch(const u8 *chain_hash32, const u8 *const *msgs, const size_t *lens, size_t n, const u8 *signer_kind,
                            const struct node_id *signers, int *status) {
     if (n == 0) return;
-    size_t total = 0;
-    for (size_t i = 0; i < n; i++) total += lens[i];
-    u8 *blob = (u8 *)malloc(total ? total : 1);
-    uint64_t *off = (uint64_t *)malloc(n * sizeof(uint64_t));
-    uint32_t *len = (uint32_t *)malloc(n * sizeof(uint32_t));
-    if (!blob || !off || !len) die("malloc", -3);
-    size_t t = 0;
-    for (size_t i = 0; i < n; i++) {
-        off[i] = t;
-        len[i] = (uint32_t)lens[i];
-        memcpy(blob + t, msgs[i], lens[i]);
-        t += lens[i];
-    }
+    uint64_t *off;
+    uint32_t *len;
+    size_t total;
+    u8 *blob = concat_msgs(msgs, lens, n, &total, &off, &len);
     if (client()) {
         remote_gossip_burst(chain_hash32, blob, total, lens, n, signer_kind, signers ? signers[0].k : NULL, status);
     } else {

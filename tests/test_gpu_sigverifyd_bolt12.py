@@ -10,14 +10,14 @@ import socket
 import subprocess
 import sys
 import threading
-import time
 
 import numpy as np
 import pytest
 
-from lightning_b200 import build
 from lightning_b200 import sigverifyd_wire as W
 from tests import bolt12, ecc
+from tests.sigverifyd_daemon import connect as _connect
+from tests.sigverifyd_daemon import daemon  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -26,34 +26,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 @pytest.fixture(scope="module")
 def fx():
     return bolt12.load_fixture()
-
-
-@pytest.fixture
-def daemon(tmp_path):
-    """a fresh cln_sigverifyd on a socket under tmp_path; stopped (killed if need be) however the test ends"""
-    sock_path = str(tmp_path / "sv.sock")
-    proc = subprocess.Popen([build.DAEMON, sock_path, "0"], stderr=subprocess.PIPE)
-    try:
-        for _ in range(600):
-            if os.path.exists(sock_path) or proc.poll() is not None:
-                break
-            time.sleep(0.1)
-        assert os.path.exists(sock_path), "daemon did not come up"
-        yield sock_path
-    finally:
-        proc.terminate()
-        try:
-            proc.wait(timeout=10)
-        except subprocess.TimeoutExpired:
-            proc.kill()
-            proc.wait(timeout=10)
-
-
-def _connect(path):
-    c = socket.socket(socket.AF_UNIX, socket.SOCK_STREAM)
-    c.settimeout(120)
-    c.connect(path)
-    return c
 
 
 def _bolt12_request(fx, rid, ni, items, want):

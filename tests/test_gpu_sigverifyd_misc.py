@@ -7,18 +7,18 @@ import hashlib
 import json
 import os
 import resource
-import socket
 import subprocess
 import sys
 import threading
-import time
 
 import numpy as np
 import pytest
 
-from lightning_b200 import build
 from lightning_b200 import sigverifyd_wire as W
 from tests import ecc
+from tests.sigverifyd_daemon import connect as _connect
+from tests.sigverifyd_daemon import daemon  # noqa: F401  (fixture)
+from tests.sigverifyd_daemon import stats as _stats
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -28,43 +28,6 @@ BOUNDARIES = [0, 1, 55, 56, 63, 64, 119, 120, 174]  # every SHA-256 padding boun
 
 def _sha256d(b):
     return hashlib.sha256(hashlib.sha256(b).digest()).digest()
-
-
-@pytest.fixture
-def daemon(tmp_path):
-    """a fresh cln_sigverifyd on a socket under tmp_path; stopped (killed if need be) however the test ends"""
-    sock_path = str(tmp_path / "sv.sock")
-    proc = subprocess.Popen([build.DAEMON, sock_path, "0"], stderr=subprocess.PIPE)
-    try:
-        for _ in range(600):
-            if os.path.exists(sock_path) or proc.poll() is not None:
-                break
-            time.sleep(0.1)
-        assert os.path.exists(sock_path), "daemon did not come up"
-        yield sock_path
-    finally:
-        proc.terminate()
-        try:
-            proc.wait(timeout=10)
-        except subprocess.TimeoutExpired:
-            proc.kill()
-            proc.wait(timeout=10)
-
-
-def _connect(path):
-    c = socket.socket(socket.AF_UNIX, socket.SOCK_STREAM)
-    c.settimeout(120)
-    c.connect(path)
-    return c
-
-
-def _stats(path):
-    c = _connect(path)
-    c.sendall(W.encode("sigverifyd_stats", req_id=77))
-    name, st = W.read_msg(c)
-    c.close()
-    assert name == "sigverifyd_stats_reply"
-    return st
 
 
 def _golden_keys():

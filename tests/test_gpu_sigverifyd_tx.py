@@ -7,61 +7,24 @@ import ctypes
 import json
 import os
 import resource
-import socket
 import subprocess
 import sys
 import threading
-import time
 
 import numpy as np
 import pytest
 
 import lightning_b200 as L
-from lightning_b200 import build
 from lightning_b200 import sigverifyd_wire as W
 from tests import bolt12, txsig
+from tests.sigverifyd_daemon import connect as _connect
+from tests.sigverifyd_daemon import daemon  # noqa: F401  (fixture)
+from tests.sigverifyd_daemon import stats as _stats
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden")
 SKS = [bytes([0x11 + s]) * 32 for s in range(2)]
-
-
-@pytest.fixture
-def daemon(tmp_path):
-    """a fresh cln_sigverifyd on a socket under tmp_path; stopped (killed if need be) however the test ends"""
-    sock_path = str(tmp_path / "sv.sock")
-    proc = subprocess.Popen([build.DAEMON, sock_path, "0"], stderr=subprocess.PIPE)
-    try:
-        for _ in range(600):
-            if os.path.exists(sock_path) or proc.poll() is not None:
-                break
-            time.sleep(0.1)
-        assert os.path.exists(sock_path), "daemon did not come up"
-        yield sock_path
-    finally:
-        proc.terminate()
-        try:
-            proc.wait(timeout=10)
-        except subprocess.TimeoutExpired:
-            proc.kill()
-            proc.wait(timeout=10)
-
-
-def _connect(path):
-    c = socket.socket(socket.AF_UNIX, socket.SOCK_STREAM)
-    c.settimeout(120)
-    c.connect(path)
-    return c
-
-
-def _stats(path):
-    c = _connect(path)
-    c.sendall(W.encode("sigverifyd_stats", req_id=77))
-    name, st = W.read_msg(c)
-    c.close()
-    assert name == "sigverifyd_stats_reply"
-    return st
 
 
 @pytest.fixture(scope="module")
@@ -290,21 +253,9 @@ CLIENT = r"""
 import ctypes, json, sys
 import numpy as np
 from lightning_b200 import engine
+from tests.txsig import WallyIn as In, WallyOut as Out, WallyTx as WTx, BitcoinTx as BTx
 lib = ctypes.CDLL(engine.LIB_PATH)
 vp, sz = ctypes.c_void_p, ctypes.c_size_t
-class In(ctypes.Structure):
-    _fields_ = [("txhash", ctypes.c_uint8 * 32), ("index", ctypes.c_uint32), ("sequence", ctypes.c_uint32), ("script", vp),
-                ("script_len", sz), ("witness", vp), ("features", ctypes.c_uint8), ("blinding_nonce", ctypes.c_uint8 * 32),
-                ("entropy", ctypes.c_uint8 * 32)] + [(f, t) for f in ("issuance_amount", "inflation_keys",
-                "issuance_amount_rangeproof", "inflation_keys_rangeproof") for t in (vp, sz)] + [("pegin_witness", vp)]
-class Out(ctypes.Structure):
-    _fields_ = [("satoshi", ctypes.c_uint64), ("script", vp), ("script_len", sz), ("features", ctypes.c_uint8)] + \
-               [(f + s, t) for f in ("asset", "value", "nonce", "surjectionproof", "rangeproof") for s, t in (("", vp), ("_len", sz))]
-class WTx(ctypes.Structure):
-    _fields_ = [("version", ctypes.c_uint32), ("locktime", ctypes.c_uint32), ("inputs", vp), ("num_inputs", sz),
-                ("inputs_allocation_len", sz), ("outputs", vp), ("num_outputs", sz), ("outputs_allocation_len", sz)]
-class BTx(ctypes.Structure):
-    _fields_ = [("wtx", ctypes.POINTER(WTx)), ("chainparams", vp), ("psbt", vp)]
 lib.check_tx_sig.restype = ctypes.c_bool
 lib.check_tx_sig.argtypes = [vp, sz, vp, vp, vp, vp]
 lib.check_tx_sigs_bip143_batch.argtypes = [vp, vp, sz, vp, vp, sz, vp]

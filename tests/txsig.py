@@ -1,6 +1,8 @@
 """Transactions for the sigverifyd_tx tests and tools/measure_sigverifyd_tx.py: multi-input / multi-output sv_tx records
 (the shape check_tx_sig hands over for a commitment transaction), a commitment_signed-shaped workload, signing through
 the device's own sighash, and the sigverifyd_tx request for a set of records."""
+import ctypes
+
 import numpy as np
 
 from lightning_b200 import SvTx
@@ -9,6 +11,29 @@ from tests import ecc, util
 
 SV_TX_OUTPUTS_SERIALIZED, SV_TX_INPUTS_SERIALIZED, SV_TX_OUTPUTS_ZERO = 1, 2, 4
 U32_FIELDS = ["version", "locktime", "sequence", "sighash_type", "prev_index", "flags"]
+_vp, _sz = ctypes.c_void_p, ctypes.c_size_t
+
+
+# the stand-alone libwally structs check_tx_sig reads (include/cln_dropin.h), for driving the drop-in through ctypes
+class WallyIn(ctypes.Structure):
+    _fields_ = [("txhash", ctypes.c_uint8 * 32), ("index", ctypes.c_uint32), ("sequence", ctypes.c_uint32), ("script", _vp),
+                ("script_len", _sz), ("witness", _vp), ("features", ctypes.c_uint8), ("blinding_nonce", ctypes.c_uint8 * 32),
+                ("entropy", ctypes.c_uint8 * 32)] + [(f, t) for f in ("issuance_amount", "inflation_keys",
+                "issuance_amount_rangeproof", "inflation_keys_rangeproof") for t in (_vp, _sz)] + [("pegin_witness", _vp)]
+
+
+class WallyOut(ctypes.Structure):
+    _fields_ = [("satoshi", ctypes.c_uint64), ("script", _vp), ("script_len", _sz), ("features", ctypes.c_uint8)] + \
+               [(f + s, t) for f in ("asset", "value", "nonce", "surjectionproof", "rangeproof") for s, t in (("", _vp), ("_len", _sz))]
+
+
+class WallyTx(ctypes.Structure):
+    _fields_ = [("version", ctypes.c_uint32), ("locktime", ctypes.c_uint32), ("inputs", _vp), ("num_inputs", _sz),
+                ("inputs_allocation_len", _sz), ("outputs", _vp), ("num_outputs", _sz), ("outputs_allocation_len", _sz)]
+
+
+class BitcoinTx(ctypes.Structure):
+    _fields_ = [("wtx", ctypes.POINTER(WallyTx)), ("chainparams", _vp), ("psbt", _vp)]
 
 
 def _output(rng, amount=None):
