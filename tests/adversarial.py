@@ -109,6 +109,73 @@ def cases(limit=None):
     return tuple(np.stack(c) for c in cols)
 
 
+BETA = 0x7AE96A2B657C07106E64479EAC3434E99CF0497512F58995C1396C28719501EE  # lambda*(x, y) = (beta*x, y)
+
+
+def _schnorr_sign_nonce(d0, k0, msg32):
+    """BIP-340 signature of msg32 under secret d0 with the nonce k0 chosen by the caller (both negated as BIP-340 requires
+    when their point has odd y) -> (sig64, xonly32).  k0 = d0 gives R = P."""
+    from tests import ecc
+    x, y = ecc.base_mult(d0)
+    d = d0 if y % 2 == 0 else N - d0
+    rx, ry = (x, y) if k0 == d0 else ecc.base_mult(k0)
+    k = k0 if ry % 2 == 0 else N - k0
+    px = x.to_bytes(32, "big")
+    e = int.from_bytes(ecc.tagged_hash("BIP0340/challenge", rx.to_bytes(32, "big") + px + bytes(msg32)), "big") % N
+    return rx.to_bytes(32, "big") + ((k + e * d) % N).to_bytes(32, "big"), px
+
+
+def bip340_collision_groups(size=1024):
+    """Four all-valid groups of `size` BIP-340 signatures whose points meet inside the buckets of batch verification
+    (batch.cuh: every R_i, lambda*R_i, P_i, lambda*P_i enters a bucket; equal points there need a doubling, opposite ones
+    give infinity):
+      copies  one signature repeated
+      onekey  one key, a fresh message and nonce per signature
+      r_eq_p  nonce = key, so R = P
+      r_eq_lp nonce = lambda*key, so R = lambda*P = (beta*x, y): even y, since P has it
+    Returns [(name, msg (size, 32), xonly (size, 32), sig (size, 64))], deterministic."""
+    import hashlib
+    h = lambda *a: int.from_bytes(hashlib.sha256(b"/".join(str(v).encode() for v in a)).digest(), "big") % N or 1
+    m32 = lambda *a: hashlib.sha256(b"msg/" + b"/".join(str(v).encode() for v in a)).digest()
+    out = []
+
+    def pack(name, rows):
+        msg = np.array([np.frombuffer(m, np.uint8) for m, _, _ in rows])
+        key = np.array([np.frombuffer(k, np.uint8) for _, k, _ in rows])
+        sig = np.array([np.frombuffer(s, np.uint8) for _, _, s in rows])
+        out.append((name, msg, key, sig))
+    s, px = _schnorr_sign_nonce(h("copies"), h("copies", "k"), m32("copies"))
+    pack("copies", [(m32("copies"), px, s)] * size)
+    rows = []
+    for i in range(size):
+        s, px = _schnorr_sign_nonce(h("onekey"), h("onekey", i), m32("onekey", i))
+        rows.append((m32("onekey", i), px, s))
+    pack("onekey", rows)
+    rows = []
+    for i in range(size):
+        d = h("r_eq_p", i)
+        s, px = _schnorr_sign_nonce(d, d, m32("r_eq_p", i))
+        assert s[:32] == px
+        rows.append((m32("r_eq_p", i), px, s))
+    pack("r_eq_p", rows)
+    rows = []
+    for i in range(size):
+        d = h("r_eq_lp", i)
+        s, px = _schnorr_sign_nonce(d, LAMBDA * d % N, m32("r_eq_lp", i))
+        assert int.from_bytes(s[:32], "big") == BETA * int.from_bytes(px, "big") % P
+        rows.append((m32("r_eq_lp", i), px, s))
+    pack("r_eq_lp", rows)
+    return out
+
+
+def by_key():
+    """The committed fixture grouped by signing key: [(pub33, pubxy, indices)], one entry per key."""
+    msg, pub33, pubxy, sig = load()
+    keys, first, inv = np.unique(pub33, axis=0, return_index=True, return_inverse=True)
+    inv = inv.reshape(-1)
+    return [(pub33[f], pubxy[f], np.nonzero(inv == g)[0]) for g, f in enumerate(first)]
+
+
 FIXTURE = __import__("os").path.join(__import__("os").path.dirname(__import__("os").path.abspath(__file__)), "golden", "adversarial.npz")
 
 

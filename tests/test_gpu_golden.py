@@ -351,22 +351,38 @@ def test_htlc_loop_device_side_bip143(engine, ref, cln):
 
 def test_host_api_chunking_and_pipelining(engine):
     """sv_verify_host above its internal chunk size (2^21) and with slice pipelining: 2.2 M synthesised signatures
-    copied to (pageable) host memory, a few corrupted, verified through the host-buffer API."""
+    copied to (pageable) host memory, a few corrupted, verified through the host-buffer API.  Then x||y keys and BIP-340
+    at 16 waves + 999: four slices alternating between the two compute streams, the first one with the ragged wave."""
     import torch
+
+    def synth(kind, n, seed):
+        msg = torch.empty((n, 32), dtype=torch.uint8, device="cuda")
+        key = torch.empty((n, (33, 64, 32)[kind]), dtype=torch.uint8, device="cuda")
+        sig = torch.empty((n, 64), dtype=torch.uint8, device="cuda")
+        torch.cuda.synchronize()
+        engine.synth_device(kind, seed, n, msg.data_ptr(), key.data_ptr(), sig.data_ptr())
+        engine.sync()
+        return msg.cpu().numpy(), key.cpu().numpy(), sig.cpu().numpy()
     n = 2_200_000
-    msg = torch.empty((n, 32), dtype=torch.uint8, device="cuda")
-    key = torch.empty((n, 33), dtype=torch.uint8, device="cuda")
-    sig = torch.empty((n, 64), dtype=torch.uint8, device="cuda")
-    torch.cuda.synchronize()
-    engine.synth_device(0, 4242, n, msg.data_ptr(), key.data_ptr(), sig.data_ptr())
-    engine.sync()
-    m, k, s = msg.cpu().numpy(), key.cpu().numpy(), sig.cpu().numpy()
+    m, k, s = synth(0, n, 4242)
     bad = np.array([0, 1, 151551, 151552, 757759, 757760, 2097151, 2097152, 2097153, n - 1])
     m[bad, 9] ^= 0x40
     got = engine.verify(0, m, k, s)
     want = np.ones(n, np.uint8)
     want[bad] = 0
     assert np.array_equal(got, want)
+    info = engine.info()
+    wave = info["main_grid"] * info["main_block"]
+    n = 16 * wave + 999
+    first = wave + n % wave  # the first slice: sv_verify_host's slicing
+    for kind in (1, 2):
+        m, k, s = synth(kind, n, 4243 + kind)
+        bad = np.array([0, first - 1, first, first + 6 * wave - 1, first + 6 * wave, first + 12 * wave, n - 1])
+        m[bad, 9] ^= 0x40
+        got = engine.verify(kind, m, k, s)
+        want = np.ones(n, np.uint8)
+        want[bad] = 0
+        assert np.array_equal(got, want), (kind, np.nonzero(got != want)[0][:5])
 
 
 def test_samekey_batch(engine, ref):

@@ -213,6 +213,47 @@ def test_samekey_path(emul, ref):
     assert not out.any()
 
 
+def test_samekey_path_adversarial_scalars_per_key(emul):
+    """The crafted signatures of tests/adversarial.py (ladder and comb driven into their exceptional branches), grouped by
+    key, through the shared-key verification (host build of verify_curve_side_shared), both key forms: every one is valid;
+    with the last message byte flipped the verdicts equal the per-item verification's (emul_verify_batch)."""
+    msg, _, _, sig = adversarial.load()
+    groups = adversarial.by_key()
+    assert len(groups) == 9
+    for pub33, pubxy, idx in groups:
+        m, s = np.ascontiguousarray(msg[idx]), np.ascontiguousarray(sig[idx])
+        m2 = m.copy()
+        m2[:, 31] ^= 1
+        want2 = emul_verify(emul, 0, m2, np.tile(pub33, (len(idx), 1)), s)
+        for kind, key in ((0, pub33), (1, pubxy)):
+            for mm, want in ((m, np.ones(len(idx), np.uint8)), (m2, want2)):
+                out = np.full(len(idx), 7, np.uint8)
+                emul.emul_verify_samekey(kind, P(np.ascontiguousarray(key)), P(mm), P(s), ctypes.c_size_t(len(idx)), P(out))
+                assert np.array_equal(out, want), (bytes(pub33).hex(), kind, np.nonzero(out != want)[0][:5])
+
+
+def test_bip340_batch_group_equations_with_colliding_points(emul):
+    """BIP-340 batch verification (host build, straightforward window sums) on groups whose points meet inside buckets
+    (adversarial.bip340_collision_groups: copies of one signature, one key, R = P, R = lambda*P): each group's equation
+    holds whatever the seed, and one wrong signature fails its group."""
+    for name, m, k, s in adversarial.bip340_collision_groups():
+        n = m.shape[0]
+        assert emul_verify(emul, 2, m, k, s).all(), name
+
+        def run(mm, seed):
+            ok, gok = np.zeros(n, np.uint8), np.zeros(1, np.uint8)
+            sd = np.frombuffer(seed, dtype=np.uint8).copy()
+            emul.emul_schnorr_batch(P(mm), P(k), P(s), ctypes.c_size_t(n), P(sd), P(ok), P(gok))
+            return ok, gok[0]
+        for seed in (bytes(32), bytes(range(32))):
+            ok, gok = run(m, seed)
+            assert ok.all() and gok == 1, (name, seed[:2])
+        m3 = m.copy()
+        m3[n // 2, 0] ^= 1
+        ok, gok = run(m3, bytes(range(32)))
+        assert ok.all() and gok == 0, name
+
+
 def test_mutation_differential(emul, ref):
     """~3,000 structured mutations (boundary values of r, s, x, m; swapped/negated fields; random flips) of valid
     triples: the host build of the kernel code and the reference must agree on every verdict, for all three kinds."""
