@@ -164,7 +164,8 @@ int sv_set_l2_policy(sv_ctx *ctx, int on);
  *      a group whose equation fails are re-verified one by one, so every verdict is the one sv_verify_host(SV_KIND_SCHNORR)
  *      gives, up to the 2^-127 chance that random a_i hide a bad signature.  Meant for batches that are almost all valid
  *      (a bad signature costs its whole group the fast path).  seed32: 32 bytes the signers could not predict (NULL: taken
- *      from getrandom()).  groups_total / groups_failed (optional) report how the batch went. ---- */
+ *      from getrandom()); a seed the signers can learn lets them make invalid signatures pass, as
+ *      tests/test_gpu_batch_rlc.py shows.  groups_total / groups_failed (optional) report how the batch went. ---- */
 int sv_verify_schnorr_batch_host(sv_ctx *ctx, const uint8_t *msg32, const uint8_t *xonly32, const uint8_t *sig64, size_t n,
                                  const uint8_t *seed32, uint8_t *verdicts, uint32_t *groups_total, uint32_t *groups_failed);
 

@@ -168,6 +168,92 @@ def bip340_collision_groups(size=1024):
     return out
 
 
+# ---- soundness of BIP-340 batch verification: invalid signatures that cancel in a group equation -------------------------
+# A group of the batch (batch.cuh) passes iff  sum a_i*R_i + sum (a_i*e_i)*P_i - (sum a_i*s_i)*G == infinity.  A BIP-340
+# signature has exactly one valid s for its (r, P, m), so moving s_i by d_i makes it invalid and adds -a_i*d_i*G to its
+# group's sum: a group whose only damage is such shifts passes iff sum a_i*d_i == 0 (mod n).  The random coefficients a_i
+# are what keeps invalid signatures from cancelling; the helpers below build signatures that cancel when a_i are weaker
+# than they should be (all equal, predictable, or derived from the wrong index).
+
+BATCH_GROUP = 1024  # SV_SB_GROUP: signatures per group equation
+
+
+def batch_coefficient(seed32, i):
+    """a_i of signature i (its index in the WHOLE batch) as sb_prepare (batch.cuh) derives it: W0..W7 = SHA-256(seed32 ||
+    LE64(i)) as big-endian 32-bit words, alpha = (W1 << 32 | W0) | 1, beta = W3 << 32 | W2, a_i = alpha + beta*lambda mod n."""
+    import hashlib
+    import struct
+    w = struct.unpack(">8I", hashlib.sha256(bytes(seed32) + int(i).to_bytes(8, "little")).digest())
+    return (((w[1] << 32 | w[0]) | 1) + (w[3] << 32 | w[2]) * LAMBDA) % N
+
+
+def _shift_s(sig, i, d):
+    s = int.from_bytes(bytes(sig[i, 32:]), "big")
+    sig[i, 32:] = np.frombuffer(((s + d) % N).to_bytes(32, "big"), np.uint8)
+
+
+def forge_pair(sig, i, j, seed32, d=1):
+    """Copy of the (n, 64) signatures with s_i += d*a_j and s_j -= d*a_i (mod n), a = batch_coefficient(seed32, .): two
+    invalid signatures whose shifts cancel, -a_i*d*a_j + a_j*d*a_i = 0, in a batch verified with seed32 when i and j share
+    a group."""
+    out = sig.copy()
+    _shift_s(out, i, d * batch_coefficient(seed32, j))
+    _shift_s(out, j, -d * batch_coefficient(seed32, i))
+    return out
+
+
+def cancel_pair(sig, i, j, d=1):
+    """Copy of the (n, 64) signatures with s_i += d and s_j -= d (mod n): invalid signatures that cancel whenever a_i = a_j."""
+    out = sig.copy()
+    _shift_s(out, i, d)
+    _shift_s(out, j, -d)
+    return out
+
+
+def s_shifts(sig0, sig1):
+    """{i: (s1_i - s0_i) mod n} over the rows where two (n, 64) signature arrays differ in s only."""
+    rows = np.nonzero((sig0 != sig1).any(axis=1))[0]
+    out = {}
+    for i in rows:
+        assert np.array_equal(sig0[i, :32], sig1[i, :32]), "r differs: not an s shift"
+        out[int(i)] = (int.from_bytes(bytes(sig1[i, 32:]), "big") - int.from_bytes(bytes(sig0[i, 32:]), "big")) % N
+    return out
+
+
+def predict_groups(n, seed32, shifts):
+    """Per-group verdicts of a batch of n signatures, valid but for the s shifts {i: d_i}, verified with seed32: group g
+    passes iff sum over its members of a_i*d_i == 0 (mod n)."""
+    acc = [0] * ((n + BATCH_GROUP - 1) // BATCH_GROUP)
+    for i, d in shifts.items():
+        acc[i // BATCH_GROUP] += batch_coefficient(seed32, i) * d
+    return [int(a % N == 0) for a in acc]
+
+
+def swap_nonce_pair(msg, xonly, sig, i, j):
+    """Copies of (msg (n, 32), xonly (n, 32), sig (n, 64)) with items i and j replaced by two signatures under fresh keys,
+    each made with the OTHER one's nonce point: item i is (r_j, k_i + H(r_j || P_i || m_i)*d_i), likewise item j.  Item i
+    is off by R_i - R_j and item j by R_j - R_i, so together they add (a_i - a_j)*(R_i - R_j) to their group's sum:
+    nothing when a_i = a_j.  Deterministic in (i, j)."""
+    import hashlib
+    from tests import ecc
+    h = lambda *a: int.from_bytes(hashlib.sha256(b"swap/" + b"/".join(str(v).encode() for v in a)).digest(), "big") % N or 1
+    side = []
+    for t in (i, j):
+        d0, k0 = h(i, j, t, "key"), h(i, j, t, "nonce")
+        x, y = ecc.base_mult(d0)
+        rx, ry = ecc.base_mult(k0)
+        m = hashlib.sha256(b"swap/msg/%d/%d/%d" % (i, j, t)).digest()
+        side.append((d0 if y % 2 == 0 else N - d0, k0 if ry % 2 == 0 else N - k0, x.to_bytes(32, "big"), rx.to_bytes(32, "big"), m))
+    msg, xonly, sig = msg.copy(), xonly.copy(), sig.copy()
+    for t, (d, k, px, _, m), other in ((i, side[0], side[1]), (j, side[1], side[0])):
+        r = other[3]
+        e = int.from_bytes(ecc.tagged_hash("BIP0340/challenge", r + px + m), "big") % N
+        msg[t] = np.frombuffer(m, np.uint8)
+        xonly[t] = np.frombuffer(px, np.uint8)
+        sig[t] = np.frombuffer(r + ((k + e * d) % N).to_bytes(32, "big"), np.uint8)
+    return msg, xonly, sig
+
+
 def by_key():
     """The committed fixture grouped by signing key: [(pub33, pubxy, indices)], one entry per key."""
     msg, pub33, pubxy, sig = load()
