@@ -28,6 +28,9 @@
  *                                           gates gossipd/gossmap_manage.c:659-670, :1048-1051, sigcheck_*, and the
  *                                           pending map that gives a channel_update its signer (:695-703,
  *                                           :1060-1097), or the source peer's private-update check (:1099-1110)
+ *   sv_verify_gossip_store_host(...)        gossmap's map_catchup over a whole gossip_store (common/gossmap.c:815-937:
+ *                                           record walk, crc32c) plus every signature it never checks, with the
+ *                                           signer its channel table gives
  *   sv_sha256d_host(...)                    sha256_double()              bitcoin/shadouble.c:7-11
  *   sv_pubkey_parse_host(...)               pubkey_from_der()            bitcoin/pubkey.c:14-24
  *   sv_enqueue_* / sv_flush                 the deferral queue a batching caller (gossipd ingest,
@@ -152,6 +155,62 @@ int sv_verify_gossip_burst_host(sv_ctx *ctx, const uint8_t chain_hash32[32], con
                                 const uint64_t *msg_off, const uint32_t *msg_len, size_t n_msgs, const uint8_t *signer_kind,
                                 const uint8_t *signers33, int *status);
 unsigned sv_last_gossip_repairs(const sv_ctx *ctx);
+
+/* ---- a whole GOSSIP_STORE (common/gossip_store.h layout: version byte, then records of a 12-byte header and a message),
+ *      audited before gossmap loads it.  gossmap's map_catchup (common/gossmap.c:815-937) trusts the store: it checks each
+ *      record's CRC-32C and no signature.  This call walks the store exactly as map_catchup does, checks every checksum it
+ *      would check, and verifies every channel_announcement, node_announcement and channel_update it would load.
+ *
+ *      Walk (host, headers only): from offset 1 while off + 12 < len.  A record without the COMPLETED flag stops it
+ *      (SV_GS_INCOMPLETE); a DELETED record is skipped unchecked (SV_GS_DELETED); a record running past the end stops it
+ *      (SV_GS_PARTIAL), as does a message under 2 bytes (SV_GS_TRUNCATED), a checksum mismatch (SV_GS_BAD_CRC: crc32c with
+ *      the header timestamp as start value), a gossip_store_ended record (SV_GS_ENDED) and a channel_announcement that
+ *      holds its channel but has no room for the amount record after it (SV_GS_NO_AMOUNT, gossmap.c:488-492).  Records of
+ *      types 4101, 4103, 4106, 4107 are SV_GS_STORE_RECORD, any other type SV_GS_UNKNOWN.  Records after a BAD_CRC or
+ *      NO_AMOUNT stop are SV_GS_NOT_REACHED and are not verified.
+ *
+ *      Messages: rec_status is what sv_verify_gossip_host reports (0, 1..4, -1).  With chain_hash32, the gates of
+ *      sv_verify_gossip_burst_host apply too (-4 node ids out of order, -3 another chain); NULL means no gates.  A
+ *      channel_update is signed by the channel gossmap holds for its scid at the update's position: the first
+ *      non-deleted channel_announcement of the scid holds it (whatever its own status, as long as it holds the fixed
+ *      layout through node_id_2), a later one is redundant and never signs, a non-deleted gossip_store_delete_chan frees
+ *      the scid for the next announcement.  The signer is node_id_1 or node_id_2 by channel_flags & 1.  An update whose
+ *      scid has no channel at its position is -2 (after -1 and -3).
+ *
+ *      rec_off / rec_type / rec_status (and rec_holder, optional): one entry per record the walk reads, in store order;
+ *      rec_holder is the header offset of the announcement holding the channel, for a channel_update and for a redundant
+ *      channel_announcement, else UINT64_MAX.  rec_capacity below sv_gossip_store_count(store, len), or a major version
+ *      other than 0 (gossmap.c:958-963): SV_ERR_ARG, nothing written.  The store is staged on the device for the call only.
+ *      On the device: the checksums (the first bad one cuts the walk), the slicing, gates, hashing and verification of
+ *      sv_verify_gossip_host, and the channel table (events sorted by scid, one thread walks each scid). ---- */
+#define SV_GS_EOF 0 /* summary.stop only: the walk reached the end of the store */
+#define SV_GS_DELETED 16
+#define SV_GS_STORE_RECORD 17
+#define SV_GS_UNKNOWN 18
+#define SV_GS_NOT_REACHED 19
+#define SV_GS_INCOMPLETE 32
+#define SV_GS_PARTIAL 33
+#define SV_GS_TRUNCATED 34
+#define SV_GS_BAD_CRC 35
+#define SV_GS_ENDED 36
+#define SV_GS_NO_AMOUNT 37
+typedef struct {
+    uint32_t version;                 /* the store's version byte */
+    int32_t stop;                     /* SV_GS_EOF or the status of the record the walk stopped at */
+    uint64_t end_offset;              /* gossmap's map_end: the offset of that record, or where the walk ran out */
+    uint64_t ended_equivalent_offset; /* stop == SV_GS_ENDED: the record's equivalent_offset */
+    uint64_t records;                 /* entries written */
+    uint64_t good, bad_signature, malformed, no_channel, wrong_chain, bad_order; /* messages: 0, 1..4, -1, -2, -3, -4 */
+    uint64_t deleted, store_records, unknown, not_reached;
+    uint64_t redundant_announcements; /* reached channel_announcements of an scid whose channel was already held */
+    uint64_t updates_without_channel; /* reached channel_updates (scid and flags present) whose scid held no channel */
+} sv_gossip_store_summary;
+size_t sv_gossip_store_count(const uint8_t *store, size_t len);
+int sv_verify_gossip_store_host(sv_ctx *ctx, const uint8_t *store, size_t len, const uint8_t *chain_hash32,
+                                uint64_t *rec_off, uint16_t *rec_type, int *rec_status, uint64_t *rec_holder,
+                                size_t rec_capacity, sv_gossip_store_summary *summary);
+/* profiling mode (sv_set_profiling): ms4 = host header walk, H2D copy of the store, checksum kernel, the rest of the call */
+int sv_get_last_gossip_store_timing(sv_ctx *ctx, float *ms4);
 
 /* L2 residency hint for the throughput kernels (default on): the G comb table and the per-thread multiples tables are
  * marked persisting through a stream access-policy window, the rest of the stream's traffic streaming.  0 switches it off

@@ -5,6 +5,7 @@ Everything is built IN-TREE, so the package and the tests run from the source tr
   tests/host_emul/libemul.so           kernel headers compiled for the host, tests only [g++]
   oracle/libsecp_port.so               the plain-C restatement oracle                 [gcc]
   oracle/_ref/libsecp_ref.so           the unmodified reference, from the Core Lightning tree at $CLN_SRC or /root/reference [gcc]
+  lightning_b200/cln_sigverifyd, cln_verify_gossip_store   the verifier subdaemon and the gossip_store audit tool [gcc]
   oracle/_ref/libcln_ref.so, libcln_bolt12.so   CLN's own plumbing and BOLT12 Merkle code from the same tree [gcc]
 """
 import os
@@ -17,6 +18,7 @@ CSRC = os.path.join(ROOT, "lightning_b200", "csrc")
 LIB = os.path.join(ROOT, "lightning_b200", "libcln_sigverify.so")
 EMUL = os.path.join(ROOT, "tests", "host_emul", "libemul.so")
 DAEMON = os.path.join(ROOT, "lightning_b200", "cln_sigverifyd")
+STORE_TOOL = os.path.join(ROOT, "lightning_b200", "cln_verify_gossip_store")
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -51,7 +53,7 @@ def build_engine(force=False, verbose=False, extra_flags=()):
     stamp = os.path.join(os.path.dirname(LIB), ".build_flags")
     flags_now = " ".join(NVCC_FLAGS + list(extra_flags))
     same_flags = os.path.exists(stamp) and open(stamp).read() == flags_now
-    if not force and same_flags and _newer(LIB, srcs) and _newer(DAEMON, srcs):
+    if not force and same_flags and _newer(LIB, srcs) and _newer(DAEMON, srcs) and _newer(STORE_TOOL, srcs):
         return LIB
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     # host side of the drop-in is plain C (as the reference's bitcoin/signature.c), compiled by gcc
@@ -81,12 +83,17 @@ def build_engine(force=False, verbose=False, extra_flags=()):
                         "-L" + os.path.dirname(LIB), "-lcln_sigverify", "-Wl,-rpath,$ORIGIN"], capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("gcc (sigverifyd.c) failed:\n" + r.stdout + r.stderr)
+    # gossip_store audit tool: plain C, links the engine
+    r = subprocess.run(["gcc"] + DAEMON_CFLAGS + [os.path.join(CSRC, "cln_verify_gossip_store.c"), "-o", STORE_TOOL,
+                        "-L" + os.path.dirname(LIB), "-lcln_sigverify", "-Wl,-rpath,$ORIGIN"], capture_output=True, text=True)
+    if r.returncode != 0:
+        raise RuntimeError("gcc (cln_verify_gossip_store.c) failed:\n" + r.stdout + r.stderr)
     open(stamp, "w").write(flags_now)
     return LIB
 
 
 def build_host_emul(force=False):
-    src = [os.path.join(ROOT, "tests", "host_emul", f) for f in ("emul.cpp", "bolt12_emul.cpp")]
+    src = [os.path.join(ROOT, "tests", "host_emul", f) for f in ("emul.cpp", "bolt12_emul.cpp", "gossip_store_emul.cpp")]
     srcs = _sources(CSRC, (".cuh",)) + src
     if not force and _newer(EMUL, srcs):
         return EMUL

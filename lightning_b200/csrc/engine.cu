@@ -23,7 +23,9 @@
 // There is no host implementation of any of the arithmetic in this library: every entry point either
 // runs the kernels or fails with an error code.
 #include <cuda_runtime.h>
+#include <cub/device/device_radix_sort.cuh>
 #include <stdio.h>
+#include <chrono>
 #include <stdlib.h>
 #include <string.h>
 #include <string>
@@ -32,6 +34,7 @@
 #include "../../include/cln_sigverify.h"
 #include "verify.cuh"
 #include "bolt12.cuh"
+#include "gossip_store.cuh"
 #include "selftest.cuh"
 #include "batch.cuh"  // constants and the host-testable stages; the kernels themselves are in batch.cu
 
@@ -625,6 +628,64 @@ __global__ void __launch_bounds__(128) k_gossip_status(const u8* blob, const u64
     status[m] = st;
 }
 
+// ---- gossip_store (gossip_store.cuh): record checksums and the channel each update is signed for ---------------------
+// k_store_crc: one thread per live record the host walk read (header offsets), slice-by-8 tables in shared memory.
+// *first_bad = the lowest entry whose checksum fails: map_catchup stops there.
+__global__ void __launch_bounds__(256) k_store_crc(const u8* store, const u64* rec_off, size_t n, u32* first_bad) {
+    __shared__ u32 tab[2048];
+    for (u32 i = threadIdx.x; i < 256; i += blockDim.x) gs_crc_fill(tab, i);
+    __syncthreads();
+    size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    u32 bad = (r < n && !gs_record_crc_ok(tab, store, rec_off[r])) ? (u32)r : 0xFFFFFFFFu;
+    bad = __reduce_min_sync(0xFFFFFFFFu, bad);
+    if ((threadIdx.x & 31) == 0 && bad != 0xFFFFFFFFu) atomicMin(first_bad, bad);
+}
+// one thread per channel event (announcement, delete_chan, update, listed by the host in store order): its scid as the
+// sort key and its own index as the value; a record too short to take part gets ok = 0
+__global__ void __launch_bounds__(256) k_store_events(const u8* store, const u64* ev_off, const u32* ev_len, const u8* ev_kind,
+                                                      size_t n, u64* key, u32* val, u8* ok) {
+    size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    const u8* p = store + ev_off[e];
+    const bool good = gs_event_ok(ev_kind[e], p, ev_len[e]);
+    key[e] = good ? gs_event_scid(ev_kind[e], p) : ~0ull;
+    val[e] = (u32)e;
+    ok[e] = good;
+}
+// After the stable sort by scid every scid's events are one run in store order.  The thread at the head of a run walks
+// it with gs_event.  holder[m] = what message m saw (an update: the announcement it is signed for; an announcement: the
+// one that already held its channel, i.e. it is redundant), GS_NONE otherwise; an update's signer (the holder's
+// node_id_1 or node_id_2 by channel_flags & 1, byte 111) goes to signers33[m].
+__global__ void __launch_bounds__(128) k_store_resolve(const u8* store, const u64* key, const u32* val, const u8* ok,
+                                                       const u8* ev_kind, const u64* ev_off, const u32* ev_msg, size_t n,
+                                                       const u64* msg_off, u32* holder, u8* signers33) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || (i > 0 && key[i - 1] == key[i])) return;
+    u32 held = GS_NONE;
+    for (size_t j = i; j < n && key[j] == key[i]; j++) {
+        const u32 e = val[j];
+        if (!ok[e]) continue;
+        const int kind = ev_kind[e];
+        const u32 h = gs_event(&held, kind, ev_msg[e]);
+        if (kind == GS_EV_DEL) continue;
+        const u32 m = ev_msg[e];
+        holder[m] = h;
+        if (kind == GS_EV_UPD && h != GS_NONE) {
+            const u8* a = store + msg_off[h];
+            const u8* kp = a + 260 + gs_be16(a + 258) + 32 + 8 + 33 * (store[ev_off[e] + 111] & 1);
+            for (int b = 0; b < 33; b++) signers33[33 * (size_t)m + b] = kp[b];
+        }
+    }
+}
+// an update whose scid holds no channel at its position: -2, once the parse (-1) and the chain gate (-3) have passed
+__global__ void __launch_bounds__(256) k_store_finish(const u8* store, const u64* msg_off, const u32* holder, size_t n,
+                                                      int* status) {
+    size_t m = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (m >= n) return;
+    const u8* p = store + msg_off[m];
+    if (p[0] == 1 && p[1] == 2 && holder[m] == GS_NONE && (status[m] == 0 || status[m] == 1)) status[m] = -2;
+}
+
 // ---- BOLT12 signatures (bolt12.cuh): the message hash of bolt12_check_signature on the device -----------------------
 // k_b12_count: one thread per stream walks its BigSize headers (bytes only): field count, or 0 if the parse fails
 __global__ void __launch_bounds__(128) k_b12_count(const u8* blob, const u64* off, const u32* len, size_t n, u32* cnt) {
@@ -1179,6 +1240,7 @@ struct sv_ctx {
     int profiling;
     cudaEvent_t ev[3];  // before prep, between prep and main, after main (profiling mode only)
     cudaEvent_t b12_ev[2];  // around the BOLT12 parse / Merkle / sighash kernels (profiling mode only)
+    float gs_ms[4];         // last sv_verify_gossip_store_host: header walk, H2D, checksums, verification (profiling mode)
     unsigned long long launches;
     std::vector<sv_queue_item> queue;
     std::string err;
@@ -1966,6 +2028,221 @@ extern "C" int sv_verify_gossip_burst_host(sv_ctx* ctx, const uint8_t chain_hash
     return gossip_run(ctx, chain_hash32, blob, blob_len, msg_off, msg_len, n_msgs, signer_kind, signers33, status);
 }
 extern "C" unsigned sv_last_gossip_repairs(const sv_ctx* ctx) { return ctx ? ctx->last_repair : 0; }
+
+// ---- a whole gossip_store: gossmap's record walk (host, headers only), every checksum, and every signature with the
+// signer gossmap's channel table gives, on the device (see cln_sigverify.h) --------------------------------------------
+extern "C" size_t sv_gossip_store_count(const uint8_t* store, size_t len) {
+    if (!store || len < 1) return 0;
+    gs_walk_end we;
+    return (size_t)gs_walk(store, len, [](const gs_rec&) {}, &we);
+}
+
+static_assert(GS_ST_DELETED == SV_GS_DELETED && GS_ST_STORE_RECORD == SV_GS_STORE_RECORD && GS_ST_UNKNOWN == SV_GS_UNKNOWN &&
+                  GS_ST_NOT_REACHED == SV_GS_NOT_REACHED && GS_ST_INCOMPLETE == SV_GS_INCOMPLETE &&
+                  GS_ST_PARTIAL == SV_GS_PARTIAL && GS_ST_TRUNCATED == SV_GS_TRUNCATED && GS_ST_BAD_CRC == SV_GS_BAD_CRC &&
+                  GS_ST_ENDED == SV_GS_ENDED && GS_ST_NO_AMOUNT == SV_GS_NO_AMOUNT,
+              "gossip_store.cuh and cln_sigverify.h must agree on the record statuses");
+
+struct ev_set {  // CUDA events of one call, destroyed on every exit path
+    cudaEvent_t e[4] = {};
+    ~ev_set() { for (cudaEvent_t x : e) if (x) cudaEventDestroy(x); }
+};
+
+extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, size_t len, const uint8_t* chain_hash32,
+                                           uint64_t* rec_off, uint16_t* rec_type, int* rec_status, uint64_t* rec_holder,
+                                           size_t rec_capacity, sv_gossip_store_summary* sum) {
+    if (!ctx || !store || len < 1 || !sum || (rec_capacity && (!rec_off || !rec_type || !rec_status))) return SV_ERR_ARG;
+    if (store[0] >> 5) return fail(ctx, SV_ERR_ARG, "gossip_store major version is not 0", cudaSuccess);
+    const auto t0 = std::chrono::steady_clock::now();
+    gs_walk_end we;
+    std::vector<gs_rec> rec;
+    rec.reserve(len / 256 + 16);
+    const size_t nrec = gs_walk(store, len, [&rec](const gs_rec& r) { rec.push_back(r); }, &we);
+    if (nrec > rec_capacity) return fail(ctx, SV_ERR_ARG, "rec_capacity is below the store's record count", cudaSuccess);
+    if (nrec >= 0xFFFFFFFFu) return fail(ctx, SV_ERR_ARG, "too many records", cudaSuccess);
+    // the records whose checksum map_catchup tests: every live one the walk reached, the ENDED record included
+    std::vector<u64> live_off;
+    std::vector<u32> live_rec;
+    for (size_t r = 0; r < nrec; r++)
+        if (rec[r].status == GS_LIVE || rec[r].status == GS_ST_ENDED) { live_off.push_back(rec[r].off); live_rec.push_back((u32)r); }
+    const float walk_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    dev_guard dg__;
+    CK(dg__.enter(ctx->device));
+    cudaStream_t st = ctx->stream;
+    ev_set ev;
+    if (ctx->profiling)
+        for (cudaEvent_t& e : ev.e) CK(cudaEventCreate(&e));
+    // the store is staged in a buffer of its own, freed on return: a store can be hundreds of MB
+    dev_tmp t_store, t_live;
+    CK(t_store.alloc(len));
+    CK(t_live.alloc(live_off.size() * 8 + 16));
+    u8* d_store = t_store.as<u8>();
+    u64* d_live = t_live.as<u64>();
+    u32* d_bad = reinterpret_cast<u32*>(d_live + live_off.size());
+    if (ev.e[0]) CK(cudaEventRecord(ev.e[0], st));
+    CK(cudaMemcpyAsync(d_store, store, len, cudaMemcpyHostToDevice, st));
+    if (!live_off.empty()) CK(cudaMemcpyAsync(d_live, live_off.data(), live_off.size() * 8, cudaMemcpyHostToDevice, st));
+    if (ev.e[1]) CK(cudaEventRecord(ev.e[1], st));
+    CK(cudaMemsetAsync(d_bad, 0xFF, 4, st));
+    if (!live_off.empty()) {
+        k_store_crc<<<(unsigned)((live_off.size() + 255) / 256), 256, 0, st>>>(d_store, d_live, live_off.size(), d_bad);
+        ctx->launches += 1;
+    }
+    if (ev.e[2]) CK(cudaEventRecord(ev.e[2], st));
+    u32 bad = 0xFFFFFFFFu;
+    CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    // the walk ends at the first bad checksum: only the records before it are verified
+    size_t cut = bad < live_rec.size() ? live_rec[bad] : nrec;
+    int cut_status = bad < live_rec.size() ? GS_ST_BAD_CRC : 0;
+    // messages (item slots laid out from the 2-byte type) and channel events before the cut, in store order
+    std::vector<u64> moff, eoff;
+    std::vector<u32> mlen, base, mrec, elen, emsg, msg_of(nrec, GS_NONE);
+    std::vector<u8> ekind;
+    size_t items = 0;
+    for (size_t r = 0; r < cut; r++) {
+        if (rec[r].status != GS_LIVE) continue;
+        const u32 t = rec[r].type, m = (u32)moff.size();
+        if (t == 256 || t == 257 || t == 258) {
+            msg_of[r] = m;
+            moff.push_back(rec[r].off + GS_HDR); mlen.push_back(rec[r].len); base.push_back((u32)items); mrec.push_back((u32)r);
+            items += t == 256 ? 4 : 1;
+        }
+        const int k = t == 256 ? GS_EV_ANN : t == 258 ? GS_EV_UPD : t == GS_DELETE_CHAN ? GS_EV_DEL : -1;
+        if (k >= 0) {
+            eoff.push_back(rec[r].off + GS_HDR); elen.push_back(rec[r].len); ekind.push_back((u8)k);
+            emsg.push_back(k == GS_EV_DEL ? GS_NONE : m);
+        }
+    }
+    const size_t n_msgs = moff.size(), nev = eoff.size();
+    if (items >= 0xFFFFFFFFu || nev >= 0x7FFFFFFFu) return fail(ctx, SV_ERR_ARG, "too many signatures in one store", cudaSuccess);
+    std::vector<int> mstatus(n_msgs);
+    std::vector<u32> holder(n_msgs);
+    if (n_msgs) {
+        int rc = ensure_staging(ctx, items);
+        if (rc) return rc;
+        if (items > ctx->span_cap) {
+            cudaFree(ctx->d_off); cudaFree(ctx->d_len); ctx->d_off = nullptr; ctx->d_len = nullptr; ctx->span_cap = 0;
+            CK(cudaMalloc(&ctx->d_off, items * sizeof(u64)));
+            CK(cudaMalloc(&ctx->d_len, items * sizeof(u32)));
+            ctx->span_cap = items;
+        }
+        size_t cub_bytes = 0;
+        CK(cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const u64*)nullptr, (u64*)nullptr, (const u32*)nullptr,
+                                           (u32*)nullptr, (int)nev, 0, 64, st));
+        // one slab: per message [off u64][len u32][item base u32][status int][holder u32][signer 33B][kind 1B], per item
+        // [keyok 1B], per event [off u64][key u64 x2][len u32][msg u32][value u32 x2][kind 1B][ok 1B], chain hash, sort scratch
+        size_t at = 0;
+        auto take = [&at](size_t bytes) { size_t o = at; at = (at + bytes + 15) & ~(size_t)15; return o; };
+        const size_t o_moff = take(8 * n_msgs), o_mlen = take(4 * n_msgs), o_base = take(4 * n_msgs),
+                     o_status = take(4 * n_msgs), o_holder = take(4 * n_msgs), o_sig = take(33 * n_msgs),
+                     o_kinds = take(n_msgs), o_keyok = take(items), o_eoff = take(8 * nev), o_key = take(8 * nev),
+                     o_key2 = take(8 * nev), o_elen = take(4 * nev), o_emsg = take(4 * nev), o_val = take(4 * nev),
+                     o_val2 = take(4 * nev), o_ekind = take(nev), o_ok = take(nev), o_chain = take(32), o_cub = take(cub_bytes);
+        dev_tmp t_slab;
+        CK(t_slab.alloc(at));
+        u8* s = t_slab.as<u8>();
+        u64 *d_moff = (u64*)(s + o_moff), *d_eoff = (u64*)(s + o_eoff), *d_key = (u64*)(s + o_key), *d_key2 = (u64*)(s + o_key2);
+        u32 *d_mlen = (u32*)(s + o_mlen), *d_base = (u32*)(s + o_base), *d_holder = (u32*)(s + o_holder),
+            *d_elen = (u32*)(s + o_elen), *d_emsg = (u32*)(s + o_emsg), *d_val = (u32*)(s + o_val), *d_val2 = (u32*)(s + o_val2);
+        int* d_status = (int*)(s + o_status);
+        u8 *d_signers = s + o_sig, *d_kinds = chain_hash32 ? s + o_kinds : nullptr, *d_keyok = s + o_keyok,
+           *d_ekind = s + o_ekind, *d_ok = s + o_ok, *d_chain = chain_hash32 ? s + o_chain : nullptr;
+        CK(cudaMemcpyAsync(d_moff, moff.data(), 8 * n_msgs, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(d_mlen, mlen.data(), 4 * n_msgs, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(d_base, base.data(), 4 * n_msgs, cudaMemcpyHostToDevice, st));
+        CK(cudaMemsetAsync(d_holder, 0xFF, 4 * n_msgs, st));
+        CK(cudaMemsetAsync(d_signers, 0, 33 * n_msgs, st));  // an update without a channel keeps the all-zero key
+        if (chain_hash32) {
+            // with a chain hash, k_gossip_slice applies gossipd's gates (burst mode); every update's signer is given
+            CK(cudaMemsetAsync(d_kinds, 1, n_msgs, st));
+            CK(cudaMemcpyAsync(d_chain, chain_hash32, 32, cudaMemcpyHostToDevice, st));
+        }
+        if (nev) {
+            CK(cudaMemcpyAsync(d_eoff, eoff.data(), 8 * nev, cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(d_elen, elen.data(), 4 * nev, cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(d_emsg, emsg.data(), 4 * nev, cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(d_ekind, ekind.data(), nev, cudaMemcpyHostToDevice, st));
+            k_store_events<<<(unsigned)((nev + 255) / 256), 256, 0, st>>>(d_store, d_eoff, d_elen, d_ekind, nev, d_key, d_val, d_ok);
+            CK(cub::DeviceRadixSort::SortPairs(s + o_cub, cub_bytes, d_key, d_key2, d_val, d_val2, (int)nev, 0, 64, st));
+            k_store_resolve<<<(unsigned)((nev + 127) / 128), 128, 0, st>>>(d_store, d_key2, d_val2, d_ok, d_ekind, d_eoff, d_emsg,
+                                                                            nev, d_moff, d_holder, d_signers);
+            ctx->launches += 2;
+        }
+        unsigned gm = (unsigned)((n_msgs + 127) / 128);
+        k_gossip_slice<<<gm, 128, 0, st>>>(d_store, d_moff, d_mlen, d_base, d_signers, n_msgs, ctx->d_off, ctx->d_len,
+                                           ctx->d_key, ctx->d_sig, d_status, d_chain, d_kinds);
+        k_sha256d<<<(unsigned)((items + 127) / 128), 128, 0, st>>>(d_store, ctx->d_off, ctx->d_len, items, ctx->d_msg);
+        ctx->launches += 2;
+        rc = gossip_verify_items(ctx, ctx->d_msg, ctx->d_key, ctx->d_sig, items, ctx->d_verdict, st, d_keyok, &ctx->last_distinct);
+        if (rc) return rc;
+        k_gossip_status<<<gm, 128, 0, st>>>(d_store, d_moff, d_mlen, d_base, n_msgs, ctx->d_verdict, d_keyok, d_status,
+                                            d_kinds, nullptr, nullptr);
+        k_store_finish<<<(unsigned)((n_msgs + 255) / 256), 256, 0, st>>>(d_store, d_moff, d_holder, n_msgs, d_status);
+        ctx->launches += 2;
+        if (ev.e[3]) CK(cudaEventRecord(ev.e[3], st));
+        CK(cudaMemcpyAsync(mstatus.data(), d_status, 4 * n_msgs, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(holder.data(), d_holder, 4 * n_msgs, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+    } else if (ev.e[3]) {
+        CK(cudaEventRecord(ev.e[3], st));
+        CK(cudaStreamSynchronize(st));
+    }
+    // an announcement without room for its amount record stops the walk unless it is redundant (add_channel returns the
+    // channel that already holds the scid before it looks for the amount)
+    if (we.no_amount < cut && holder[msg_of[we.no_amount]] == GS_NONE) {
+        cut = we.no_amount;
+        cut_status = GS_ST_NO_AMOUNT;
+    }
+    sv_gossip_store_summary S;
+    memset(&S, 0, sizeof S);
+    S.version = store[0];
+    S.stop = cut_status ? cut_status : we.stop;
+    S.end_offset = cut_status ? rec[cut].off : we.end;
+    S.records = nrec;
+    for (size_t r = 0; r < nrec; r++) {
+        const u32 t = rec[r].type, m = msg_of[r];
+        int s = rec[r].status;
+        u64 h = ~(u64)0;
+        if (cut_status && r >= cut) {
+            s = r == cut ? cut_status : GS_ST_NOT_REACHED;
+        } else if (s == GS_LIVE) {
+            if (m != GS_NONE) {
+                s = mstatus[m];
+                if (holder[m] != GS_NONE) h = rec[mrec[holder[m]]].off;
+                S.redundant_announcements += t == 256 && holder[m] != GS_NONE;
+                S.updates_without_channel += t == 258 && rec[r].len >= 112 && holder[m] == GS_NONE;
+            } else {
+                s = (t == GS_CHANNEL_AMOUNT || t == GS_DELETE_CHAN || t == GS_CHAN_DYING || t == GS_UUID) ? GS_ST_STORE_RECORD
+                                                                                                          : GS_ST_UNKNOWN;
+            }
+        } else if (s == GS_ST_ENDED && rec[r].len >= 10) {
+            for (int b = 0; b < 8; b++) S.ended_equivalent_offset = (S.ended_equivalent_offset << 8) | store[rec[r].off + GS_HDR + 2 + b];
+        }
+        rec_off[r] = rec[r].off;
+        rec_type[r] = (uint16_t)t;
+        rec_status[r] = s;
+        if (rec_holder) rec_holder[r] = h;
+        if (m != GS_NONE && s <= 4 && !(cut_status && r >= cut)) {
+            S.good += s == 0; S.bad_signature += s >= 1 && s <= 4; S.malformed += s == -1; S.no_channel += s == -2;
+            S.wrong_chain += s == -3; S.bad_order += s == -4;
+        }
+        S.deleted += s == GS_ST_DELETED; S.store_records += s == GS_ST_STORE_RECORD; S.unknown += s == GS_ST_UNKNOWN;
+        S.not_reached += s == GS_ST_NOT_REACHED;
+    }
+    *sum = S;
+    ctx->gs_ms[0] = walk_ms;
+    if (ev.e[0])
+        for (int i = 0; i < 3; i++) CK(cudaEventElapsedTime(&ctx->gs_ms[1 + i], ev.e[i], ev.e[i + 1]));
+    return SV_OK;
+}
+// where the last sv_verify_gossip_store_host call spent its time (profiling mode): host header walk, H2D copy of the store,
+// checksum kernel, then slicing, resolution, hashing and verification to the last status (device events)
+extern "C" int sv_get_last_gossip_store_timing(sv_ctx* ctx, float* ms4) {
+    if (!ctx || !ctx->profiling || !ms4) return SV_ERR_ARG;
+    for (int i = 0; i < 4; i++) ms4[i] = ctx->gs_ms[i];
+    return SV_OK;
+}
 
 // n ECDSA signatures by ONE key (channeld's HTLC loop): table of the key built once, ladder-only kernel
 extern "C" int sv_verify_samekey_host(sv_ctx* ctx, int kind, const uint8_t* key, const uint8_t* msg32, const uint8_t* sig64,

@@ -35,6 +35,20 @@ class SvTx(ctypes.Structure):
                 ("sequences_off", ctypes.c_uint32), ("sequences_len", ctypes.c_uint32)]
 
 
+class SvGossipStoreSummary(ctypes.Structure):
+    """sv_gossip_store_summary (include/cln_sigverify.h)"""
+    _fields_ = [("version", ctypes.c_uint32), ("stop", ctypes.c_int32)] + [(f, ctypes.c_uint64) for f in (
+        "end_offset", "ended_equivalent_offset", "records", "good", "bad_signature", "malformed", "no_channel", "wrong_chain",
+        "bad_order", "deleted", "store_records", "unknown", "not_reached", "redundant_announcements",
+        "updates_without_channel")]
+
+
+# record statuses of verify_gossip_store besides the signature statuses (include/cln_sigverify.h SV_GS_*)
+GS_EOF, GS_DELETED, GS_STORE_RECORD, GS_UNKNOWN, GS_NOT_REACHED = 0, 16, 17, 18, 19
+GS_INCOMPLETE, GS_PARTIAL, GS_TRUNCATED, GS_BAD_CRC, GS_ENDED, GS_NO_AMOUNT = 32, 33, 34, 35, 36, 37
+GS_NO_HOLDER = (1 << 64) - 1
+
+
 class SvInfo(ctypes.Structure):
     _fields_ = [("device", ctypes.c_int), ("sm_count", ctypes.c_int), ("main_block", ctypes.c_int),
                 ("main_grid", ctypes.c_int), ("main_regs", ctypes.c_int), ("gtable_bytes", ctypes.c_size_t),
@@ -62,6 +76,10 @@ def load_library():
     lib.sv_verify_gossip_burst_host.argtypes = [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp]
     lib.sv_last_gossip_repairs.argtypes = [vp]
     lib.sv_last_gossip_repairs.restype = ctypes.c_uint
+    lib.sv_gossip_store_count.argtypes = [vp, sz]
+    lib.sv_gossip_store_count.restype = sz
+    lib.sv_verify_gossip_store_host.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp, sz, ctypes.POINTER(SvGossipStoreSummary)]
+    lib.sv_get_last_gossip_store_timing.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
     lib.sv_verify_tx_host.argtypes = [vp, i, vp, vp, sz, vp, vp, sz, vp, vp]
     lib.sv_verify_samekey_host.argtypes = [vp, i, vp, vp, vp, sz, vp]
     lib.sv_verify_bolt12_host.argtypes = [vp, ctypes.c_char_p, ctypes.c_char_p, vp, sz, vp, vp, vp, vp, sz, vp, vp]
@@ -222,6 +240,38 @@ class SigVerifier:
     def last_gossip_repairs(self):
         """updates the last gossip burst re-resolved in its repair round (their first candidate announcement failed)"""
         return int(self.lib.sv_last_gossip_repairs(self._ctx))
+
+    def verify_gossip_store(self, store, chain_hash=None, capacity=None):
+        """A whole gossip_store (bytes, version byte included), walked as gossmap's map_catchup walks it, every record
+        checksum and every signature checked on the device.  Returns (rec_off uint64, rec_type uint16, rec_status int32,
+        rec_holder uint64, summary dict): one entry per record the walk reads; rec_status is a signature status for
+        256/257/258 (0, 1..4, -1, -2 no channel, and with chain_hash -3 / -4) or a GS_* record status; rec_holder is the
+        header offset of the announcement holding the channel (updates, redundant announcements), else GS_NO_HOLDER.
+        capacity: entries to provide (default: sv_gossip_store_count)."""
+        buf = np.frombuffer(bytes(store), dtype=np.uint8)
+        chain = None
+        if chain_hash is not None:
+            chain = np.frombuffer(bytes(chain_hash), dtype=np.uint8)
+            if chain.size != 32:
+                raise ValueError("chain_hash must be 32 bytes")
+        n = int(self.lib.sv_gossip_store_count(buf.ctypes.data, buf.size)) if capacity is None else int(capacity)
+        off = np.zeros(max(n, 1), np.uint64)
+        typ = np.zeros(max(n, 1), np.uint16)
+        status = np.zeros(max(n, 1), np.int32)
+        holder = np.zeros(max(n, 1), np.uint64)
+        s = SvGossipStoreSummary()
+        self._check(self.lib.sv_verify_gossip_store_host(
+            self._ctx, buf.ctypes.data, buf.size, chain.ctypes.data if chain is not None else None, off.ctypes.data,
+            typ.ctypes.data, status.ctypes.data, holder.ctypes.data, n, ctypes.byref(s)), "sv_verify_gossip_store_host")
+        summary = {f: getattr(s, f) for f, _ in SvGossipStoreSummary._fields_}
+        k = s.records
+        return off[:k], typ[:k], status[:k], holder[:k], summary
+
+    def last_gossip_store_timing(self):
+        """(header walk, H2D, checksums, verification) in ms of the last verify_gossip_store (profiling mode)"""
+        ms = (ctypes.c_float * 4)()
+        self._check(self.lib.sv_get_last_gossip_store_timing(self._ctx, ms), "sv_get_last_gossip_store_timing")
+        return tuple(ms)
 
     def verify_samekey(self, kind, key, msg32, sig64):
         """n ECDSA signatures by ONE key (channeld's HTLC loop): the key's table is built once on the device."""
