@@ -125,6 +125,7 @@ void cln_sigverify_shutdown(void);
  *   check_signed_hash, check_signed_hash_nodeid, check_schnorr_sig, check_tx_sigs_batch   (sigverifyd_verify)
  *   bolt12_check_signature                                                              (sigverifyd_bolt12)
  *   check_tx_sig, check_tx_sigs_bip143_batch                                            (sigverifyd_tx)
+ *   check_tx_sig_grind_fee                                                              (sigverifyd_fee_grind)
  *   sigcheck_channel_announcement_batch / _node_announcement_batch / _channel_update_batch (sigverifyd_gossip)
  *   sigcheck_gossip_batch                                                               (sigverifyd_gossip_burst)
  *   sha256_double                                                                       (sigverifyd_sha256d)
@@ -155,6 +156,14 @@ bool check_tx_sig(const struct bitcoin_tx *tx, size_t input_num, const u8 *redee
                   const struct pubkey *key, const struct bitcoin_signature *sig);
 void cln_sigverify_set_tx_hooks(size_t (*script_bytelen)(const void *tal_script),
                                 uint64_t (*input_amount_sat)(const struct bitcoin_tx *tx, size_t input_num));
+
+/* grind_htlc_tx_fee (onchaind/onchaind.c:389-437) in one call.  tx is NOT modified: on true the caller sets output 0 to
+ * input - *fee_sat and finalizes, as the loop leaves it.  remotesig's sighash type is gated as check_tx_sig does.
+ *      The record is built as check_tx_sig builds it (input amount from the same hook); a transaction that is not one
+ *      input and one output aborts.  Semantics of the walk: sv_grind_tx_fee_host (cln_sigverify.h). */
+bool check_tx_sig_grind_fee(const struct bitcoin_tx *tx, const u8 *witness_script, const struct pubkey *key,
+                            const struct bitcoin_signature *remotesig, uint64_t weight, uint32_t min_feerate,
+                            uint32_t max_feerate, uint64_t *fee_sat, uint32_t *feerate);
 
 /* common/bolt12.h: bolt12_check_signature (common/bolt12.c:80-92).  fields is a tal array (its length comes from
  * tal_bytelen(fields) / sizeof(struct tlv_field), through the same weak tal_bytelen reference or hook as check_tx_sig);

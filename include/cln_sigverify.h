@@ -31,6 +31,8 @@
  *   sv_verify_gossip_store_host(...)        gossmap's map_catchup over a whole gossip_store (common/gossmap.c:815-937:
  *                                           record walk, crc32c) plus every signature it never checks, with the
  *                                           signer its channel table gives
+ *   sv_grind_tx_fee_host(...)               onchaind's grind_htlc_tx_fee loop over check_tx_sig
+ *                                           onchaind/onchaind.c:389-437, every candidate feerate in one call
  *   sv_sha256d_host(...)                    sha256_double()              bitcoin/shadouble.c:7-11
  *   sv_pubkey_parse_host(...)               pubkey_from_der()            bitcoin/pubkey.c:14-24
  *   sv_enqueue_* / sv_flush                 the deferral queue a batching caller (gossipd ingest,
@@ -276,6 +278,21 @@ typedef struct {
 } sv_tx;
 int sv_verify_tx_host(sv_ctx *ctx, int kind, const sv_tx *txs, const uint8_t *scripts, size_t scripts_len,
                       const uint8_t *key, const uint8_t *sig64, size_t n, uint8_t *verdicts, uint8_t *sighash32_out);
+
+/* onchaind's HTLC fee grind (onchaind/onchaind.c:389-437) as one call: the first feerate f in [min_feerate, max_feerate],
+ * ascending, whose fee = f*weight/1000 (common/amount.c:698-707 amount_tx_fee) makes sig64 verify under key for the
+ * transaction *tx with its single output set to input_amount - fee.  A feerate whose fee equals the previous feerate's
+ * is skipped; the walk ends at the first fee above input_amount, as the reference loop does.  *feerate_out = -1 when
+ * none verifies (including a signature or key the reference would refuse).  tx->output_amount is ignored; tx->flags
+ * must be 0 (one input, one output); weight < 2^32.  Verdict per candidate = sv_verify_tx_host's.
+ *      kind: SV_KIND_ECDSA33 or _XY.  min_feerate > max_feerate: none found, no launch.  weight 0: one candidate, fee 0.
+ *      Spans out of range, a non-zero flags, weight >= 2^32 and NULL required pointers: SV_ERR_ARG.  On the device: one
+ *      warp computes s^-1, u2*Q and the preimage through nSequence once (k_grind_setup), then one thread per feerate
+ *      (k_grind) hashes its output and adds u1*G; the range runs in ascending chunks of 2^20 feerates from min_feerate and
+ *      the call returns after the first chunk with a match.  *fee_out: the matching fee (0 when none). */
+int sv_grind_tx_fee_host(sv_ctx *ctx, int kind, const sv_tx *tx, const uint8_t *scripts, size_t scripts_len,
+                         const uint8_t *key, const uint8_t *sig64, uint64_t weight, uint32_t min_feerate,
+                         uint32_t max_feerate, int64_t *feerate_out, uint64_t *fee_out);
 
 /* ---- BOLT12 signatures with the message hash computed ON THE DEVICE: bolt12_check_signature (common/bolt12.c:80-92)
  *      for n TLV streams.  Stream i is blob[off[i] .. off[i]+len[i]), the raw TLV bytes of an offer, invoice_request or

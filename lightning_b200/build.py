@@ -93,7 +93,8 @@ def build_engine(force=False, verbose=False, extra_flags=()):
 
 
 def build_host_emul(force=False):
-    src = [os.path.join(ROOT, "tests", "host_emul", f) for f in ("emul.cpp", "bolt12_emul.cpp", "gossip_store_emul.cpp")]
+    src = [os.path.join(ROOT, "tests", "host_emul", f) for f in ("emul.cpp", "bolt12_emul.cpp", "gossip_store_emul.cpp",
+                                                             "fee_grind_emul.cpp")]
     srcs = _sources(CSRC, (".cuh",)) + src
     if not force and _newer(EMUL, srcs):
         return EMUL

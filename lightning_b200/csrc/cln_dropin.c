@@ -13,6 +13,10 @@
 #include "sigverifyd_proto.h"
 #include "sigverifyd_wiregen.h"
 
+/* weak: the library's client mode is also linked against engine builds without the fee grind (the fake engine of the
+ * client-mode CPU tests); check_tx_sig_grind_fee then works through the daemon only */
+#pragma weak sv_grind_tx_fee_host
+
 #include <errno.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -386,21 +390,30 @@ static void remote_tx(int kind, const u8 *key, const sv_tx *txs, const u8 *scrip
     }
 }
 
-bool check_tx_sig(const struct bitcoin_tx *tx, size_t input_num, const u8 *redeemscript, const u8 *witness_script,
-                  const struct pubkey *key, const struct bitcoin_signature *sig) {
-    const u8 *script = witness_script ? witness_script : redeemscript;
-    /* "We only support a limited subset of sighash types." (signature.c:205-211) */
-    if (sig->sighash_type != SIGHASH_ALL) {
-        if (!witness_script) return false;
-        if ((int)sig->sighash_type != (SIGHASH_SINGLE | SIGHASH_ANYONECANPAY)) return false;
-    }
+/* "We only support a limited subset of sighash types." (signature.c:205-211) */
+static bool sighash_type_supported(const struct bitcoin_signature *sig, bool have_witness_script) {
+    if (sig->sighash_type == SIGHASH_ALL) return true;
+    return have_witness_script && (int)sig->sighash_type == (SIGHASH_SINGLE | SIGHASH_ANYONECANPAY);
+}
+
+/* The record and span blob (returned, *blob_len bytes; the caller frees it) sv_verify_tx_host takes for input input_num of
+ * tx signed under sig's sighash type, with script as the scriptCode and the input amount from the hook or
+ * psbt_input_get_amount.  Every output / outpoint is handed over serialised, so the host hashes nothing.  With one_output
+ * the transaction has exactly one input and one output (`who` aborts otherwise), and the record takes the single-output
+ * form (flags 0): out_script is output 0's scriptPubKey alone, its amount goes in output_amount. */
+static u8 *tx_record(const struct bitcoin_tx *tx, size_t input_num, const u8 *script, const struct bitcoin_signature *sig,
+                     bool one_output, const char *who, sv_tx *t, size_t *blob_len) {
     const struct wally_tx *w = tx->wtx;
     if (input_num >= w->num_inputs) { /* assert(input_num < tx->wtx->num_inputs), signature.c:212 */
-        fprintf(stderr, "cln_sigverify: check_tx_sig: input %zu of %zu\n", input_num, w->num_inputs);
+        fprintf(stderr, "cln_sigverify: %s: input %zu of %zu\n", who, input_num, w->num_inputs);
+        abort();
+    }
+    if (one_output && (w->num_inputs != 1 || w->num_outputs != 1)) {
+        fprintf(stderr, "cln_sigverify: %s: %zu inputs and %zu outputs, not one of each\n", who, w->num_inputs, w->num_outputs);
         abort();
     }
     size_t script_len = tal_len(script, "check_tx_sig: no tal_bytelen (cln_sigverify_set_tx_hooks)");
-    uint64_t amount;
+    uint64_t amount = 0;
     if (g_input_sat) amount = g_input_sat(tx, input_num);
     else if (psbt_input_get_amount) amount = psbt_input_get_amount(tx->psbt, input_num).satoshis;
     else die("check_tx_sig: no psbt_input_get_amount (cln_sigverify_set_tx_hooks)", -4);
@@ -411,45 +424,58 @@ bool check_tx_sig(const struct bitcoin_tx *tx, size_t input_num, const u8 *redee
     size_t cap = script_len + out_bytes + 40 * w->num_inputs + 16;
     u8 *blob = (u8 *)malloc(cap);
     if (!blob) die("malloc", -3);
-    sv_tx t;
-    memset(&t, 0, sizeof t);
+    memset(t, 0, sizeof *t);
     size_t n = 0;
-    t.version = w->version;
-    t.locktime = w->locktime;
-    t.sequence = w->inputs[input_num].sequence;
-    t.sighash_type = (uint32_t)sig->sighash_type;
-    memcpy(t.prev_txid, w->inputs[input_num].txhash, 32);
-    t.prev_index = w->inputs[input_num].index;
-    t.input_amount = amount;
-    t.script_off = (uint32_t)n;
-    t.script_len = (uint32_t)script_len;
+    t->version = w->version;
+    t->locktime = w->locktime;
+    t->sequence = w->inputs[input_num].sequence;
+    t->sighash_type = (uint32_t)sig->sighash_type;
+    memcpy(t->prev_txid, w->inputs[input_num].txhash, 32);
+    t->prev_index = w->inputs[input_num].index;
+    t->input_amount = amount;
+    t->script_off = (uint32_t)n;
+    t->script_len = (uint32_t)script_len;
     if (script_len) memcpy(blob + n, script, script_len);
     n += script_len;
-    t.out_script_off = (uint32_t)n;
-    if (single) { /* the output at the input's index, or none (tx_io.c:725-731) */
-        if (input_num < w->num_outputs) { n += put_output(blob + n, &w->outputs[input_num]); t.flags |= SV_TX_OUTPUTS_SERIALIZED; }
-        else t.flags |= SV_TX_OUTPUTS_ZERO;
+    t->out_script_off = (uint32_t)n;
+    if (one_output) { /* ALL and SINGLE of input 0 both commit to output 0 alone (tx_io.c:714-731) */
+        t->output_amount = w->outputs[0].satoshi;
+        if (w->outputs[0].script_len) memcpy(blob + n, w->outputs[0].script, w->outputs[0].script_len);
+        n += w->outputs[0].script_len;
+    } else if (single) { /* the output at the input's index, or none (tx_io.c:725-731) */
+        if (input_num < w->num_outputs) { n += put_output(blob + n, &w->outputs[input_num]); t->flags |= SV_TX_OUTPUTS_SERIALIZED; }
+        else t->flags |= SV_TX_OUTPUTS_ZERO;
     } else {
         for (size_t i = 0; i < w->num_outputs; i++) n += put_output(blob + n, &w->outputs[i]);
-        t.flags |= SV_TX_OUTPUTS_SERIALIZED;
+        t->flags |= SV_TX_OUTPUTS_SERIALIZED;
     }
-    t.out_script_len = (uint32_t)(n - t.out_script_off);
+    t->out_script_len = (uint32_t)(n - t->out_script_off);
     if (w->num_inputs > 1) {
-        t.flags |= SV_TX_INPUTS_SERIALIZED;
-        t.prevouts_off = (uint32_t)n;
+        t->flags |= SV_TX_INPUTS_SERIALIZED;
+        t->prevouts_off = (uint32_t)n;
         for (size_t i = 0; i < w->num_inputs; i++) {
             memcpy(blob + n, w->inputs[i].txhash, 32);
             for (int b = 0; b < 4; b++) blob[n + 32 + b] = (u8)(w->inputs[i].index >> (8 * b));
             n += 36;
         }
-        t.prevouts_len = (uint32_t)(n - t.prevouts_off);
-        t.sequences_off = (uint32_t)n;
+        t->prevouts_len = (uint32_t)(n - t->prevouts_off);
+        t->sequences_off = (uint32_t)n;
         for (size_t i = 0; i < w->num_inputs; i++) {
             for (int b = 0; b < 4; b++) blob[n + b] = (u8)(w->inputs[i].sequence >> (8 * b));
             n += 4;
         }
-        t.sequences_len = (uint32_t)(n - t.sequences_off);
+        t->sequences_len = (uint32_t)(n - t->sequences_off);
     }
+    *blob_len = n;
+    return blob;
+}
+
+bool check_tx_sig(const struct bitcoin_tx *tx, size_t input_num, const u8 *redeemscript, const u8 *witness_script,
+                  const struct pubkey *key, const struct bitcoin_signature *sig) {
+    if (!sighash_type_supported(sig, witness_script != NULL)) return false;
+    sv_tx t;
+    size_t n;
+    u8 *blob = tx_record(tx, input_num, witness_script ? witness_script : redeemscript, sig, false, "check_tx_sig", &t, &n);
     u8 xy[64], s64[64], v = 0;
     pubkey_to_xy(xy, &key->pubkey);
     sig_to_wire(s64, &sig->s);
@@ -462,6 +488,56 @@ bool check_tx_sig(const struct bitcoin_tx *tx, size_t input_num, const u8 *redee
     free(blob);
     if (rc != SV_OK) die("sv_verify_tx_host", rc);
     return v == 1;
+}
+
+/* one fee grind through sigverifyd_fee_grind: the record's two spans travel as they are */
+static int64_t remote_grind(int kind, const u8 *key, const sv_tx *t, const u8 *blob, const u8 *sig64, uint64_t weight,
+                            uint32_t min_feerate, uint32_t max_feerate, uint64_t *fee) {
+    const size_t ks = sv_key_size(kind);
+    uint64_t mlen64 = 2 + 8 + 1 + 4 + ks + 5 * 4 + 32 + 8 + 4 + (uint64_t)t->script_len + 4 + t->out_script_len + 64 + 8 + 4 + 4;
+    if (mlen64 > MAX_FRAME) die_daemon("transaction too large for one request");
+    size_t mlen = (size_t)mlen64, rl;
+    u8 *f = (u8 *)malloc(4 + mlen);
+    if (!f) die("malloc", -3);
+    uint64_t id = ++g_req_id;
+    towire_sigverifyd_fee_grind(f + 4, mlen, id, (uint8_t)kind, (uint32_t)ks, key, t->version, t->locktime, t->sequence,
+                                t->sighash_type, t->prev_index, t->prev_txid, t->input_amount, t->script_len,
+                                blob + t->script_off, t->out_script_len, blob + t->out_script_off, sig64, weight, min_feerate,
+                                max_feerate);
+    u8 *r = roundtrip(f, mlen, id, &rl);
+    struct sigverifyd_fee_grind_reply g;
+    if (!fromwire_sigverifyd_fee_grind_reply(r, rl, &g)) die_daemon("malformed fee grind reply");
+    *fee = g.fee;
+    int64_t feerate = g.found ? (int64_t)g.feerate : -1;
+    free(r);
+    free(f);
+    return feerate;
+}
+
+bool check_tx_sig_grind_fee(const struct bitcoin_tx *tx, const u8 *witness_script, const struct pubkey *key,
+                            const struct bitcoin_signature *remotesig, uint64_t weight, uint32_t min_feerate,
+                            uint32_t max_feerate, uint64_t *fee_sat, uint32_t *feerate) {
+    if (!sighash_type_supported(remotesig, witness_script != NULL)) return false;
+    sv_tx t;
+    size_t n;
+    u8 *blob = tx_record(tx, 0, witness_script, remotesig, true, "check_tx_sig_grind_fee", &t, &n);
+    u8 xy[64], s64[64];
+    pubkey_to_xy(xy, &key->pubkey);
+    sig_to_wire(s64, &remotesig->s);
+    int64_t f = -1;
+    uint64_t fee = 0;
+    if (client()) {
+        f = remote_grind(SV_KIND_ECDSA_XY, xy, &t, blob, s64, weight, min_feerate, max_feerate, &fee);
+    } else {
+        if (!sv_grind_tx_fee_host) die("check_tx_sig_grind_fee: this engine has no sv_grind_tx_fee_host", SV_ERR_ARG);
+        int rc = sv_grind_tx_fee_host(ctx(), SV_KIND_ECDSA_XY, &t, blob, n, xy, s64, weight, min_feerate, max_feerate, &f, &fee);
+        if (rc != SV_OK) die("sv_grind_tx_fee_host", rc);
+    }
+    free(blob);
+    if (f < 0) return false;
+    *fee_sat = fee;
+    *feerate = (uint32_t)f;
+    return true;
 }
 
 /* ---- bolt12_check_signature (common/bolt12.c:80-92): the fields go back to wire form (towire_tlvstream_raw's layout:

@@ -424,6 +424,28 @@ __global__ void k_mask_verdicts(u8* verdict, const u8* ok, size_t n) {
     if (i < n && !ok[i]) verdict[i] = 0;
 }
 
+// ---- onchaind's HTLC fee grind (verify.cuh grind_*): one warp builds the shared state, then one thread per feerate ----
+__global__ void k_grind_setup(int kind, const u8* key, const u8* sig, const sv_tx_item* tx, const u8* blob, qtab_entry* tab,
+                              sv_grind_state* out) {
+    sv_grind_state g;  // all 32 lanes compute the same values (the table stores coincide); lane 0 publishes the state
+    grind_setup(&g, tab, kind, key, sig, *tx, blob, blockDim.x);
+    if (threadIdx.x == 0) *out = g;
+}
+// feerates first .. first + count - 1; *best = the lowest feerate that verified so far (UINT64_MAX: none)
+__global__ void __launch_bounds__(128) k_grind(const sv_grind_state* __restrict__ g, const sv_tx_item* __restrict__ tx,
+                                               const u8* __restrict__ blob, const u8* __restrict__ sig,
+                                               const ge_mem* __restrict__ gtab, u64 weight, u64 min_feerate, u64 first,
+                                               u64 count, unsigned long long* best) {
+    u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    const u64 f = first + i;
+    const sv_tx_item t = *tx;
+    u64 fee;
+    if (!grind_feerate_checked(f, weight, min_feerate, t.input_amount, &fee)) return;
+    if (f > *(volatile unsigned long long*)best) return;  // a lower feerate of this chunk matched already
+    if (grind_candidate(g, t, blob, sig, t.input_amount - fee, gtab)) atomicMin(best, (unsigned long long)f);
+}
+
 // ---- gossip ingest (SURVEY.md §8f N1): the device slices raw wire messages itself ----------------------------
 // One thread per message.  Field offsets: wire/peer_wire.csv:340-377; signed regions and checking order:
 // gossipd/sigcheck.c:9-43 (channel_update), 45-115 (channel_announcement), 118-164 (node_announcement).
@@ -2432,6 +2454,77 @@ extern "C" int sv_verify_mixed_host(sv_ctx* ctx, const uint8_t* kinds, const uin
     if (rc) return rc;
     CK(cudaMemcpyAsync(verdicts, d_o, n, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
+    return SV_OK;
+}
+
+// ---- onchaind's HTLC fee grind (onchaind/onchaind.c:389-437) in one call ---------------------------------------------
+// The host stages one transaction record, the two script spans, the key and the signature (a few hundred bytes), runs
+// k_grind_setup once and then k_grind over ascending chunks of SV_GRIND_CHUNK feerates, reading back the 8-byte best
+// feerate after each chunk and stopping at the first chunk with a match.
+#define SV_GRIND_CHUNK (1u << 20)
+extern "C" int sv_grind_tx_fee_host(sv_ctx* ctx, int kind, const sv_tx* tx, const uint8_t* scripts, size_t scripts_len,
+                                    const uint8_t* key, const uint8_t* sig64, uint64_t weight, uint32_t min_feerate,
+                                    uint32_t max_feerate, int64_t* feerate_out, uint64_t* fee_out) {
+    size_t ks = sv_key_size(kind);
+    if (!ctx || ks == 0 || kind == SV_KIND_SCHNORR || !tx || !key || !sig64 || !feerate_out || !fee_out ||
+        (scripts_len && !scripts))
+        return SV_ERR_ARG;
+    if (tx->flags) return fail(ctx, SV_ERR_ARG, "sv_grind_tx_fee_host: tx->flags must be 0 (one input, one output)", cudaSuccess);
+    if (weight >> 32) return fail(ctx, SV_ERR_ARG, "sv_grind_tx_fee_host: weight >= 2^32", cudaSuccess);
+    if ((size_t)tx->script_off + tx->script_len > scripts_len || (size_t)tx->out_script_off + tx->out_script_len > scripts_len)
+        return fail(ctx, SV_ERR_ARG, "script span out of range", cudaSuccess);
+#ifdef SV_COMB_SMEM
+    return fail(ctx, SV_ERR_ARG, "sv_grind_tx_fee_host: not available in the SV_COMB_SMEM build variant", cudaSuccess);
+#endif
+    *feerate_out = -1;
+    *fee_out = 0;
+    if (min_feerate > max_feerate) return SV_OK;
+    const u64 last = grind_last_feerate(min_feerate, max_feerate, weight, tx->input_amount);
+    if (last < min_feerate) return SV_OK;  // the fee at min_feerate is already above the input: the loop breaks at once
+    dev_guard dg__;
+    CK(dg__.enter(ctx->device));
+    // staging: [state | 8 table entries | tx record | best | key 64 | sig 64 | witness script | output script]
+    const size_t o_tab = (sizeof(sv_grind_state) + 255) & ~(size_t)255, o_tx = o_tab + 8 * sizeof(qtab_entry),
+                 o_best = o_tx + sizeof(sv_tx_item), o_key = o_best + 16, o_sig = o_key + 64, o_blob = o_sig + 64;
+    const size_t blob_len = (size_t)tx->script_len + tx->out_script_len;
+    int rc = ensure_gbuf(ctx, o_blob + blob_len + 16);
+    if (rc) return rc;
+    std::vector<u8> h(o_blob + blob_len - o_tx, 0);
+    sv_tx_item t;
+    memcpy(&t, tx, sizeof t);
+    t.script_off = 0;
+    t.out_script_off = tx->script_len;
+    memcpy(h.data(), &t, sizeof t);
+    memset(h.data() + (o_best - o_tx), 0xFF, 8);
+    memcpy(h.data() + (o_key - o_tx), key, ks);
+    memcpy(h.data() + (o_sig - o_tx), sig64, 64);
+    if (tx->script_len) memcpy(h.data() + (o_blob - o_tx), scripts + tx->script_off, tx->script_len);
+    if (tx->out_script_len) memcpy(h.data() + (o_blob - o_tx) + tx->script_len, scripts + tx->out_script_off, tx->out_script_len);
+    u8* b = ctx->g_buf;
+    sv_grind_state* d_state = reinterpret_cast<sv_grind_state*>(b);
+    qtab_entry* d_tab = reinterpret_cast<qtab_entry*>(b + o_tab);
+    const sv_tx_item* d_tx = reinterpret_cast<const sv_tx_item*>(b + o_tx);
+    unsigned long long* d_best = reinterpret_cast<unsigned long long*>(b + o_best);
+    cudaStream_t st = ctx->stream;
+    CK(cudaMemcpyAsync(b + o_tx, h.data(), h.size(), cudaMemcpyHostToDevice, st));
+    k_grind_setup<<<1, 32, 0, st>>>(kind, b + o_key, b + o_sig, d_tx, b + o_blob, d_tab, d_state);
+    ctx->launches += 1;
+    CK(cudaGetLastError());
+    unsigned long long best = ~0ull;
+    for (u64 first = min_feerate; first <= last; first += SV_GRIND_CHUNK) {
+        u64 count = last - first + 1 < SV_GRIND_CHUNK ? last - first + 1 : SV_GRIND_CHUNK;
+        k_grind<<<(unsigned)((count + 127) / 128), 128, 0, st>>>(d_state, d_tx, b + o_blob, b + o_sig, ctx->d_gtab, weight,
+                                                                 min_feerate, first, count, d_best);
+        ctx->launches += 1;
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(&best, d_best, 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        if (best != ~0ull) break;
+    }
+    if (best != ~0ull) {
+        *feerate_out = (int64_t)best;
+        *fee_out = best * weight / 1000;
+    }
     return SV_OK;
 }
 

@@ -219,23 +219,21 @@ SV_HD void sha_stream_final_double(sha256_stream& c, u8 out32[32]) {
     }
 }
 
-// Returns false only if the sighash type has bits above the low byte (libwally refuses those, tx_io.c:682); there is no
-// bound on script sizes.  hashOutputs: by default the transaction has ONE output (output_amount, scriptPubKey span) —
-// the HTLC-transaction shape; with pad == SV_TX_OUTPUTS_SERIALIZED the out_script span holds the serialised outputs to
-// commit to (amount || CompactSize || script, concatenated: all of them for SIGHASH_ALL, the one at the input's index
-// for SIGHASH_SINGLE, tx_io.c:714-737) — what check_tx_sig's adapter passes for commitment transactions.  With
-// SV_TX_INPUTS_SERIALIZED hashPrevouts / hashSequence run over the supplied spans (multi-input transactions).
-SV_HD bool bip143_sighash(u8 out32[32], const sv_tx_item& t, const u8* blob) {
-    if (t.sighash_type & 0xffffff00u) {
-        for (int i = 0; i < 32; i++) out32[i] = 0;
-        return false;
-    }
+// The sighash is built in three steps: bip143_prefix (the preimage up to and including nSequence), bip143_hash_outputs
+// and bip143_tail.  bip143_sighash runs them in turn; onchaind's fee grind (k_grind) runs the prefix once and the other
+// two once per candidate output amount, so both paths hash with the same code.
+//
+// Prefix: false only if the sighash type has bits above the low byte (libwally refuses those, tx_io.c:682); there is no
+// bound on script sizes.  With SV_TX_INPUTS_SERIALIZED hashPrevouts / hashSequence run over the supplied spans
+// (multi-input transactions).
+SV_HD bool bip143_prefix(sha256_stream& c, const sv_tx_item& t, const u8* blob) {
+    sha_stream_init(c);
+    if (t.sighash_type & 0xffffff00u) return false;
     const bool acp = (t.sighash_type & 0x80u) != 0;
     const u32 base = t.sighash_type & 0x1fu;
     const bool sh_none = base == 2, sh_single = base == 3;
-    u8 h_prev[32], h_seq[32], h_out[32];
-    sha256_stream c;
-    for (int i = 0; i < 32; i++) { h_prev[i] = 0; h_seq[i] = 0; h_out[i] = 0; }
+    u8 h_prev[32], h_seq[32];
+    for (int i = 0; i < 32; i++) { h_prev[i] = 0; h_seq[i] = 0; }
     const bool multi_in = (t.flags & SV_TX_INPUTS_SERIALIZED) != 0;
     if (!acp) {  // hashPrevouts
         sha_stream_init(c);
@@ -252,17 +250,6 @@ SV_HD bool bip143_sighash(u8 out32[32], const sv_tx_item& t, const u8* blob) {
         else sha_stream_le(c, t.sequence, 4);
         sha_stream_final_double(c, h_seq);
     }
-    if (!sh_none && !(t.flags & SV_TX_OUTPUTS_ZERO)) {  // hashOutputs
-        sha_stream_init(c);
-        if (t.flags & SV_TX_OUTPUTS_SERIALIZED) {
-            sha_stream_put(c, blob + t.out_script_off, t.out_script_len);
-        } else {
-            sha_stream_le(c, t.output_amount, 8);
-            sha_stream_varint(c, t.out_script_len);
-            sha_stream_put(c, blob + t.out_script_off, t.out_script_len);
-        }
-        sha_stream_final_double(c, h_out);
-    }
     sha_stream_init(c);
     sha_stream_le(c, t.version, 4);
     sha_stream_put(c, h_prev, 32);
@@ -273,9 +260,45 @@ SV_HD bool bip143_sighash(u8 out32[32], const sv_tx_item& t, const u8* blob) {
     sha_stream_put(c, blob + t.script_off, t.script_len);
     sha_stream_le(c, t.input_amount, 8);
     sha_stream_le(c, t.sequence, 4);
+    return true;
+}
+
+// hashOutputs.  By default the transaction has ONE output (output_amount, scriptPubKey span) — the HTLC-transaction
+// shape; with SV_TX_OUTPUTS_SERIALIZED the out_script span holds the serialised outputs to commit to (amount ||
+// CompactSize || script, concatenated: all of them for SIGHASH_ALL, the one at the input's index for SIGHASH_SINGLE,
+// tx_io.c:714-737) — what check_tx_sig's adapter passes for commitment transactions.  32 zero bytes for SIGHASH_NONE and
+// SV_TX_OUTPUTS_ZERO.
+SV_HD void bip143_hash_outputs(u8 h_out[32], const sv_tx_item& t, const u8* blob, u64 output_amount) {
+    for (int i = 0; i < 32; i++) h_out[i] = 0;
+    if ((t.sighash_type & 0x1fu) == 2 || (t.flags & SV_TX_OUTPUTS_ZERO)) return;
+    sha256_stream c;
+    sha_stream_init(c);
+    if (t.flags & SV_TX_OUTPUTS_SERIALIZED) {
+        sha_stream_put(c, blob + t.out_script_off, t.out_script_len);
+    } else {
+        sha_stream_le(c, output_amount, 8);
+        sha_stream_varint(c, t.out_script_len);
+        sha_stream_put(c, blob + t.out_script_off, t.out_script_len);
+    }
+    sha_stream_final_double(c, h_out);
+}
+
+// hashOutputs || nLocktime || sighash type appended to the prefix stream c (consumed), then the double hash
+SV_HD void bip143_tail(u8 out32[32], sha256_stream& c, const u8 h_out[32], const sv_tx_item& t) {
     sha_stream_put(c, h_out, 32);
     sha_stream_le(c, t.locktime, 4);
     sha_stream_le(c, t.sighash_type, 4);
     sha_stream_final_double(c, out32);
+}
+
+SV_HD bool bip143_sighash(u8 out32[32], const sv_tx_item& t, const u8* blob) {
+    sha256_stream c;
+    if (!bip143_prefix(c, t, blob)) {
+        for (int i = 0; i < 32; i++) out32[i] = 0;
+        return false;
+    }
+    u8 h_out[32];
+    bip143_hash_outputs(h_out, t, blob, t.output_amount);
+    bip143_tail(out32, c, h_out, t);
     return true;
 }

@@ -81,6 +81,8 @@ def load_library():
     lib.sv_verify_gossip_store_host.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp, sz, ctypes.POINTER(SvGossipStoreSummary)]
     lib.sv_get_last_gossip_store_timing.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
     lib.sv_verify_tx_host.argtypes = [vp, i, vp, vp, sz, vp, vp, sz, vp, vp]
+    lib.sv_grind_tx_fee_host.argtypes = [vp, i, vp, vp, sz, vp, vp, ctypes.c_uint64, ctypes.c_uint32, ctypes.c_uint32,
+                                         ctypes.POINTER(ctypes.c_int64), ctypes.POINTER(ctypes.c_uint64)]
     lib.sv_verify_samekey_host.argtypes = [vp, i, vp, vp, vp, sz, vp]
     lib.sv_verify_bolt12_host.argtypes = [vp, ctypes.c_char_p, ctypes.c_char_p, vp, sz, vp, vp, vp, vp, sz, vp, vp]
     lib.sv_verify_bolt12_tagged_host.argtypes = [vp, sz, vp, vp, vp, vp, sz, vp, vp, vp, vp, sz, vp, vp]
@@ -298,6 +300,22 @@ class SigVerifier:
                                                key.ctypes.data, sig64.ctypes.data, n, out.ctypes.data,
                                                sh.ctypes.data if want_sighash else None), "sv_verify_tx_host")
         return (out[:n], sh[:n]) if want_sighash else out[:n]
+
+    def grind_tx_fee(self, kind, tx, scripts, key, sig64, weight, min_feerate, max_feerate):
+        """onchaind's HTLC fee grind (onchaind/onchaind.c:389-437) in one call: the first feerate in [min_feerate,
+        max_feerate] whose fee = feerate * weight // 1000 makes sig64 verify for tx (an SvTx, flags 0) with its output set
+        to input_amount - fee.  Returns (feerate, fee), or (None, 0) when none verifies."""
+        k = np.ascontiguousarray(np.frombuffer(bytes(key), dtype=np.uint8))
+        s = np.ascontiguousarray(np.frombuffer(bytes(sig64), dtype=np.uint8))
+        if k.size != KEY_SIZE[kind] or s.size != 64:
+            raise ValueError("key or signature of the wrong size")
+        blob = np.frombuffer(bytes(scripts) if len(scripts) else b"\0", dtype=np.uint8)
+        f, fee = ctypes.c_int64(), ctypes.c_uint64()
+        self._check(self.lib.sv_grind_tx_fee_host(self._ctx, kind, ctypes.byref(tx), blob.ctypes.data, len(scripts),
+                                                  k.ctypes.data, s.ctypes.data, int(weight), int(min_feerate),
+                                                  int(max_feerate), ctypes.byref(f), ctypes.byref(fee)),
+                    "sv_grind_tx_fee_host")
+        return (None, 0) if f.value < 0 else (f.value, fee.value)
 
     def verify_bolt12(self, messagename, fieldname, streams, xonly, sig, want_sighash=False):
         """bolt12_check_signature (common/bolt12.c:80) for n raw TLV streams, Merkle root and sighash computed on the
