@@ -26,6 +26,8 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <stdio.h>
 #include <chrono>
+#include <map>
+#include <mutex>
 #include <stdlib.h>
 #include <string.h>
 #include <string>
@@ -1195,6 +1197,10 @@ __global__ void __launch_bounds__(256) k_probe_addc(int iters, u32* sink) {
 // paths at the sizes around it
 #define SV_SMALL_MAX_DEFAULT 8192
 #endif
+// smallest sizes of the grow-only context buffers (dev_buf::reserve)
+#define SV_ITEMS_FLOOR ((size_t)4096)        // staging, span arrays and launch-slot records, in items
+#define SV_GBUF_FLOOR ((size_t)1 << 16)      // g_buf and d_data, in bytes
+#define SV_SCRATCH_FLOOR ((size_t)1 << 20)   // dd_buf, sk_buf and b12_buf, in bytes
 struct sv_queue_item {
     int kind;
     u8 msg[32];
@@ -1202,81 +1208,95 @@ struct sv_queue_item {
     u8 sig[64];
 };
 
+struct sv_ctx;
+
+// A device allocation owned by the context or by one call, freed when its owner goes.  It converts to its pointer, so it
+// is used like one.  reserve() is the one place a buffer grows: see its definition below.
+template <typename T = u8>
+struct dev_buf {
+    T* p = nullptr;
+    size_t cap = 0;  // bytes
+    dev_buf() = default;
+    dev_buf(const dev_buf&) = delete;
+    dev_buf& operator=(const dev_buf&) = delete;
+    ~dev_buf() { if (p) cudaFree(p); }
+    operator T*() const { return p; }
+    template <typename U> U* at(size_t off) const { return reinterpret_cast<U*>(reinterpret_cast<u8*>(p) + off); }  // a slab piece
+    int reserve(sv_ctx* ctx, size_t bytes, size_t floor, cudaEvent_t wait = nullptr);
+};
+
+// Offsets of the pieces of one scratch slab, in the order they are taken; size is the slab's length so far.
+struct slab_layout {
+    size_t size = 0;
+    size_t take(size_t bytes, size_t align = 16) {
+        const size_t at = (size + align - 1) / align * align;
+        size = at + bytes;
+        return at;
+    }
+};
+
 struct sv_ctx {
-    int device;
-    int sm_count;
-    cudaStream_t stream;
-    cudaStream_t stream2;      // second compute stream: consecutive slices of a large host batch alternate streams, so the
-                               // thin last wave of one slice's curve kernel overlaps the next slice's kernels
-    cudaStream_t copy_stream;  // H2D of the next slice overlaps the kernels of the current one (sv_verify_host)
-    cudaEvent_t h2d_ev[8];
-    ge_mem* d_gtab;
-    u8* d_hot;          // [G comb table | slot 0 table slab | slot 1 table slab]
-    size_t hot_bytes, l2_persist, l2_max_persist, hot_slab, hot_gt;
-    cudaStream_t policy_streams[4];  // (stream, slab) pairs whose access-policy window is already set
-    const void* policy_slabs[4];
-    int l2_policy;      // sv_set_l2_policy (default on)
-    ge_mem* d_bases;
-    size_t scratch_bytes;
-    int main_grid;
+    int device = 0;
+    int sm_count = 0;
+    cudaStream_t stream = nullptr;
+    cudaStream_t stream2 = nullptr;      // second compute stream: consecutive slices of a large host batch alternate
+                                         // streams, so the thin last wave of one slice's curve kernel overlaps the next
+                                         // slice's kernels
+    cudaStream_t copy_stream = nullptr;  // H2D of the next slice overlaps the kernels of the current one (sv_verify_host)
+    cudaEvent_t h2d_ev[8] = {};
+    ge_mem* d_gtab = nullptr;
+    dev_buf<> d_hot;    // [slot 0 table slab | G comb table | slot 1 table slab]
+    size_t l2_persist = 0, l2_max_persist = 0, hot_slab = 0, hot_gt = 0;
+    cudaStream_t policy_streams[4] = {};  // (stream, slab) pairs whose access-policy window is already set
+    const void* policy_slabs[4] = {};
+    int l2_policy = 1;  // sv_set_l2_policy (default on)
+    dev_buf<ge_mem> d_bases;
+    size_t scratch_bytes = 0;
+    int main_grid = 0;
     // Launch slots: the scalar-side work records and the per-thread Q-table slab of one prep+main launch pair.  Two slots,
     // used round-robin, let launches issued on DIFFERENT streams overlap (the partially filled last wave of one batch's
     // curve kernel runs beside the next batch's kernels); a slot is re-used only after the event recorded behind its
     // previous use, so calls on one context can never corrupt each other whatever streams the caller picks.
     struct slot_t {
-        sv_work* d_work;
-        size_t work_cap;
-        qtab_entry* d_scratch;
-        cudaEvent_t done;
-        cudaStream_t last_stream;
-        int used;
+        dev_buf<sv_work> d_work;
+        qtab_entry* d_scratch = nullptr;
+        cudaEvent_t done = nullptr;
+        cudaStream_t last_stream = nullptr;
+        int used = 0;
     } slot[SV_NSLOTS];
-    unsigned next_slot;
+    unsigned next_slot = 0;
     // small-batch path: calls of up to small_max signatures run as ONE launch of k_small reading their inputs straight
     // from this pinned, device-mapped staging block (no H2D/D2H copy commands, no allocation)
-    size_t small_max, small_cap;
-    u8* h_small;
-    // key de-duplication scratch (hash table + index lists) and the table array of the distinct keys, grow-only
-    u8 *dd_buf, *sk_buf;
-    size_t dd_cap, sk_cap;
-    int dedup;  // gossip batches: look for repeated keys (sv_set_dedup; default on)
-    int nosqrt; // compressed-key ECDSA through the flow without the square root (default on; env SV_NOSQRT=0: measurement aid)
-    u32 last_distinct;
-    u32 last_repair;  // updates the last gossip burst re-resolved in its repair round
-    // growable device staging for the host-buffer entry points
-    size_t cap;  // items
-    u8 *d_msg, *d_key, *d_sig, *d_verdict;
+    size_t small_max = SV_SMALL_MAX_DEFAULT, small_cap = SV_SMALL_CAP;
+    u8* h_small = nullptr;
+    // key de-duplication scratch (hash table + index lists; also the BIP-340 batch scratch) and the table array of the
+    // distinct keys
+    dev_buf<> dd_buf, sk_buf;
+    int dedup = 1;   // gossip batches: look for repeated keys (sv_set_dedup; default on)
+    int nosqrt = 1;  // compressed-key ECDSA through the flow without the square root (default on; env SV_NOSQRT=0: measurement aid)
+    u32 last_distinct = 0;
+    u32 last_repair = 0;  // updates the last gossip burst re-resolved in its repair round
+    // device staging for the host-buffer entry points (ensure_staging)
+    dev_buf<> d_msg, d_key, d_sig, d_verdict;
     // raw-span staging
-    u8* d_data;
-    size_t data_cap;
-    u64* d_off;
-    u32* d_len;
-    size_t span_cap;
-    u32* d_sink;
-    // gossip ingest scratch (grow-only)
-    u8* g_buf;
-    size_t g_cap;
-    // BOLT12 field records and tree nodes (grow-only, sized by the counting pass)
-    u8* b12_buf;
-    size_t b12_cap;
-    int profiling;
-    cudaEvent_t ev[3];  // before prep, between prep and main, after main (profiling mode only)
-    cudaEvent_t b12_ev[2];  // around the BOLT12 parse / Merkle / sighash kernels (profiling mode only)
-    float gs_ms[4];         // last sv_verify_gossip_store_host: header walk, H2D, checksums, verification (profiling mode)
-    unsigned long long launches;
+    dev_buf<> d_data;
+    dev_buf<u64> d_off;
+    dev_buf<u32> d_len;
+    dev_buf<u32> d_sink;
+    // per-call scratch of the gossip, transaction, mixed, BOLT12 and fee-grind entry points (ensure_gbuf)
+    dev_buf<> g_buf;
+    // BOLT12 field records and tree nodes, sized by the counting pass
+    dev_buf<> b12_buf;
+    int profiling = 0;
+    cudaEvent_t ev[3] = {};      // before prep, between prep and main, after main (profiling mode only)
+    cudaEvent_t b12_ev[2] = {};  // around the BOLT12 parse / Merkle / sighash kernels (profiling mode only)
+    float gs_ms[4] = {};         // last sv_verify_gossip_store_host: header walk, H2D, checksums, verification (profiling mode)
+    unsigned long long launches = 0;
     std::vector<sv_queue_item> queue;
     std::string err;
 };
 
 static std::string g_create_err;
-
-// temporary device allocation released on every exit path
-struct dev_tmp {
-    void* p = nullptr;
-    ~dev_tmp() { if (p) cudaFree(p); }
-    cudaError_t alloc(size_t bytes) { return cudaMalloc(&p, bytes ? bytes : 1); }
-    template <typename T> T* as() const { return static_cast<T*>(p); }
-};
 
 // every entry point runs on the context's device and puts the caller's current device back on return
 struct dev_guard {
@@ -1302,6 +1322,30 @@ static int fail(sv_ctx* ctx, int code, const char* what, cudaError_t e) {
         if (e__ != cudaSuccess) return fail(ctx, e__ == cudaErrorMemoryAllocation ? SV_ERR_NOMEM : SV_ERR_CUDA, #call, e__); \
     } while (0)
 
+// Grow-only: nothing happens while the buffer holds `bytes`.  Otherwise it waits until no launch can still read the old
+// allocation (the whole device, or only the event `wait` when the caller knows the last user), frees it and allocates the
+// smallest power-of-two multiple of `floor` that holds `bytes`; a failure leaves the buffer empty.  floor == bytes is an
+// exact fit, for the fixed allocations and the per-call ones.  A successful reserve always leaves an allocation, even for
+// 0 bytes (floor 0 counts as 1), so the pointer handed to a copy or a kernel is never null.
+template <typename T>
+int dev_buf<T>::reserve(sv_ctx* ctx, size_t bytes, size_t floor, cudaEvent_t wait) {
+    if (p && bytes <= cap) return SV_OK;
+    if (bytes > ((size_t)-1) / 2) return fail(ctx, SV_ERR_NOMEM, "device buffer size", cudaSuccess);
+    if (p) {
+        CK(wait ? cudaEventSynchronize(wait) : cudaDeviceSynchronize());
+        cudaFree(p);
+        p = nullptr;
+        cap = 0;
+    }
+    size_t want = floor ? floor : 1;
+    while (want < bytes) want *= 2;
+    T* q = nullptr;
+    CK(cudaMalloc(&q, want));
+    p = q;
+    cap = want;
+    return SV_OK;
+}
+
 extern "C" size_t sv_key_size(int kind) {
     return kind == SV_KIND_ECDSA33 ? 33 : kind == SV_KIND_ECDSA_XY ? 64 : kind == SV_KIND_SCHNORR ? 32 : 0;
 }
@@ -1312,16 +1356,9 @@ extern "C" const char* sv_last_error(const sv_ctx* ctx) { return ctx ? ctx->err.
 static int acquire_slot(sv_ctx* ctx, size_t n, cudaStream_t st, sv_ctx::slot_t** out) {
     sv_ctx::slot_t* sl = &ctx->slot[ctx->next_slot++ % SV_NSLOTS];
     if (sl->used && sl->last_stream != st) CK(cudaStreamWaitEvent(st, sl->done, 0));
-    if (n > sl->work_cap) {
-        if (sl->used) CK(cudaEventSynchronize(sl->done));
-        size_t cap = sl->work_cap ? sl->work_cap : 4096;
-        while (cap < n) cap *= 2;
-        if (sl->d_work) cudaFree(sl->d_work);
-        sl->d_work = nullptr;
-        sl->work_cap = 0;
-        CK(cudaMalloc(&sl->d_work, cap * sizeof(sv_work)));
-        sl->work_cap = cap;
-    }
+    // only this slot's previous launch reads its records: the other slot's launch may go on running meanwhile
+    int rc = sl->d_work.reserve(ctx, n * sizeof(sv_work), SV_ITEMS_FLOOR * sizeof(sv_work), sl->done);
+    if (rc) return rc;
     *out = sl;
     return SV_OK;
 }
@@ -1332,19 +1369,101 @@ static int release_slot(sv_ctx* ctx, sv_ctx::slot_t* sl, cudaStream_t st) {
     return SV_OK;
 }
 static int ensure_staging(sv_ctx* ctx, size_t n) {
-    if (n <= ctx->cap) return SV_OK;
-    CK(cudaDeviceSynchronize());  // growth only: in-flight launches may still read the old buffers
-    size_t want = ctx->cap ? ctx->cap : 4096;
-    while (want < n) want *= 2;
-    n = want;
-    cudaFree(ctx->d_msg); cudaFree(ctx->d_key); cudaFree(ctx->d_sig); cudaFree(ctx->d_verdict);
-    ctx->d_msg = ctx->d_key = ctx->d_sig = ctx->d_verdict = nullptr;
-    ctx->cap = 0;
-    CK(cudaMalloc(&ctx->d_msg, n * 32));
-    CK(cudaMalloc(&ctx->d_key, n * 64));
-    CK(cudaMalloc(&ctx->d_sig, n * 64));
-    CK(cudaMalloc(&ctx->d_verdict, n));
-    ctx->cap = n;
+    int rc = ctx->d_msg.reserve(ctx, n * 32, SV_ITEMS_FLOOR * 32);
+    if (!rc) rc = ctx->d_key.reserve(ctx, n * 64, SV_ITEMS_FLOOR * 64);
+    if (!rc) rc = ctx->d_sig.reserve(ctx, n * 64, SV_ITEMS_FLOOR * 64);
+    if (!rc) rc = ctx->d_verdict.reserve(ctx, n, SV_ITEMS_FLOOR);
+    return rc;
+}
+static int ensure_spans(sv_ctx* ctx, size_t n) {
+    int rc = ctx->d_off.reserve(ctx, n * sizeof(u64), SV_ITEMS_FLOOR * sizeof(u64));
+    return rc ? rc : ctx->d_len.reserve(ctx, n * sizeof(u32), SV_ITEMS_FLOOR * sizeof(u32));
+}
+static int ensure_gbuf(sv_ctx* ctx, size_t bytes) { return ctx->g_buf.reserve(ctx, bytes, SV_GBUF_FLOOR); }
+
+#ifdef SV_COMB_SMEM
+// g_t8 is one pointer per device, read by the curve kernel of every context on that device, so the table it points to
+// belongs to the device, not to a context: the first context created on a device fills it from its G table (every
+// context's G table is the same), and it stays allocated for the life of the process.  The map is never destroyed, so
+// no cudaFree runs during static destruction.
+static int comb_t8_init(sv_ctx* ctx) {
+    struct table { dev_buf<ge_mem> t8; bool ready = false; };
+    static std::mutex mu;
+    static std::map<int, table>* tables = new std::map<int, table>;
+    std::lock_guard<std::mutex> lock(mu);
+    table& t = (*tables)[ctx->device];
+    if (t.ready) return SV_OK;
+    int rc = t.t8.reserve(ctx, 17 * 128 * sizeof(ge_mem), 17 * 128 * sizeof(ge_mem));
+    if (rc) return rc;
+    k_t8_fill<<<17, 128, 0, ctx->stream>>>(t.t8, ctx->d_gtab);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyToSymbolAsync(g_t8, &t.t8.p, sizeof(t.t8.p), 0, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    t.ready = true;
+    return SV_OK;
+}
+#endif
+
+// everything sv_create sets up after the defaults, on the context's device
+static int ctx_init(sv_ctx* ctx) {
+    cudaDeviceProp prop;
+    CK(cudaGetDeviceProperties(&prop, ctx->device));
+    ctx->sm_count = prop.multiProcessorCount;
+    CK(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
+    CK(cudaStreamCreateWithFlags(&ctx->stream2, cudaStreamNonBlocking));
+    CK(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
+    for (cudaEvent_t& e : ctx->h2d_ev) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    for (sv_ctx::slot_t& sl : ctx->slot) CK(cudaEventCreateWithFlags(&sl.done, cudaEventDisableTiming));
+    int rc = ctx->d_bases.reserve(ctx, 16 * sizeof(ge_mem), 16 * sizeof(ge_mem));
+    if (!rc) rc = ctx->d_sink.reserve(ctx, 64, 64);
+    if (rc) return rc;
+    CK(cudaHostAlloc((void**)&ctx->h_small, (size_t)SV_SMALL_CAP * (32 + 64 + 64 + 2), cudaHostAllocMapped | cudaHostAllocPortable));
+    int occ = 0;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_main<SV_KIND_ECDSA33>, SV_MAIN_BLOCK, SV_MAIN_SMEM));
+    if (occ < 1) occ = 1;
+    ctx->main_grid = ctx->sm_count * occ;
+    // deployment knob: leave a few CTA slots of the persistent curve kernel free for a collective's kernel that becomes
+    // ready while the grid is resident (bench.py sets 2 when it gathers verdict bitmaps over NCCL)
+    if (const char* e = getenv("SV_MAIN_GRID_RESERVE")) {
+        int r = atoi(e);
+        if (r > 0 && r < ctx->main_grid) ctx->main_grid -= r;
+    }
+    ctx->scratch_bytes = (size_t)ctx->main_grid * SV_MAIN_BLOCK * 8 * sizeof(qtab_entry);
+    // G table and the launch slots' per-thread table slabs live in ONE allocation: a single L2 access-policy window
+    // then covers everything the curve kernel reads more than once (see apply_l2_policy).  Layout [slab 0 | G table |
+    // slab 1]: each slot's slab is contiguous with the G table, so one window covers both.
+    static_assert(SV_NSLOTS == 2, "the hot-region layout below is for two launch slots");
+    slab_layout hot;
+    hot.take(ctx->scratch_bytes, 256);
+    const size_t o_gt = hot.take((size_t)SV_GT_ENTRIES * sizeof(ge_mem), 256), o_slab1 = hot.take(ctx->scratch_bytes, 256);
+    rc = ctx->d_hot.reserve(ctx, hot.size, hot.size);
+    if (rc) return rc;
+    ctx->slot[0].d_scratch = reinterpret_cast<qtab_entry*>(ctx->d_hot.p);
+    ctx->d_gtab = reinterpret_cast<ge_mem*>(ctx->d_hot + o_gt);
+    ctx->slot[1].d_scratch = reinterpret_cast<qtab_entry*>(ctx->d_hot + o_slab1);
+    const size_t sb = o_gt, gt = o_slab1 - o_gt;
+    ctx->hot_slab = sb;
+    ctx->hot_gt = gt;
+    // persisting L2 carve-out (as much as the device allows); failure is not an error: the hint is then simply absent
+    int maxp = 0;
+    if (cudaDeviceGetAttribute(&maxp, cudaDevAttrMaxPersistingL2CacheSize, ctx->device) == cudaSuccess && maxp > 0 &&
+        cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, (size_t)maxp < sb + gt ? (size_t)maxp : sb + gt) == cudaSuccess)
+        ctx->l2_persist = (size_t)maxp < sb + gt ? (size_t)maxp : sb + gt;  // one slab + the G table; the rest of L2 stays ordinary
+    else (void)cudaGetLastError();
+    ctx->l2_max_persist = maxp > 0 ? (size_t)maxp : 0;
+    k_gtable_bases<<<1, 32, 0, ctx->stream>>>(ctx->d_bases);
+    k_gtable_fill<<<(SV_GT_ENTRIES + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_gtab, ctx->d_bases);
+    ctx->launches += 2;
+    CK(cudaGetLastError());
+#ifdef SV_COMB_SMEM
+    rc = comb_t8_init(ctx);
+    if (rc) return rc;
+    const int smem = 17 * 128 * (int)sizeof(ge_mem);
+    CK(cudaFuncSetAttribute(k_main<SV_KIND_ECDSA33>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    CK(cudaFuncSetAttribute(k_main<SV_KIND_ECDSA_XY>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    CK(cudaFuncSetAttribute(k_main<SV_KIND_SCHNORR>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+#endif
+    CK(cudaStreamSynchronize(ctx->stream));
     return SV_OK;
 }
 
@@ -1360,109 +1479,16 @@ extern "C" int sv_create(sv_ctx** out, int device) {
     CK(dg__.enter(device));
     ctx = new sv_ctx();
     ctx->device = device;
-    ctx->cap = ctx->data_cap = ctx->span_cap = 0;
-    for (int i = 0; i < SV_NSLOTS; i++) { ctx->slot[i].d_work = nullptr; ctx->slot[i].work_cap = 0; ctx->slot[i].d_scratch = nullptr;
-                                          ctx->slot[i].done = nullptr; ctx->slot[i].last_stream = nullptr; ctx->slot[i].used = 0; }
-    ctx->next_slot = 0;
-    ctx->d_hot = nullptr;
-    ctx->hot_bytes = ctx->l2_persist = ctx->l2_max_persist = ctx->hot_slab = ctx->hot_gt = 0;
-    ctx->l2_policy = 1;
     if (const char* e = getenv("SV_L2_POLICY")) ctx->l2_policy = atoi(e) != 0;  // measurement aid
-    for (int i = 0; i < 4; i++) { ctx->policy_streams[i] = nullptr; ctx->policy_slabs[i] = nullptr; }
-    ctx->h_small = nullptr;
-    ctx->dd_buf = ctx->sk_buf = nullptr;
-    ctx->dd_cap = ctx->sk_cap = 0;
-    ctx->dedup = 1;
-    ctx->nosqrt = 1;
     if (const char* e = getenv("SV_NOSQRT")) ctx->nosqrt = atoi(e) != 0;
-    ctx->last_distinct = 0;
-    ctx->last_repair = 0;
-    ctx->small_cap = SV_SMALL_CAP;
-    ctx->small_max = SV_SMALL_MAX_DEFAULT;
     if (const char* e = getenv("SV_SMALL_MAX")) ctx->small_max = (size_t)strtoull(e, nullptr, 10);
     if (ctx->small_max > ctx->small_cap) ctx->small_max = ctx->small_cap;
-    ctx->d_msg = ctx->d_key = ctx->d_sig = ctx->d_verdict = ctx->d_data = nullptr;
-    ctx->d_off = nullptr; ctx->d_len = nullptr;
-    ctx->launches = 0;
-    ctx->g_buf = nullptr;
-    ctx->g_cap = 0;
-    ctx->b12_buf = nullptr;
-    ctx->b12_cap = 0;
-    ctx->profiling = 0;
-    ctx->ev[0] = ctx->ev[1] = ctx->ev[2] = nullptr;
-    ctx->b12_ev[0] = ctx->b12_ev[1] = nullptr;
-    ctx->stream = ctx->stream2 = ctx->copy_stream = nullptr;
-    for (int i = 0; i < 8; i++) ctx->h2d_ev[i] = nullptr;
-    cudaDeviceProp prop;
-    e = cudaGetDeviceProperties(&prop, device);
-    if (e != cudaSuccess) { int rc = fail(nullptr, SV_ERR_CUDA, "cudaGetDeviceProperties", e); delete ctx; return rc; }
-    ctx->sm_count = prop.multiProcessorCount;
-    int rc = SV_OK;
-    do {
-#define CK2(call) { cudaError_t e2 = (call); if (e2 != cudaSuccess) { rc = fail(nullptr, e2 == cudaErrorMemoryAllocation ? SV_ERR_NOMEM : SV_ERR_CUDA, #call, e2); break; } }
-        CK2(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
-        CK2(cudaStreamCreateWithFlags(&ctx->stream2, cudaStreamNonBlocking));
-        CK2(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
-        for (int i = 0; i < 8 && rc == SV_OK; i++) CK2(cudaEventCreateWithFlags(&ctx->h2d_ev[i], cudaEventDisableTiming));
-        if (rc != SV_OK) break;
-        // G table and the launch slots' per-thread table slabs live in ONE allocation: a single L2 access-policy window
-        // then covers everything the curve kernel reads more than once (see apply_l2_policy)
-        CK2(cudaMalloc(&ctx->d_bases, 16 * sizeof(ge_mem)));
-        CK2(cudaMalloc(&ctx->d_sink, 64));
-        CK2(cudaHostAlloc((void**)&ctx->h_small, (size_t)SV_SMALL_CAP * (32 + 64 + 64 + 2), cudaHostAllocMapped | cudaHostAllocPortable));
-        int occ = 0;
-        CK2(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_main<SV_KIND_ECDSA33>, SV_MAIN_BLOCK, SV_MAIN_SMEM));
-        if (occ < 1) occ = 1;
-        ctx->main_grid = ctx->sm_count * occ;
-        // deployment knob: leave a few CTA slots of the persistent curve kernel free for a collective's kernel that becomes
-        // ready while the grid is resident (bench.py sets 2 when it gathers verdict bitmaps over NCCL)
-        if (const char* e = getenv("SV_MAIN_GRID_RESERVE")) {
-            int r = atoi(e);
-            if (r > 0 && r < ctx->main_grid) ctx->main_grid -= r;
-        }
-        ctx->scratch_bytes = (size_t)ctx->main_grid * SV_MAIN_BLOCK * 8 * sizeof(qtab_entry);
-        {
-            size_t gt = ((size_t)SV_GT_ENTRIES * sizeof(ge_mem) + 255) & ~(size_t)255;
-            size_t sb = (ctx->scratch_bytes + 255) & ~(size_t)255;
-            ctx->hot_bytes = gt + SV_NSLOTS * sb;
-            CK2(cudaMalloc(&ctx->d_hot, ctx->hot_bytes));
-            // layout [slab 0 | G table | slab 1]: each slot's slab is contiguous with the G table, so one window covers both
-            static_assert(SV_NSLOTS == 2, "the hot-region layout below is for two launch slots");
-            ctx->slot[0].d_scratch = reinterpret_cast<qtab_entry*>(ctx->d_hot);
-            ctx->d_gtab = reinterpret_cast<ge_mem*>(ctx->d_hot + sb);
-            ctx->slot[1].d_scratch = reinterpret_cast<qtab_entry*>(ctx->d_hot + sb + gt);
-            ctx->hot_slab = sb;
-            ctx->hot_gt = gt;
-            // persisting L2 carve-out (as much as the device allows); failure is not an error: the hint is then simply absent
-            int maxp = 0;
-            if (cudaDeviceGetAttribute(&maxp, cudaDevAttrMaxPersistingL2CacheSize, device) == cudaSuccess && maxp > 0 &&
-                cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, (size_t)maxp < sb + gt ? (size_t)maxp : sb + gt) == cudaSuccess)
-                ctx->l2_persist = (size_t)maxp < sb + gt ? (size_t)maxp : sb + gt;  // one slab + the G table; the rest of L2 stays ordinary
-            else (void)cudaGetLastError();
-            ctx->l2_max_persist = maxp > 0 ? (size_t)maxp : 0;
-        }
-        for (int i = 0; i < SV_NSLOTS && rc == SV_OK; i++) CK2(cudaEventCreateWithFlags(&ctx->slot[i].done, cudaEventDisableTiming));
-        if (rc != SV_OK) break;
-        k_gtable_bases<<<1, 32, 0, ctx->stream>>>(ctx->d_bases);
-        k_gtable_fill<<<(SV_GT_ENTRIES + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_gtab, ctx->d_bases);
-        ctx->launches += 2;
-        CK2(cudaGetLastError());
-#ifdef SV_COMB_SMEM
-        {
-            ge_mem* t8 = nullptr;
-            CK2(cudaMalloc(&t8, 17 * 128 * sizeof(ge_mem)));
-            k_t8_fill<<<17, 128, 0, ctx->stream>>>(t8, ctx->d_gtab);
-            CK2(cudaMemcpyToSymbolAsync(g_t8, &t8, sizeof(t8), 0, cudaMemcpyHostToDevice, ctx->stream));
-            const int smem = 17 * 128 * (int)sizeof(ge_mem);
-            CK2(cudaFuncSetAttribute(k_main<SV_KIND_ECDSA33>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-            CK2(cudaFuncSetAttribute(k_main<SV_KIND_ECDSA_XY>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-            CK2(cudaFuncSetAttribute(k_main<SV_KIND_SCHNORR>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        }
-#endif
-        CK2(cudaStreamSynchronize(ctx->stream));
-#undef CK2
-    } while (0);
-    if (rc != SV_OK) { sv_destroy(ctx); return rc; }
+    int rc = ctx_init(ctx);
+    if (rc) {
+        g_create_err = ctx->err;
+        sv_destroy(ctx);
+        return rc;
+    }
     *out = ctx;
     return SV_OK;
 }
@@ -1472,22 +1498,14 @@ extern "C" void sv_destroy(sv_ctx* ctx) {
     dev_guard dg__;
     dg__.enter(ctx->device);
     cudaDeviceSynchronize();
-    cudaFree(ctx->d_hot); cudaFree(ctx->d_bases); cudaFree(ctx->d_sink);
     if (ctx->h_small) cudaFreeHost(ctx->h_small);
-    cudaFree(ctx->dd_buf); cudaFree(ctx->sk_buf);
-    for (int i = 0; i < SV_NSLOTS; i++) {
-        cudaFree(ctx->slot[i].d_work);
-        if (ctx->slot[i].done) cudaEventDestroy(ctx->slot[i].done);
-    }
-    cudaFree(ctx->d_msg); cudaFree(ctx->d_key); cudaFree(ctx->d_sig); cudaFree(ctx->d_verdict);
-    cudaFree(ctx->d_data); cudaFree(ctx->d_off); cudaFree(ctx->d_len); cudaFree(ctx->g_buf); cudaFree(ctx->b12_buf);
-    for (int i = 0; i < 3; i++) if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
-    for (int i = 0; i < 2; i++) if (ctx->b12_ev[i]) cudaEventDestroy(ctx->b12_ev[i]);
-    for (int i = 0; i < 8; i++) if (ctx->h2d_ev[i]) cudaEventDestroy(ctx->h2d_ev[i]);
-    if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
-    if (ctx->stream2) cudaStreamDestroy(ctx->stream2);
-    if (ctx->stream) cudaStreamDestroy(ctx->stream);
-    delete ctx;
+    for (sv_ctx::slot_t& sl : ctx->slot)
+        if (sl.done) cudaEventDestroy(sl.done);
+    for (cudaEvent_t e : ctx->ev) if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : ctx->b12_ev) if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : ctx->h2d_ev) if (e) cudaEventDestroy(e);
+    for (cudaStream_t s : {ctx->copy_stream, ctx->stream2, ctx->stream}) if (s) cudaStreamDestroy(s);
+    delete ctx;  // the device buffers free themselves
 }
 
 extern "C" int sv_get_info(const sv_ctx* ctx, sv_info* info) {
@@ -1507,8 +1525,19 @@ extern "C" int sv_get_info(const sv_ctx* ctx, sv_info* info) {
     return SV_OK;
 }
 
-// launch prep + main on device-resident SoA arrays.  *used (optional) receives the slot whose work records the launch
-// wrote (the gossip status kernel reads their flags afterwards, on the same stream).
+// the ECDSA scalar side of n signatures into the work records (two launches)
+static void launch_ecdsa_prep(sv_ctx* ctx, const u8* d_msg, const u8* d_sig, size_t n, sv_work* work, cudaStream_t st) {
+    size_t threads = (n + SV_PREP_BATCH - 1) / SV_PREP_BATCH;
+    k_prep_inv<<<(unsigned)((threads + 63) / 64), 64, 0, st>>>(d_msg, d_sig, n, work);
+    k_prep_finish<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(d_msg, d_sig, n, work);
+    ctx->launches += 2;
+}
+// grid of a curve kernel over n items: one thread per item, at most the persistent grid
+static unsigned main_grid_for(const sv_ctx* ctx, size_t n) {
+    size_t want = (n + SV_MAIN_BLOCK - 1) / SV_MAIN_BLOCK;
+    return (unsigned)(want < (size_t)ctx->main_grid ? want : (size_t)ctx->main_grid);
+}
+
 // ECDSA batch with repeated keys: returns 1 if it handled the batch (enough repetition to pay), 0 if the caller should take
 // the ordinary path, < 0 on error.  Synchronises the stream once (the number of distinct keys sizes the table array).
 static int launch_verify_dedup(sv_ctx* ctx, int kind, const u8* d_msg, const u8* d_key, const u8* d_sig, size_t n,
@@ -1518,17 +1547,14 @@ static int launch_verify_dedup(sv_ctx* ctx, int kind, const u8* d_msg, const u8*
     const int keylen = (int)sv_key_size(kind);
     u32 cap = 1;
     while (cap < 2 * n) cap <<= 1;
-    size_t head = (size_t)cap * 4 + 3 * n * 4 + 64;  // [slots cap][rep n][tid n][replist n][counter]
-    if (head > ctx->dd_cap) {
-        CK(cudaDeviceSynchronize());
-        size_t want = ctx->dd_cap ? ctx->dd_cap : (1u << 20);
-        while (want < head) want *= 2;
-        cudaFree(ctx->dd_buf); ctx->dd_buf = nullptr; ctx->dd_cap = 0;
-        CK(cudaMalloc(&ctx->dd_buf, want));
-        ctx->dd_cap = want;
-    }
-    u32* slots = reinterpret_cast<u32*>(ctx->dd_buf);
-    u32 *rep = slots + cap, *tid = rep + n, *replist = tid + n, *counter = replist + n;
+    slab_layout head;  // [slots cap][rep n][tid n][replist n][counter]
+    const size_t o_slots = head.take(4 * (size_t)cap), o_rep = head.take(4 * n), o_tid = head.take(4 * n),
+                 o_replist = head.take(4 * n), o_counter = head.take(4);
+    int rc = ctx->dd_buf.reserve(ctx, head.size, SV_SCRATCH_FLOOR);
+    if (rc) return rc;
+    const dev_buf<>& B = ctx->dd_buf;
+    u32 *slots = B.at<u32>(o_slots), *rep = B.at<u32>(o_rep), *tid = B.at<u32>(o_tid), *replist = B.at<u32>(o_replist),
+        *counter = B.at<u32>(o_counter);
     CK(cudaMemsetAsync(slots, 0xFF, (size_t)cap * 4, st));
     CK(cudaMemsetAsync(counter, 0, 4, st));
     unsigned gb = (unsigned)((n + 255) / 256);
@@ -1541,30 +1567,19 @@ static int launch_verify_dedup(sv_ctx* ctx, int kind, const u8* d_msg, const u8*
     CK(cudaStreamSynchronize(st));
     if (distinct_out) *distinct_out = distinct;
     if ((size_t)distinct * 10 > n * 6) return 0;  // fewer than 40 % repeats: the per-thread tables are as cheap
-    size_t need_sk = (size_t)distinct * sizeof(sv_shared_key);
-    if (need_sk > ctx->sk_cap) {
-        CK(cudaDeviceSynchronize());
-        size_t want = ctx->sk_cap ? ctx->sk_cap : (1u << 20);
-        while (want < need_sk) want *= 2;
-        cudaFree(ctx->sk_buf); ctx->sk_buf = nullptr; ctx->sk_cap = 0;
-        CK(cudaMalloc(&ctx->sk_buf, want));
-        ctx->sk_cap = want;
-    }
-    sv_shared_key* sk = reinterpret_cast<sv_shared_key*>(ctx->sk_buf);
+    rc = ctx->sk_buf.reserve(ctx, (size_t)distinct * sizeof(sv_shared_key), SV_SCRATCH_FLOOR);
+    if (rc) return rc;
+    sv_shared_key* sk = ctx->sk_buf.at<sv_shared_key>(0);
     sv_ctx::slot_t* sl = nullptr;
-    int rc = acquire_slot(ctx, n, st, &sl);
+    rc = acquire_slot(ctx, n, st, &sl);
     if (rc) return rc;
     if (ctx->profiling) cudaEventRecord(ctx->ev[0], st);
-    size_t threads = (n + SV_PREP_BATCH - 1) / SV_PREP_BATCH;
-    k_prep_inv<<<(unsigned)((threads + 63) / 64), 64, 0, st>>>(d_msg, d_sig, n, sl->d_work);
-    k_prep_finish<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(d_msg, d_sig, n, sl->d_work);
+    launch_ecdsa_prep(ctx, d_msg, d_sig, n, sl->d_work, st);
     if (ctx->profiling) cudaEventRecord(ctx->ev[1], st);
     k_sharedkey_build_many<<<(distinct + 127) / 128, 128, 0, st>>>(kind, d_key, keylen, replist, distinct, sk);
-    size_t want = (n + SV_MAIN_BLOCK - 1) / SV_MAIN_BLOCK;
-    unsigned grid = (unsigned)(want < (size_t)ctx->main_grid ? want : (size_t)ctx->main_grid);
-    k_main_shared<<<grid, SV_MAIN_BLOCK, 0, st>>>(sl->d_work, d_sig, n, ctx->d_gtab, sk, tid, d_verdict, d_aux);
+    k_main_shared<<<main_grid_for(ctx, n), SV_MAIN_BLOCK, 0, st>>>(sl->d_work, d_sig, n, ctx->d_gtab, sk, tid, d_verdict, d_aux);
     if (ctx->profiling) cudaEventRecord(ctx->ev[2], st);
-    ctx->launches += 4;
+    ctx->launches += 2;
     CK(cudaGetLastError());
     rc = release_slot(ctx, sl, st);
     return rc ? rc : 1;
@@ -1588,7 +1603,7 @@ static void apply_l2_policy(sv_ctx* ctx, cudaStream_t st, const void* slab) {
     memset(&v, 0, sizeof v);
     // slot 0: [slab 0 | G table], slot 1: [G table | slab 1] — the slab and the comb table, the two things a verification re-reads
     const bool first = slab == (const void*)ctx->slot[0].d_scratch;
-    v.accessPolicyWindow.base_ptr = first ? (void*)ctx->d_hot : (void*)ctx->d_gtab;
+    v.accessPolicyWindow.base_ptr = first ? (void*)ctx->d_hot.p : (void*)ctx->d_gtab;
     v.accessPolicyWindow.num_bytes = ctx->hot_slab + ctx->hot_gt;
     double ratio = 0.95 * (double)ctx->l2_persist / (double)(ctx->hot_slab + ctx->hot_gt);
     v.accessPolicyWindow.hitRatio = (float)(ratio > 1.0 ? 1.0 : ratio);
@@ -1640,15 +1655,12 @@ static int launch_verify(sv_ctx* ctx, int kind, const u8* d_msg, const u8* d_key
     if (ctx->profiling) cudaEventRecord(ctx->ev[0], st);
     if (kind == SV_KIND_SCHNORR) {
         k_prep_schnorr<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(d_msg, d_key, d_sig, n, work);
-    } else {
-        size_t threads = (n + SV_PREP_BATCH - 1) / SV_PREP_BATCH;
-        k_prep_inv<<<(unsigned)((threads + 63) / 64), 64, 0, st>>>(d_msg, d_sig, n, work);
-        k_prep_finish<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(d_msg, d_sig, n, work);
         ctx->launches += 1;
+    } else {
+        launch_ecdsa_prep(ctx, d_msg, d_sig, n, work, st);
     }
     if (ctx->profiling) cudaEventRecord(ctx->ev[1], st);
-    size_t want = (n + SV_MAIN_BLOCK - 1) / SV_MAIN_BLOCK;
-    unsigned grid = (unsigned)(want < (size_t)ctx->main_grid ? want : (size_t)ctx->main_grid);
+    const unsigned grid = main_grid_for(ctx, n);
     if (kind == SV_KIND_ECDSA33 && ctx->nosqrt) {
         // compressed keys: the flow that skips the square root (verify.cuh "without the square root")
         k_main<SV_KIND_ECDSA33_NS><<<grid, SV_MAIN_BLOCK, SV_MAIN_SMEM, st>>>(work, d_key, d_sig, n, ctx->d_gtab, sl->d_scratch, d_verdict, nullptr);
@@ -1671,7 +1683,7 @@ static int launch_verify(sv_ctx* ctx, int kind, const u8* d_msg, const u8* d_key
         ctx->launches += 1;
     }
     if (ctx->profiling) cudaEventRecord(ctx->ev[2], st);
-    ctx->launches += 2;
+    ctx->launches += 1;
     if (d_bitmap) {
         size_t nb = (n + 255) / 256;
         k_pack_bitmap<<<(unsigned)nb, 256, 0, st>>>(d_verdict, n, d_bitmap);
@@ -1752,6 +1764,26 @@ extern "C" int sv_sync(sv_ctx* ctx, void* stream) {
 #define SV_HOST_CHUNK (1u << 21)
 #endif
 
+// Small batch (n <= small_max): inputs go through the pinned staging block, the kernel reads them over the bus itself and
+// writes the verdict bytes back the same way: one launch and one stream synchronisation, nothing else.  same_key: `key` is
+// one key, repeated for every item.
+static int verify_small_host(sv_ctx* ctx, int kind, const u8* msg32, const u8* key, bool same_key, const u8* sig64, size_t n,
+                             u8* verdicts) {
+    const size_t ks = sv_key_size(kind);
+    u8 *hm = ctx->h_small, *hk = hm + 32 * ctx->small_cap, *hs = hk + 64 * ctx->small_cap, *hv = hs + 64 * ctx->small_cap;
+    memcpy(hm, msg32, 32 * n);
+    if (same_key)
+        for (size_t i = 0; i < n; i++) memcpy(hk + ks * i, key, ks);
+    else
+        memcpy(hk, key, ks * n);
+    memcpy(hs, sig64, 64 * n);
+    int rc = launch_small(ctx, kind, hm, hk, hs, n, hv, nullptr, ctx->stream);
+    if (rc) return rc;
+    CK(cudaStreamSynchronize(ctx->stream));
+    memcpy(verdicts, hv, n);
+    return SV_OK;
+}
+
 extern "C" int sv_verify_host(sv_ctx* ctx, int kind, const uint8_t* msg32, const uint8_t* key, const uint8_t* sig64,
                               size_t n, uint8_t* verdicts) {
     size_t ks_ = sv_key_size(kind);
@@ -1759,19 +1791,7 @@ extern "C" int sv_verify_host(sv_ctx* ctx, int kind, const uint8_t* msg32, const
     if (n == 0) return SV_OK;
     dev_guard dg__;
     CK(dg__.enter(ctx->device));
-    if (n <= ctx->small_max) {
-        // small batch: inputs go through the pinned staging block, the kernel reads them over the bus itself and writes the
-        // verdict bytes back the same way: one launch and one stream synchronisation, nothing else
-        u8 *hm = ctx->h_small, *hk = hm + 32 * ctx->small_cap, *hs = hk + 64 * ctx->small_cap, *hv = hs + 64 * ctx->small_cap;
-        memcpy(hm, msg32, 32 * n);
-        memcpy(hk, key, ks_ * n);
-        memcpy(hs, sig64, 64 * n);
-        int rc = launch_small(ctx, kind, hm, hk, hs, n, hv, nullptr, ctx->stream);
-        if (rc) return rc;
-        CK(cudaStreamSynchronize(ctx->stream));
-        memcpy(verdicts, hv, n);
-        return SV_OK;
-    }
+    if (n <= ctx->small_max) return verify_small_host(ctx, kind, msg32, key, false, sig64, n, verdicts);
     size_t chunk = n < SV_HOST_CHUNK ? n : SV_HOST_CHUNK;
     int rc = ensure_staging(ctx, chunk);
     if (rc) return rc;
@@ -1817,17 +1837,9 @@ static int stage_spans(sv_ctx* ctx, const uint8_t* data, size_t data_len, const 
                        size_t n) {
     for (size_t i = 0; i < n; i++)
         if (off[i] > data_len || (size_t)len[i] > data_len - off[i]) return fail(ctx, SV_ERR_ARG, "span out of range", cudaSuccess);
-    if (data_len > ctx->data_cap) {
-        cudaFree(ctx->d_data); ctx->d_data = nullptr; ctx->data_cap = 0;
-        CK(cudaMalloc(&ctx->d_data, data_len ? data_len : 1));
-        ctx->data_cap = data_len;
-    }
-    if (n > ctx->span_cap) {
-        cudaFree(ctx->d_off); cudaFree(ctx->d_len); ctx->d_off = nullptr; ctx->d_len = nullptr; ctx->span_cap = 0;
-        CK(cudaMalloc(&ctx->d_off, n * sizeof(u64)));
-        CK(cudaMalloc(&ctx->d_len, n * sizeof(u32)));
-        ctx->span_cap = n;
-    }
+    int rc = ctx->d_data.reserve(ctx, data_len, SV_GBUF_FLOOR);
+    if (!rc) rc = ensure_spans(ctx, n);
+    if (rc) return rc;
     CK(cudaMemcpyAsync(ctx->d_data, data, data_len, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_off, off, n * sizeof(u64), cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_len, len, n * sizeof(u32), cudaMemcpyHostToDevice, ctx->stream));
@@ -1932,47 +1944,32 @@ static int gossip_run(sv_ctx* ctx, const uint8_t* chain32, const uint8_t* blob, 
     // burst: item slots [items, items + n_cu) take the updates of a repair round
     size_t cap = items + n_cu ? items + n_cu : 1;
     int rc = ensure_staging(ctx, cap);
+    if (!rc) rc = ctx->d_data.reserve(ctx, blob_len, SV_GBUF_FLOOR);
+    if (!rc) rc = ensure_spans(ctx, cap > n_msgs ? cap : n_msgs);
     if (rc) return rc;
-    if (blob_len > ctx->data_cap) {
-        cudaFree(ctx->d_data); ctx->d_data = nullptr; ctx->data_cap = 0;
-        CK(cudaMalloc(&ctx->d_data, blob_len));
-        ctx->data_cap = blob_len;
-    }
-    size_t need = (cap > n_msgs ? cap : n_msgs);
-    if (need > ctx->span_cap) {
-        cudaFree(ctx->d_off); cudaFree(ctx->d_len); ctx->d_off = nullptr; ctx->d_len = nullptr; ctx->span_cap = 0;
-        CK(cudaMalloc(&ctx->d_off, need * sizeof(u64)));
-        CK(cudaMalloc(&ctx->d_len, need * sizeof(u32)));
-        ctx->span_cap = need;
-    }
-    // one grow-only slab: [msg_off u64][msg_len u32][item_base u32][status int][signers 33B][keyok 1B per item], and for a
-    // burst [kinds 1B][cand u32][repair list u32 (count, then indices)][chain_hash 32B][scid table u32], 16-byte aligned
-    auto a16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
+    // one slab: [msg_off u64][msg_len u32][item_base u32][status int][signers 33B][keyok 1B per item], and for a burst
+    // [kinds 1B][cand u32][repair list u32 (count, then indices)][chain_hash 32B][scid table u32]
     u32 tcap = 64;
     while (tcap < 2 * n_ca) tcap <<= 1;
-    const size_t ex = a16(n_msgs * (8 + 4 + 4 + 4 + 33) + cap), ex_cand = ex + a16(n_msgs), ex_rep = ex_cand + a16(4 * n_msgs),
-                 ex_chain = ex_rep + a16(4 * (n_msgs + 1)), ex_slots = ex_chain + 32;
-    size_t need_g = burst ? ex_slots + (size_t)tcap * 4 : n_msgs * (8 + 4 + 4 + 4 + 33) + cap + 64;
-    if (need_g > ctx->g_cap) {
-        CK(cudaDeviceSynchronize());
-        size_t gcap = ctx->g_cap ? ctx->g_cap : (1u << 16);
-        while (gcap < need_g) gcap *= 2;
-        cudaFree(ctx->g_buf); ctx->g_buf = nullptr; ctx->g_cap = 0;
-        CK(cudaMalloc(&ctx->g_buf, gcap));
-        ctx->g_cap = gcap;
-    }
-    u64* d_moff = reinterpret_cast<u64*>(ctx->g_buf);
-    u32* d_mlen = reinterpret_cast<u32*>(d_moff + n_msgs);
-    u32* d_base = d_mlen + n_msgs;
-    int* d_status = reinterpret_cast<int*>(d_base + n_msgs);
-    u8* d_signers = reinterpret_cast<u8*>(d_status + n_msgs);
-    u8* d_keyok = d_signers + 33 * n_msgs;
-    u8* d_kinds = burst ? ctx->g_buf + ex : nullptr;
-    u32* d_cand = reinterpret_cast<u32*>(ctx->g_buf + ex_cand);
-    u32* d_repair = reinterpret_cast<u32*>(ctx->g_buf + ex_rep);
-    u8* d_chain = burst ? ctx->g_buf + ex_chain : nullptr;
-    u32* d_slots = reinterpret_cast<u32*>(ctx->g_buf + ex_slots);
-    if (!cu_signers33) d_signers = nullptr;
+    slab_layout L;
+    const size_t o_moff = L.take(8 * n_msgs), o_mlen = L.take(4 * n_msgs), o_base = L.take(4 * n_msgs),
+                 o_status = L.take(4 * n_msgs), o_signers = L.take(33 * n_msgs), o_keyok = L.take(cap),
+                 o_kinds = L.take(burst ? n_msgs : 0), o_cand = L.take(burst ? 4 * n_msgs : 0),
+                 o_rep = L.take(burst ? 4 * (n_msgs + 1) : 0), o_chain = L.take(burst ? 32 : 0),
+                 o_slots = L.take(burst ? 4 * (size_t)tcap : 0);
+    rc = ensure_gbuf(ctx, L.size + 64);
+    if (rc) return rc;
+    const dev_buf<>& G = ctx->g_buf;
+    u64* d_moff = G.at<u64>(o_moff);
+    u32 *d_mlen = G.at<u32>(o_mlen), *d_base = G.at<u32>(o_base);
+    int* d_status = G.at<int>(o_status);
+    u8* d_signers = cu_signers33 ? G.at<u8>(o_signers) : nullptr;
+    u8* d_keyok = G.at<u8>(o_keyok);
+    u8* d_kinds = burst ? G.at<u8>(o_kinds) : nullptr;
+    u32* d_cand = burst ? G.at<u32>(o_cand) : nullptr;
+    u32* d_repair = burst ? G.at<u32>(o_rep) : nullptr;
+    u8* d_chain = burst ? G.at<u8>(o_chain) : nullptr;
+    u32* d_slots = burst ? G.at<u32>(o_slots) : nullptr;
     cudaStream_t st = ctx->stream;
     CK(cudaMemcpyAsync(ctx->d_data, blob, blob_len, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_moff, msg_off, n_msgs * sizeof(u64), cudaMemcpyHostToDevice, st));
@@ -2095,12 +2092,13 @@ extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, si
     if (ctx->profiling)
         for (cudaEvent_t& e : ev.e) CK(cudaEventCreate(&e));
     // the store is staged in a buffer of its own, freed on return: a store can be hundreds of MB
-    dev_tmp t_store, t_live;
-    CK(t_store.alloc(len));
-    CK(t_live.alloc(live_off.size() * 8 + 16));
-    u8* d_store = t_store.as<u8>();
-    u64* d_live = t_live.as<u64>();
-    u32* d_bad = reinterpret_cast<u32*>(d_live + live_off.size());
+    dev_buf<> d_store, t_live;
+    const size_t live_bytes = live_off.size() * 8 + 16;
+    int rc = d_store.reserve(ctx, len, len);
+    if (!rc) rc = t_live.reserve(ctx, live_bytes, live_bytes);
+    if (rc) return rc;
+    u64* d_live = t_live.at<u64>(0);
+    u32* d_bad = t_live.at<u32>(live_off.size() * 8);
     if (ev.e[0]) CK(cudaEventRecord(ev.e[0], st));
     CK(cudaMemcpyAsync(d_store, store, len, cudaMemcpyHostToDevice, st));
     if (!live_off.empty()) CK(cudaMemcpyAsync(d_live, live_off.data(), live_off.size() * 8, cudaMemcpyHostToDevice, st));
@@ -2141,33 +2139,28 @@ extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, si
     std::vector<int> mstatus(n_msgs);
     std::vector<u32> holder(n_msgs);
     if (n_msgs) {
-        int rc = ensure_staging(ctx, items);
+        rc = ensure_staging(ctx, items);
+        if (!rc) rc = ensure_spans(ctx, items);
         if (rc) return rc;
-        if (items > ctx->span_cap) {
-            cudaFree(ctx->d_off); cudaFree(ctx->d_len); ctx->d_off = nullptr; ctx->d_len = nullptr; ctx->span_cap = 0;
-            CK(cudaMalloc(&ctx->d_off, items * sizeof(u64)));
-            CK(cudaMalloc(&ctx->d_len, items * sizeof(u32)));
-            ctx->span_cap = items;
-        }
         size_t cub_bytes = 0;
         CK(cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const u64*)nullptr, (u64*)nullptr, (const u32*)nullptr,
                                            (u32*)nullptr, (int)nev, 0, 64, st));
         // one slab: per message [off u64][len u32][item base u32][status int][holder u32][signer 33B][kind 1B], per item
         // [keyok 1B], per event [off u64][key u64 x2][len u32][msg u32][value u32 x2][kind 1B][ok 1B], chain hash, sort scratch
-        size_t at = 0;
-        auto take = [&at](size_t bytes) { size_t o = at; at = (at + bytes + 15) & ~(size_t)15; return o; };
-        const size_t o_moff = take(8 * n_msgs), o_mlen = take(4 * n_msgs), o_base = take(4 * n_msgs),
-                     o_status = take(4 * n_msgs), o_holder = take(4 * n_msgs), o_sig = take(33 * n_msgs),
-                     o_kinds = take(n_msgs), o_keyok = take(items), o_eoff = take(8 * nev), o_key = take(8 * nev),
-                     o_key2 = take(8 * nev), o_elen = take(4 * nev), o_emsg = take(4 * nev), o_val = take(4 * nev),
-                     o_val2 = take(4 * nev), o_ekind = take(nev), o_ok = take(nev), o_chain = take(32), o_cub = take(cub_bytes);
-        dev_tmp t_slab;
-        CK(t_slab.alloc(at));
-        u8* s = t_slab.as<u8>();
-        u64 *d_moff = (u64*)(s + o_moff), *d_eoff = (u64*)(s + o_eoff), *d_key = (u64*)(s + o_key), *d_key2 = (u64*)(s + o_key2);
-        u32 *d_mlen = (u32*)(s + o_mlen), *d_base = (u32*)(s + o_base), *d_holder = (u32*)(s + o_holder),
-            *d_elen = (u32*)(s + o_elen), *d_emsg = (u32*)(s + o_emsg), *d_val = (u32*)(s + o_val), *d_val2 = (u32*)(s + o_val2);
-        int* d_status = (int*)(s + o_status);
+        slab_layout L;
+        const size_t o_moff = L.take(8 * n_msgs), o_mlen = L.take(4 * n_msgs), o_base = L.take(4 * n_msgs),
+                     o_status = L.take(4 * n_msgs), o_holder = L.take(4 * n_msgs), o_sig = L.take(33 * n_msgs),
+                     o_kinds = L.take(n_msgs), o_keyok = L.take(items), o_eoff = L.take(8 * nev), o_key = L.take(8 * nev),
+                     o_key2 = L.take(8 * nev), o_elen = L.take(4 * nev), o_emsg = L.take(4 * nev), o_val = L.take(4 * nev),
+                     o_val2 = L.take(4 * nev), o_ekind = L.take(nev), o_ok = L.take(nev), o_chain = L.take(32),
+                     o_cub = L.take(cub_bytes);
+        dev_buf<> s;
+        rc = s.reserve(ctx, L.size, L.size);
+        if (rc) return rc;
+        u64 *d_moff = s.at<u64>(o_moff), *d_eoff = s.at<u64>(o_eoff), *d_key = s.at<u64>(o_key), *d_key2 = s.at<u64>(o_key2);
+        u32 *d_mlen = s.at<u32>(o_mlen), *d_base = s.at<u32>(o_base), *d_holder = s.at<u32>(o_holder),
+            *d_elen = s.at<u32>(o_elen), *d_emsg = s.at<u32>(o_emsg), *d_val = s.at<u32>(o_val), *d_val2 = s.at<u32>(o_val2);
+        int* d_status = s.at<int>(o_status);
         u8 *d_signers = s + o_sig, *d_kinds = chain_hash32 ? s + o_kinds : nullptr, *d_keyok = s + o_keyok,
            *d_ekind = s + o_ekind, *d_ok = s + o_ok, *d_chain = chain_hash32 ? s + o_chain : nullptr;
         CK(cudaMemcpyAsync(d_moff, moff.data(), 8 * n_msgs, cudaMemcpyHostToDevice, st));
@@ -2274,19 +2267,9 @@ extern "C" int sv_verify_samekey_host(sv_ctx* ctx, int kind, const uint8_t* key,
     if (n == 0) return SV_OK;
     dev_guard dg__;
     CK(dg__.enter(ctx->device));
-    if (n <= ctx->small_max) {
-        // a commitment_signed carries at most 483 HTLC signatures: latency matters more than the 18 % of work a shared
-        // table saves, so small same-key batches take the small-batch path with the key repeated per item
-        u8 *hm = ctx->h_small, *hk = hm + 32 * ctx->small_cap, *hs = hk + 64 * ctx->small_cap, *hv = hs + 64 * ctx->small_cap;
-        memcpy(hm, msg32, 32 * n);
-        for (size_t i = 0; i < n; i++) memcpy(hk + ks * i, key, ks);
-        memcpy(hs, sig64, 64 * n);
-        int rcs = launch_small(ctx, kind, hm, hk, hs, n, hv, nullptr, ctx->stream);
-        if (rcs) return rcs;
-        CK(cudaStreamSynchronize(ctx->stream));
-        memcpy(verdicts, hv, n);
-        return SV_OK;
-    }
+    // a commitment_signed carries at most 483 HTLC signatures: latency matters more than the 18 % of work a shared table
+    // saves, so small same-key batches take the small-batch path with the key repeated per item
+    if (n <= ctx->small_max) return verify_small_host(ctx, kind, msg32, key, true, sig64, n, verdicts);
     int rc = ensure_staging(ctx, n);
     if (rc) return rc;
     cudaStream_t st = ctx->stream;
@@ -2299,21 +2282,15 @@ extern "C" int sv_verify_samekey_host(sv_ctx* ctx, int kind, const uint8_t* key,
     CK(cudaMemcpyAsync(ctx->d_msg, msg32, 32 * n, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->d_sig, sig64, 64 * n, cudaMemcpyHostToDevice, st));
     k_sharedkey_build<<<1, 32, 0, st>>>(kind, ctx->d_key, d_sk);
-    size_t threads = (n + SV_PREP_BATCH - 1) / SV_PREP_BATCH;
-    k_prep_inv<<<(unsigned)((threads + 63) / 64), 64, 0, st>>>(ctx->d_msg, ctx->d_sig, n, sl->d_work);
-    k_prep_finish<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(ctx->d_msg, ctx->d_sig, n, sl->d_work);
-    ctx->launches += 1;
-    size_t want = (n + SV_MAIN_BLOCK - 1) / SV_MAIN_BLOCK;
-    unsigned grid = (unsigned)(want < (size_t)ctx->main_grid ? want : (size_t)ctx->main_grid);
-    k_main_shared<<<grid, SV_MAIN_BLOCK, 0, st>>>(sl->d_work, ctx->d_sig, n, ctx->d_gtab, d_sk, nullptr, ctx->d_verdict, nullptr);
-    ctx->launches += 3;
-    cudaError_t ce = cudaGetLastError();
-    if (ce == cudaSuccess) ce = cudaEventRecord(sl->done, st);
-    sl->last_stream = st;
-    sl->used = 1;
-    if (ce == cudaSuccess) ce = cudaMemcpyAsync(verdicts, ctx->d_verdict, n, cudaMemcpyDeviceToHost, st);
-    if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-    if (ce != cudaSuccess) return fail(ctx, SV_ERR_CUDA, "sv_verify_samekey_host", ce);
+    launch_ecdsa_prep(ctx, ctx->d_msg, ctx->d_sig, n, sl->d_work, st);
+    k_main_shared<<<main_grid_for(ctx, n), SV_MAIN_BLOCK, 0, st>>>(sl->d_work, ctx->d_sig, n, ctx->d_gtab, d_sk, nullptr,
+                                                                   ctx->d_verdict, nullptr);
+    ctx->launches += 2;
+    CK(cudaGetLastError());
+    rc = release_slot(ctx, sl, st);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(verdicts, ctx->d_verdict, n, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
     return SV_OK;
 }
 
@@ -2334,25 +2311,15 @@ extern "C" int sv_verify_tx_host(sv_ctx* ctx, int kind, const sv_tx* txs, const 
             return fail(ctx, SV_ERR_ARG, "script span out of range", cudaSuccess);
     dev_guard dg__;
     CK(dg__.enter(ctx->device));
+    // transaction records + sighash-ok flags in the auxiliary slab (no allocation on the steady-state call path)
+    slab_layout L;
+    const size_t o_txs = L.take(n * sizeof(sv_tx_item)), o_ok = L.take(n);
     int rc = ensure_staging(ctx, n);
+    if (!rc) rc = ctx->d_data.reserve(ctx, scripts_len + 1, SV_GBUF_FLOOR);
+    if (!rc) rc = ensure_gbuf(ctx, L.size + 64);
     if (rc) return rc;
-    if (scripts_len + 1 > ctx->data_cap) {
-        cudaFree(ctx->d_data); ctx->d_data = nullptr; ctx->data_cap = 0;
-        CK(cudaMalloc(&ctx->d_data, scripts_len + 1));
-        ctx->data_cap = scripts_len + 1;
-    }
-    // transaction records + sighash-ok flags in the grow-only auxiliary slab (no allocation on the steady-state call path)
-    size_t need_g = n * sizeof(sv_tx_item) + n + 64;
-    if (need_g > ctx->g_cap) {
-        CK(cudaDeviceSynchronize());
-        size_t cap = ctx->g_cap ? ctx->g_cap : (1u << 16);
-        while (cap < need_g) cap *= 2;
-        cudaFree(ctx->g_buf); ctx->g_buf = nullptr; ctx->g_cap = 0;
-        CK(cudaMalloc(&ctx->g_buf, cap));
-        ctx->g_cap = cap;
-    }
-    sv_tx_item* d_txs = reinterpret_cast<sv_tx_item*>(ctx->g_buf);
-    u8* d_ok = ctx->g_buf + n * sizeof(sv_tx_item);
+    sv_tx_item* d_txs = ctx->g_buf.at<sv_tx_item>(o_txs);
+    u8* d_ok = ctx->g_buf + o_ok;
     cudaStream_t st = ctx->stream;
     CK(cudaMemcpyAsync(d_txs, txs, n * sizeof(sv_tx_item), cudaMemcpyHostToDevice, st));
     if (scripts_len) CK(cudaMemcpyAsync(ctx->d_data, scripts, scripts_len, cudaMemcpyHostToDevice, st));
@@ -2375,16 +2342,6 @@ extern "C" int sv_verify_tx_host(sv_ctx* ctx, int kind, const sv_tx* txs, const 
 }
 
 // ---- mixed batches: kinds[n] tags, keys in 64-byte slots (the first 33 / 64 / 32 bytes used) ----------------------
-static int ensure_gbuf(sv_ctx* ctx, size_t need) {
-    if (need <= ctx->g_cap) return SV_OK;
-    CK(cudaDeviceSynchronize());
-    size_t cap = ctx->g_cap ? ctx->g_cap : (1u << 16);
-    while (cap < need) cap *= 2;
-    cudaFree(ctx->g_buf); ctx->g_buf = nullptr; ctx->g_cap = 0;
-    CK(cudaMalloc(&ctx->g_buf, cap));
-    ctx->g_cap = cap;
-    return SV_OK;
-}
 // inputs already on the device; scratch = [count u32 x4][idx u32 x 3n]; staging = the context's SoA staging arrays
 static int mixed_device(sv_ctx* ctx, const u8* d_kinds, const u8* d_msg, const u8* d_key64, const u8* d_sig, size_t n,
                         u8* d_out, u32* d_scratch, cudaStream_t st) {
@@ -2426,7 +2383,7 @@ extern "C" int sv_verify_mixed_device(sv_ctx* ctx, const void* d_kinds, const vo
     if (rc) return rc;
     cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
     return mixed_device(ctx, (const u8*)d_kinds, (const u8*)d_msg32, (const u8*)d_key64, (const u8*)d_sig64, n,
-                        (u8*)d_verdicts, reinterpret_cast<u32*>(ctx->g_buf), st);
+                        (u8*)d_verdicts, ctx->g_buf.at<u32>(0), st);
 }
 extern "C" int sv_verify_mixed_host(sv_ctx* ctx, const uint8_t* kinds, const uint8_t* msg32, const uint8_t* key64,
                                     const uint8_t* sig64, size_t n, uint8_t* verdicts) {
@@ -2434,23 +2391,21 @@ extern "C" int sv_verify_mixed_host(sv_ctx* ctx, const uint8_t* kinds, const uin
     if (n == 0) return SV_OK;
     dev_guard dg__;
     CK(dg__.enter(ctx->device));
+    // aux slab: [count + idx lists][kinds n][msg 32n][key 64n][sig 64n][out n]
+    slab_layout L;
+    const size_t o_scratch = L.take(16 + 12 * n), o_kinds = L.take(n), o_m = L.take(32 * n), o_k = L.take(64 * n),
+                 o_s = L.take(64 * n), o_o = L.take(n);
     int rc = ensure_staging(ctx, n);
+    if (!rc) rc = ensure_gbuf(ctx, L.size + 64);
     if (rc) return rc;
-    // aux slab: [count + idx lists][kinds n][msg 32n][key 64n][sig 64n][out n], 16-byte aligned pieces
-    size_t a = (16 + 12 * n + 15) & ~(size_t)15, need = a + ((n + 15) & ~(size_t)15) * 2 + 160 * n + 64;
-    rc = ensure_gbuf(ctx, need);
-    if (rc) return rc;
-    u8* d_kinds = ctx->g_buf + a;
-    u8* d_m = d_kinds + ((n + 15) & ~(size_t)15);
-    u8* d_k = d_m + 32 * n;
-    u8* d_s = d_k + 64 * n;
-    u8* d_o = d_s + 64 * n;
+    u8 *d_kinds = ctx->g_buf + o_kinds, *d_m = ctx->g_buf + o_m, *d_k = ctx->g_buf + o_k, *d_s = ctx->g_buf + o_s,
+       *d_o = ctx->g_buf + o_o;
     cudaStream_t st = ctx->stream;
     CK(cudaMemcpyAsync(d_kinds, kinds, n, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_m, msg32, 32 * n, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_k, key64, 64 * n, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_s, sig64, 64 * n, cudaMemcpyHostToDevice, st));
-    rc = mixed_device(ctx, d_kinds, d_m, d_k, d_s, n, d_o, reinterpret_cast<u32*>(ctx->g_buf), st);
+    rc = mixed_device(ctx, d_kinds, d_m, d_k, d_s, n, d_o, ctx->g_buf.at<u32>(o_scratch), st);
     if (rc) return rc;
     CK(cudaMemcpyAsync(verdicts, d_o, n, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -2483,13 +2438,16 @@ extern "C" int sv_grind_tx_fee_host(sv_ctx* ctx, int kind, const sv_tx* tx, cons
     if (last < min_feerate) return SV_OK;  // the fee at min_feerate is already above the input: the loop breaks at once
     dev_guard dg__;
     CK(dg__.enter(ctx->device));
-    // staging: [state | 8 table entries | tx record | best | key 64 | sig 64 | witness script | output script]
-    const size_t o_tab = (sizeof(sv_grind_state) + 255) & ~(size_t)255, o_tx = o_tab + 8 * sizeof(qtab_entry),
-                 o_best = o_tx + sizeof(sv_tx_item), o_key = o_best + 16, o_sig = o_key + 64, o_blob = o_sig + 64;
+    // staging: [state | 8 table entries | tx record | best | key 64 | sig 64 | witness script | output script]; everything
+    // from the tx record on goes over in one copy
     const size_t blob_len = (size_t)tx->script_len + tx->out_script_len;
-    int rc = ensure_gbuf(ctx, o_blob + blob_len + 16);
+    slab_layout L;
+    const size_t o_state = L.take(sizeof(sv_grind_state), 256), o_tab = L.take(8 * sizeof(qtab_entry), 256),
+                 o_tx = L.take(sizeof(sv_tx_item)), o_best = L.take(16), o_key = L.take(64), o_sig = L.take(64),
+                 o_blob = L.take(blob_len);
+    int rc = ensure_gbuf(ctx, L.size + 16);
     if (rc) return rc;
-    std::vector<u8> h(o_blob + blob_len - o_tx, 0);
+    std::vector<u8> h(L.size - o_tx, 0);
     sv_tx_item t;
     memcpy(&t, tx, sizeof t);
     t.script_off = 0;
@@ -2501,10 +2459,10 @@ extern "C" int sv_grind_tx_fee_host(sv_ctx* ctx, int kind, const sv_tx* tx, cons
     if (tx->script_len) memcpy(h.data() + (o_blob - o_tx), scripts + tx->script_off, tx->script_len);
     if (tx->out_script_len) memcpy(h.data() + (o_blob - o_tx) + tx->script_len, scripts + tx->out_script_off, tx->out_script_len);
     u8* b = ctx->g_buf;
-    sv_grind_state* d_state = reinterpret_cast<sv_grind_state*>(b);
-    qtab_entry* d_tab = reinterpret_cast<qtab_entry*>(b + o_tab);
-    const sv_tx_item* d_tx = reinterpret_cast<const sv_tx_item*>(b + o_tx);
-    unsigned long long* d_best = reinterpret_cast<unsigned long long*>(b + o_best);
+    sv_grind_state* d_state = ctx->g_buf.at<sv_grind_state>(o_state);
+    qtab_entry* d_tab = ctx->g_buf.at<qtab_entry>(o_tab);
+    const sv_tx_item* d_tx = ctx->g_buf.at<sv_tx_item>(o_tx);
+    unsigned long long* d_best = ctx->g_buf.at<unsigned long long>(o_best);
     cudaStream_t st = ctx->stream;
     CK(cudaMemcpyAsync(b + o_tx, h.data(), h.size(), cudaMemcpyHostToDevice, st));
     k_grind_setup<<<1, 32, 0, st>>>(kind, b + o_key, b + o_sig, d_tx, b + o_blob, d_tab, d_state);
@@ -2545,16 +2503,16 @@ static int bolt12_pass(sv_ctx* ctx, size_t ntags, const char* const* messagename
     if (rc) return rc;
     rc = stage_spans(ctx, blob, blob_len, off, len, n);
     if (rc) return rc;
-    auto up16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
     // the tag table travels in one copy: [tag offsets u64 ntags][tag lengths u32 ntags][tag_of u32 n][tag bytes]
-    const size_t t_len = up16(8 * ntags), t_of = t_len + up16(4 * ntags), t_bytes = t_of + (tag_of ? up16(4 * n) : 0);
+    slab_layout T;
+    const size_t t_off = T.take(8 * ntags), t_len = T.take(4 * ntags), t_of = T.take(tag_of ? 4 * n : 0), t_bytes = T.take(0);
     std::vector<u8> tab(t_bytes);
     for (size_t t = 0; t < ntags; t++) {
         const u64 o = tab.size() - t_bytes;
         const size_t a = strlen(messagenames[t]), b = strlen(fieldnames[t]);
         if (9 + a + b > 0xFFFFFFFFu) return fail(ctx, SV_ERR_ARG, "tag too long", cudaSuccess);
         const u32 l = (u32)(9 + a + b);
-        memcpy(tab.data() + 8 * t, &o, 8);
+        memcpy(tab.data() + t_off + 8 * t, &o, 8);
         memcpy(tab.data() + t_len + 4 * t, &l, 4);
         tab.insert(tab.end(), "lightning", "lightning" + 9);
         tab.insert(tab.end(), messagenames[t], messagenames[t] + a);
@@ -2564,24 +2522,24 @@ static int bolt12_pass(sv_ctx* ctx, size_t ntags, const char* const* messagename
     const size_t nb = (n + SV_B12_SCAN - 1) / SV_B12_SCAN;
     // per-call scratch in the auxiliary slab: [cnt u32 n][base u64 n][block sums u64 nb+1][status int n][tree tags]
     // [sighash midstates 32 x ntags][tag table]
-    const size_t o_base = up16(4 * n), o_sums = o_base + 8 * n, o_status = up16(o_sums + 8 * (nb + 1)),
-                 o_tags = up16(o_status + 4 * n), o_mid = o_tags + up16(sizeof(b12_tags)), o_tab = o_mid + 32 * ntags,
-                 need = o_tab + tab.size() + 64;
-    rc = ensure_gbuf(ctx, need);
+    slab_layout L;
+    const size_t o_cnt = L.take(4 * n), o_base = L.take(8 * n), o_sums = L.take(8 * (nb + 1)), o_status = L.take(4 * n),
+                 o_tags = L.take(sizeof(b12_tags)), o_mid = L.take(32 * ntags), o_tab = L.take(tab.size());
+    rc = ensure_gbuf(ctx, L.size + 64);
     if (rc) return rc;
-    u32* d_cnt = reinterpret_cast<u32*>(ctx->g_buf);
-    u64* d_base = reinterpret_cast<u64*>(ctx->g_buf + o_base);
-    u64* d_sums = reinterpret_cast<u64*>(ctx->g_buf + o_sums);
-    int* d_status = reinterpret_cast<int*>(ctx->g_buf + o_status);
-    b12_tags* d_tags = reinterpret_cast<b12_tags*>(ctx->g_buf + o_tags);
-    u32* d_mid = reinterpret_cast<u32*>(ctx->g_buf + o_mid);
-    u8* d_tab = ctx->g_buf + o_tab;
+    const dev_buf<>& G = ctx->g_buf;
+    u32* d_cnt = G.at<u32>(o_cnt);
+    u64 *d_base = G.at<u64>(o_base), *d_sums = G.at<u64>(o_sums);
+    int* d_status = G.at<int>(o_status);
+    b12_tags* d_tags = G.at<b12_tags>(o_tags);
+    u32* d_mid = G.at<u32>(o_mid);
+    u8* d_tab = G + o_tab;
     cudaStream_t st = ctx->stream;
     CK(cudaMemcpyAsync(ctx->d_key, xonly32, 32 * n, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->d_sig, sig64, 64 * n, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_tab, tab.data(), tab.size(), cudaMemcpyHostToDevice, st));
     if (ctx->profiling) cudaEventRecord(ctx->b12_ev[0], st);
-    k_b12_tags<<<(unsigned)((ntags + 1 + 63) / 64), 64, 0, st>>>(d_tab + t_bytes, reinterpret_cast<const u64*>(d_tab),
+    k_b12_tags<<<(unsigned)((ntags + 1 + 63) / 64), 64, 0, st>>>(d_tab + t_bytes, reinterpret_cast<const u64*>(d_tab + t_off),
                                                               reinterpret_cast<const u32*>(d_tab + t_len), ntags, d_tags, d_mid);
     k_b12_count<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(ctx->d_data, ctx->d_off, ctx->d_len, n, d_cnt);
     k_b12_scan_local<<<(unsigned)nb, SV_B12_SCAN, 0, st>>>(d_cnt, n, d_base, d_sums);
@@ -2594,16 +2552,10 @@ static int bolt12_pass(sv_ctx* ctx, size_t ntags, const char* const* messagename
     CK(cudaStreamSynchronize(st));
     const size_t per_field = sizeof(b12_field) + 32;
     if (total > ((size_t)-1) / per_field) return fail(ctx, SV_ERR_NOMEM, "BOLT12 field scratch", cudaSuccess);
-    const size_t need_f = (size_t)total * per_field;
-    if (need_f > ctx->b12_cap) {
-        size_t want = ctx->b12_cap ? ctx->b12_cap : (1u << 20);
-        while (want < need_f) want *= 2;
-        cudaFree(ctx->b12_buf); ctx->b12_buf = nullptr; ctx->b12_cap = 0;
-        CK(cudaMalloc(&ctx->b12_buf, want));
-        ctx->b12_cap = want;
-    }
-    b12_field* d_recs = reinterpret_cast<b12_field*>(ctx->b12_buf);
-    u32* d_nodes = reinterpret_cast<u32*>(ctx->b12_buf + (size_t)total * sizeof(b12_field));
+    rc = ctx->b12_buf.reserve(ctx, (size_t)total * per_field, SV_SCRATCH_FLOOR);
+    if (rc) return rc;
+    b12_field* d_recs = ctx->b12_buf.at<b12_field>(0);
+    u32* d_nodes = ctx->b12_buf.at<u32>((size_t)total * sizeof(b12_field));
     k_b12_merkle<<<(unsigned)((n + SV_B12_WARPS - 1) / SV_B12_WARPS), 32 * SV_B12_WARPS, 0, st>>>(
         ctx->d_data, ctx->d_off, ctx->d_len, n, d_cnt, d_base, d_tags, d_mid,
         tag_of ? reinterpret_cast<const u32*>(d_tab + t_of) : nullptr, d_recs, d_nodes, ctx->d_msg);
@@ -2664,32 +2616,27 @@ extern "C" int sv_verify_schnorr_batch_host(sv_ctx* ctx, const uint8_t* msg32, c
     if (rc) return rc;
     const u32 groups = (u32)((n + SV_SB_GROUP - 1) / SV_SB_GROUP);
     // scratch: [seed 32][pts 2n x 96][t n x 32][S groups x W x 128][dig W x 4n][ok n][group_ok groups][out n][idx n x 4]
-    size_t o_pts = 64, o_t = o_pts + 2 * n * sizeof(qtab_entry), o_S = o_t + n * sizeof(sc),
-           o_dig = o_S + (size_t)groups * SV_SB_WINDOWS * sizeof(sv_jac), o_ok = (o_dig + (size_t)SV_SB_WINDOWS * 4 * n + 15) & ~(size_t)15,
-           o_gok = (o_ok + n + 15) & ~(size_t)15, o_out = (o_gok + groups + 15) & ~(size_t)15, o_idx = (o_out + n + 15) & ~(size_t)15,
-           need = o_idx + 4 * n + 64;
-    if (need > ctx->dd_cap) {
-        CK(cudaDeviceSynchronize());
-        size_t want = ctx->dd_cap ? ctx->dd_cap : (1u << 20);
-        while (want < need) want *= 2;
-        cudaFree(ctx->dd_buf); ctx->dd_buf = nullptr; ctx->dd_cap = 0;
-        CK(cudaMalloc(&ctx->dd_buf, want));
-        ctx->dd_cap = want;
-    }
-    u8* B = ctx->dd_buf;
-    qtab_entry* d_pts = reinterpret_cast<qtab_entry*>(B + o_pts);
-    sc* d_t = reinterpret_cast<sc*>(B + o_t);
-    sv_jac* d_S = reinterpret_cast<sv_jac*>(B + o_S);
-    signed char* d_dig = reinterpret_cast<signed char*>(B + o_dig);
+    slab_layout L;
+    const size_t o_seed = L.take(32), o_pts = L.take(2 * n * sizeof(qtab_entry), 64), o_t = L.take(n * sizeof(sc)),
+                 o_S = L.take((size_t)groups * SV_SB_WINDOWS * sizeof(sv_jac)), o_dig = L.take((size_t)SV_SB_WINDOWS * 4 * n),
+                 o_ok = L.take(n), o_gok = L.take(groups), o_out = L.take(n), o_idx = L.take(4 * n);
+    rc = ctx->dd_buf.reserve(ctx, L.size + 64, SV_SCRATCH_FLOOR);
+    if (rc) return rc;
+    const dev_buf<>& B = ctx->dd_buf;
+    u8* d_seed = B + o_seed;
+    qtab_entry* d_pts = B.at<qtab_entry>(o_pts);
+    sc* d_t = B.at<sc>(o_t);
+    sv_jac* d_S = B.at<sv_jac>(o_S);
+    signed char* d_dig = B.at<signed char>(o_dig);
     u8 *d_ok = B + o_ok, *d_gok = B + o_gok, *d_out = B + o_out;
-    u32* d_idx = reinterpret_cast<u32*>(B + o_idx);
+    u32* d_idx = B.at<u32>(o_idx);
     cudaStream_t st = ctx->stream;
-    CK(cudaMemcpyAsync(B, seed, 32, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_seed, seed, 32, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->d_msg, msg32, 32 * n, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->d_key, xonly32, 32 * n, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->d_sig, sig64, 64 * n, cudaMemcpyHostToDevice, st));
     if (ctx->profiling) cudaEventRecord(ctx->ev[0], st);
-    if (sv_batch_launch(ctx->d_msg, ctx->d_key, ctx->d_sig, n, B, d_pts, d_dig, d_t, d_ok, d_S, d_gok, d_out, ctx->d_gtab, st,
+    if (sv_batch_launch(ctx->d_msg, ctx->d_key, ctx->d_sig, n, d_seed, d_pts, d_dig, d_t, d_ok, d_S, d_gok, d_out, ctx->d_gtab, st,
                         ctx->profiling ? ctx->ev[1] : nullptr) != 0)
         return fail(ctx, SV_ERR_CUDA, "batch kernels", cudaGetLastError());
     if (ctx->profiling) cudaEventRecord(ctx->ev[2], st);
@@ -2779,17 +2726,18 @@ extern "C" int sv_selftest_host(sv_ctx* ctx, int op, const uint32_t* a, const ui
     if (n == 0) return SV_OK;
     dev_guard dg__;
     CK(dg__.enter(ctx->device));
-    dev_tmp ta, tb, to;
-    CK(ta.alloc(n * 32));
-    CK(tb.alloc(n * 32));
-    CK(to.alloc(n * 64));
+    dev_buf<u32> ta, tb, to;
+    int rc = ta.reserve(ctx, n * 32, n * 32);
+    if (!rc) rc = tb.reserve(ctx, n * 32, n * 32);
+    if (!rc) rc = to.reserve(ctx, n * 64, n * 64);
+    if (rc) return rc;
     cudaStream_t st = ctx->stream;
-    CK(cudaMemcpyAsync(ta.p, a, n * 32, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(tb.p, b, n * 32, cudaMemcpyHostToDevice, st));
-    k_selftest<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(op, ta.as<u32>(), tb.as<u32>(), n, to.as<u32>(), ctx->d_gtab);
+    CK(cudaMemcpyAsync(ta, a, n * 32, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(tb, b, n * 32, cudaMemcpyHostToDevice, st));
+    k_selftest<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(op, ta, tb, n, to, ctx->d_gtab);
     ctx->launches += 1;
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(out, to.p, n * 64, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(out, to, n * 64, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     return SV_OK;
 }
@@ -2821,7 +2769,8 @@ extern "C" int sv_probe(sv_ctx* ctx, int mode, double* ops_per_sec) {
     const int iters = (mode == 2 || mode == 3 || mode >= 9) ? 2000 : 4000;
     // modes 9/10: ONE warp on the whole device — the dependent-chain latency of fe_mul / fe_sqr (small-batch path)
     const int blocks = mode >= 9 ? 1 : ctx->sm_count * 8, threads = mode >= 9 ? 32 : 256;
-    cudaEvent_t e0, e1;
+    ev_set ev;
+    cudaEvent_t &e0 = ev.e[0], &e1 = ev.e[1];
     CK(cudaEventCreate(&e0));
     CK(cudaEventCreate(&e1));
     float best = 1e30f;
@@ -2847,8 +2796,6 @@ extern "C" int sv_probe(sv_ctx* ctx, int mode, double* ops_per_sec) {
         if (rep > 0 && ms < best) best = ms;
         ctx->launches += 1;
     }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
     // operations per thread per launch
     static const double per_iter[11] = {32.0, 32.0, 2.0, 2.0, 32.0, 32.0, 32.0, 64.0, 32.0, 2.0, 1.0};  // mode 10: two INDEPENDENT squaring chains -> one chain's rate
     // modes 9/10 report dependent operations per second of ONE thread (the two chains of the probe depend on each other)
