@@ -120,7 +120,7 @@ void cln_sigverify_shutdown(void);
  *   cln_sigverify_connect(path)   connect to the daemon's socket
  *   cln_sigverify_connect_fd(fd)  use an already-connected socket, e.g. a socketpair end inherited from the parent, the way
  *                                 lightningd hands fds to its subdaemons (the daemon side: cln_sigverifyd --fd N)
- * In client mode these functions send one request over one blocking connection per process and wait for the reply;
+ * In client mode these functions send one request over the process's one connection and wait for the reply;
  * they never create a context:
  *   check_signed_hash, check_signed_hash_nodeid, check_schnorr_sig, check_tx_sigs_batch   (sigverifyd_verify)
  *   bolt12_check_signature                                                              (sigverifyd_bolt12)
@@ -139,6 +139,61 @@ void cln_sigverify_shutdown(void);
  * and the calls, nothing changes. */
 int cln_sigverify_connect(const char *socket_path);
 int cln_sigverify_connect_fd(int fd);
+
+/* NON-BLOCKING CLIENT MODE: many checks in flight from one process.  A blocking call holds at most one request at the
+ * daemon; an event loop (ccan/io, libplugin) with many independent checks starts them as tickets instead, and the daemon
+ * serves everything the process has sent in the same launches, as it serves many processes.  Each _start below takes the
+ * arguments of the blocking function of the same name, plus where the answer goes and a continuation:
+ *
+ *   0    the answer is already in *ok / status and no callback follows: always in in-process mode (the _start calls the
+ *        blocking function), and for the local gates, which send nothing: check_tx_sig's sighash-type gate,
+ *        bolt12_check_signature's empty or not strictly ascending field array (false, as the device answers the blocking
+ *        call), sigcheck_gossip_batch with n == 0.
+ *   > 0  a ticket.  The answer is written to *ok / status[0..n), then done(arg) runs (done may be NULL).  The caller keeps
+ *        that output memory alive until the callback; every input is copied before the _start returns.
+ *
+ * Verdicts, statuses and aborts are exactly the blocking function's: the request is built by the same code and the reply
+ * passes the same checks.
+ * Ordering: callbacks run in ticket order, each exactly once, and only from cln_sigverify_process() or
+ * cln_sigverify_drain(), never from inside a _start or a blocking call.  A callback may call any function of this header,
+ * _start and blocking ones included.
+ * Blocking calls with tickets outstanding: the blocking call's request goes behind the unsent ones and it reads replies
+ * until its own arrives, writing the earlier tickets' answers on the way; their callbacks wait for the next
+ * cln_sigverify_process() (call it after such a blocking call: the socket may have nothing more to read).
+ * Back-pressure: writes never block; what the socket does not take stays in a buffer of this library.  While 1,024
+ * tickets await replies, or 64 MiB of requests are unsent, a _start first waits (as a blocking call would) until the
+ * oldest are answered or written; their callbacks still wait for cln_sigverify_process().  One request's own limits are the
+ * blocking function's (MAX_FRAME; a gossip burst is never split).
+ * Errors: a lost daemon, a short read, an error reply, a malformed reply or a reply out of request order abort(), as in
+ * blocking mode; nothing is ever reported as a bad signature.  cln_sigverify_shutdown() and a new connection discard the
+ * outstanding tickets without running their callbacks. */
+/* the continuation of a ticket */ typedef void (*cln_sigverify_done)(void *arg);
+
+uint64_t check_signed_hash_start(const struct sha256_double *hash, const secp256k1_ecdsa_signature *signature,
+                                 const struct pubkey *key, bool *ok, cln_sigverify_done done, void *arg);
+uint64_t check_signed_hash_nodeid_start(const struct sha256_double *hash, const secp256k1_ecdsa_signature *signature,
+                                        const struct node_id *id, bool *ok, cln_sigverify_done done, void *arg);
+uint64_t check_schnorr_sig_start(const struct sha256 *hash, const secp256k1_pubkey *pubkey, const struct bip340sig *sig,
+                                 bool *ok, cln_sigverify_done done, void *arg);
+uint64_t check_tx_sig_start(const struct bitcoin_tx *tx, size_t input_num, const u8 *redeemscript, const u8 *witness_script,
+                            const struct pubkey *key, const struct bitcoin_signature *sig, bool *ok, cln_sigverify_done done,
+                            void *arg);
+uint64_t bolt12_check_signature_start(const struct tlv_field *fields, const char *messagename, const char *fieldname,
+                                      const struct pubkey *key, const struct bip340sig *sig, bool *ok,
+                                      cln_sigverify_done done, void *arg);
+uint64_t sigcheck_gossip_batch_start(const u8 *chain_hash32, const u8 *const *msgs, const size_t *lens, size_t n,
+                                     const u8 *signer_kind, const struct node_id *signers, int *status,
+                                     cln_sigverify_done done, void *arg);
+
+/* The event loop's side.  cln_sigverify_fd(): the daemon socket to watch, -1 in in-process mode.
+ * cln_sigverify_events(): POLLIN while tickets are outstanding, | POLLOUT while request bytes are unsent (0: nothing to
+ * watch).  cln_sigverify_process(): never blocks; writes what the socket takes, reads what has arrived and runs the
+ * callbacks of the answered tickets in ticket order; returns the number of tickets still outstanding.
+ * cln_sigverify_drain(): blocks until no ticket is outstanding, running their callbacks. */
+int cln_sigverify_fd(void);
+short cln_sigverify_events(void);
+size_t cln_sigverify_process(void);
+void cln_sigverify_drain(void);
 
 bool check_signed_hash(const struct sha256_double *hash, const secp256k1_ecdsa_signature *signature,
                        const struct pubkey *key);
