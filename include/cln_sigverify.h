@@ -382,6 +382,31 @@ enum {
 };
 int sv_selftest_host(sv_ctx *ctx, int op, const uint32_t *a, const uint32_t *b, size_t n, uint32_t *out);
 
+/* ---- device-side self test of the group law and the scalar-multiplication schedules (TEST SUPPORT).  One op per item:
+ *      in[n][SV_STG_IN_WORDS] -> out[n][SV_STG_OUT_WORDS], 32-bit little-endian limbs.  A field element takes 8 words, a
+ *      Jacobian point 25 (x, y, z, then the infinity flag); field outputs are in the engine's weak form.  In the list,
+ *      "a" is the point at in[0..24], "b" the point at in[32..56] (affine: x, y only), "w" the work record built from
+ *      in[32..36] = k1 and in[40..44] = k2 (magnitude, sign in bit 31 of the last word, as SV_ST_PREPARE_U2 returns them)
+ *      and the comb digits of u1 = in[48..55]; "Q" is the affine point at in[0..15]. ---- */
+#define SV_STG_IN_WORDS 64
+#define SV_STG_OUT_WORDS 200
+enum {
+    SV_STG_GEJ_DOUBLE = 0,        /* 2a -> out[0..24] */
+    SV_STG_GEJ_ADD_GE = 1,        /* a + b (b affine) -> out[0..24], rzr -> out[32..39]; in[60] bit 0: r aliases a */
+    SV_STG_GEJ_ADD_GEJ = 2,       /* a + b -> out[0..24]; in[60] = 0: r separate, 1: r aliases a, 2: r aliases b */
+    SV_STG_GE_SET_XO = 3,         /* x = in[0..7], odd = in[8]: x -> out[0..7], y -> out[8..15], out[16] = x^3+7 is a residue */
+    SV_STG_QTABLE_BUILD = 4,      /* table of Q: entry e at out[24e..24e+23] (x, y, beta*x), zc -> out[192..199] */
+    SV_STG_ECMULT_LADDER_Q = 5,   /* table of Q, then ecmult_ladder_q with w -> out[0..24] (true coordinates) */
+    SV_STG_ECMULT_HALF_LADDER = 6, /* table of Q, then ecmult_half_ladder over the magnitude at in[32..36], lambda half iff
+                                      in[60] != 0 -> out[0..24] on the scaled curve (true Z = Z * zc), zc -> out[32..39] */
+    SV_STG_ECMULT_COMB_ADD = 7,   /* a + u1*G through ecmult_comb_add -> out[0..24] */
+    SV_STG_SMALL_COMB = 8,        /* u1*G through small_comb (from infinity) -> out[0..24] */
+    SV_STG_ECMULT_LADDER = 9,     /* table of Q, then ecmult_ladder with w (u1*G + u2*Q) -> out[0..24] */
+    SV_STG_NS_LINEAR_FORM = 10    /* X1, Y1, Zs = in[0..7], [8..15], [16..23], c = in[24..31], T = in[32..55], r = in[56..63]:
+                                     D, B, N, CG -> out[0..7], [8..15], [16..23], [24..31]; out[32] = exceptional */
+};
+int sv_selftest_group_host(sv_ctx *ctx, int op, const uint32_t *in, size_t n, uint32_t *out);
+
 /* ---- synthetic workload generator (benchmark / test support; NOT constant time, no secrets):
  *      item i gets secret key and nonce derived from (seed, i); writes msg32, key (per kind) and a
  *      VALID low-S ECDSA / BIP-340 signature to device arrays. ---- */

@@ -930,6 +930,13 @@ __global__ void __launch_bounds__(128) k_selftest(int op, const u32* __restrict_
 #pragma unroll
     for (int k = 0; k < 16; k++) out[16 * i + k] = R[k];
 }
+// ---- device-side self test of the group law and the multiplication schedules (test support; body in selftest.cuh) ---
+__global__ void __launch_bounds__(128) k_selftest_group(int op, const u32* __restrict__ in, size_t n, u32* __restrict__ out,
+                                                        const ge_mem* __restrict__ gtab) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    selftest_group_item(op, in + SV_STG_IN_WORDS * i, out + SV_STG_OUT_WORDS * i, gtab);
+}
 
 // ---- synthetic workload generator ---------------------------------------------------------------
 SV_D void synth_hash(u8 out[32], u64 seed, u64 idx, u32 tag) {
@@ -2738,6 +2745,25 @@ extern "C" int sv_selftest_host(sv_ctx* ctx, int op, const uint32_t* a, const ui
     ctx->launches += 1;
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(out, to, n * 64, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return SV_OK;
+}
+extern "C" int sv_selftest_group_host(sv_ctx* ctx, int op, const uint32_t* in, size_t n, uint32_t* out) {
+    if (!ctx || op < 0 || op > SV_STG_NS_LINEAR_FORM || (n && (!in || !out))) return SV_ERR_ARG;
+    if (n == 0) return SV_OK;
+    dev_guard dg__;
+    CK(dg__.enter(ctx->device));
+    const size_t ib = n * 4 * SV_STG_IN_WORDS, ob = n * 4 * SV_STG_OUT_WORDS;
+    dev_buf<u32> ti, to;
+    int rc = ti.reserve(ctx, ib, ib);
+    if (!rc) rc = to.reserve(ctx, ob, ob);
+    if (rc) return rc;
+    cudaStream_t st = ctx->stream;
+    CK(cudaMemcpyAsync(ti, in, ib, cudaMemcpyHostToDevice, st));
+    k_selftest_group<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(op, ti, n, to, ctx->d_gtab);
+    ctx->launches += 1;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(out, to, ob, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     return SV_OK;
 }

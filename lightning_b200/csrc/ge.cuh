@@ -8,6 +8,20 @@
 #pragma once
 #include "fe.cuh"
 
+// Which branch of the case analysis each addition took.  The host build of the tests (tests/host_emul) defines
+// SV_GE_TRACE to log these so that tests/group_schedule.py can be checked against the code, addition by addition;
+// everywhere else it expands to nothing.
+#define SV_GE_ADD_GENERIC 0
+#define SV_GE_ADD_DOUBLE 1
+#define SV_GE_ADD_INFINITY 2
+#define SV_GE_ADD_A_INF 3
+#define SV_GE_ADD_B_INF 4
+#define SV_GE_MIXED 0  // gej_add_ge / pair_add_ge
+#define SV_GE_FULL 8   // gej_add_gej
+#ifndef SV_GE_TRACE
+#define SV_GE_TRACE(ev) ((void)0)
+#endif
+
 struct ge {  // affine point (never infinity)
     fe x, y;
 };
@@ -60,6 +74,7 @@ SV_HD void gej_double(gej& r, const gej& a) {
 // If rzr != nullptr it receives H, the ratio Z3/Z1 (used when building effective-affine tables).
 SV_HD void gej_add_ge(gej& r, const gej& a, const ge& b, fe* rzr = nullptr) {
     if (a.inf) {
+        SV_GE_TRACE(SV_GE_MIXED | SV_GE_ADD_A_INF);
         gej_set_ge(r, b);
         if (rzr) fe_set_u32(*rzr, 1);  // not meaningful (reference asserts this never happens in table builds)
         return;
@@ -73,14 +88,17 @@ SV_HD void gej_add_ge(gej& r, const gej& a, const ge& b, fe* rzr = nullptr) {
     fe_sub(rr, s2, a.y);
     if (fe_is_zero(h)) {
         if (fe_is_zero(rr)) {
+            SV_GE_TRACE(SV_GE_MIXED | SV_GE_ADD_DOUBLE);
             if (rzr) fe_dbl(*rzr, a.y);
             gej_double(r, a);
         } else {
+            SV_GE_TRACE(SV_GE_MIXED | SV_GE_ADD_INFINITY);
             r.inf = 1;
             if (rzr) fe_set_zero(*rzr);
         }
         return;
     }
+    SV_GE_TRACE(SV_GE_MIXED | SV_GE_ADD_GENERIC);
     if (rzr) *rzr = h;
     fe_sqr(hh, h);
     fe_mul(hhh, h, hh);
@@ -104,10 +122,12 @@ SV_HD void gej_add_ge(gej& r, const gej& a, const ge& b, fe* rzr = nullptr) {
 // Used where independently computed partial sums meet (the small-batch path adds its two half-ladders and the comb sum).
 SV_HD void gej_add_gej(gej& r, const gej& a, const gej& b) {
     if (a.inf) {
+        SV_GE_TRACE(SV_GE_FULL | SV_GE_ADD_A_INF);
         r = b;
         return;
     }
     if (b.inf) {
+        SV_GE_TRACE(SV_GE_FULL | SV_GE_ADD_B_INF);
         r = a;
         return;
     }
@@ -124,8 +144,10 @@ SV_HD void gej_add_gej(gej& r, const gej& a, const gej& b) {
     fe_sub(rr, s2, s1);
     if (fe_is_zero(h)) {
         if (fe_is_zero(rr)) {
+            SV_GE_TRACE(SV_GE_FULL | SV_GE_ADD_DOUBLE);
             gej_double(r, a);
         } else {
+            SV_GE_TRACE(SV_GE_FULL | SV_GE_ADD_INFINITY);
             r.inf = 1;
             fe_set_zero(r.x);
             fe_set_zero(r.y);
@@ -133,6 +155,7 @@ SV_HD void gej_add_gej(gej& r, const gej& a, const gej& b) {
         }
         return;
     }
+    SV_GE_TRACE(SV_GE_FULL | SV_GE_ADD_GENERIC);
     fe hh, hhh, v, x3;
     fe_sqr(hh, h);
     fe_mul(hhh, h, hh);

@@ -117,3 +117,126 @@ SV_UNROLL
         for (int k = 0; k < 8; k++) R[k] = s.v[k];
     }
 }
+
+// ONE group-law operation or scalar-multiplication schedule of the engine on a caller record (test support): IN holds
+// SV_STG_IN_WORDS words, OUT receives SV_STG_OUT_WORDS (layouts in the SV_STG_* list of include/cln_sigverify.h).  Every op
+// calls the production function unchanged.
+SV_HD void stg_load_gej(gej& r, const u32* w) {
+    for (int k = 0; k < 8; k++) { r.x.v[k] = w[k]; r.y.v[k] = w[8 + k]; r.z.v[k] = w[16 + k]; }
+    r.inf = w[24];
+}
+SV_HD void stg_store_gej(u32* w, const gej& r) {
+    for (int k = 0; k < 8; k++) { w[k] = r.x.v[k]; w[8 + k] = r.y.v[k]; w[16 + k] = r.z.v[k]; }
+    w[24] = r.inf;
+}
+SV_HD void stg_load_fe(fe& r, const u32* w) {
+    for (int k = 0; k < 8; k++) r.v[k] = w[k];
+}
+SV_HD void stg_store_fe(u32* w, const fe& r) {
+    for (int k = 0; k < 8; k++) w[k] = r.v[k];
+}
+SV_HD void stg_load_work(sv_work& w, const u32* in) {  // k1 <- in[32..36], k2 <- in[40..44], u1 <- in[48..55] (comb digits)
+    for (int k = 0; k < 5; k++) { w.k1[k] = in[32 + k]; w.k2[k] = in[40 + k]; w.pad[k] = 0; }
+    sc u1;
+    for (int k = 0; k < 8; k++) u1.v[k] = in[48 + k];
+    sc_prepare_u1(w, u1);
+    w.flags = SV_WF_VALID;
+}
+
+SV_HD void selftest_group_item(int op, const u32* in, u32* out, const ge_mem* gtab) {
+    for (int k = 0; k < SV_STG_OUT_WORDS; k++) out[k] = 0;
+    gej a, b, r;
+    ge q;
+    qtab_entry tab[8];
+    fe zc;
+    switch (op) {
+        case SV_STG_GEJ_DOUBLE:
+            stg_load_gej(a, in);
+            gej_double(r, a);
+            stg_store_gej(out, r);
+            break;
+        case SV_STG_GEJ_ADD_GE: {
+            fe rzr;
+            fe_set_zero(rzr);
+            stg_load_gej(a, in);
+            stg_load_fe(q.x, in + 32);
+            stg_load_fe(q.y, in + 40);
+            r = a;
+            if (in[60] & 1u) gej_add_ge(r, r, q, &rzr); else gej_add_ge(r, a, q, &rzr);  // in[60] bit 0: r aliases a
+            stg_store_gej(out, r);
+            stg_store_fe(out + 32, rzr);
+            break;
+        }
+        case SV_STG_GEJ_ADD_GEJ:
+            stg_load_gej(a, in);
+            stg_load_gej(b, in + 32);
+            if (in[60] == 1u) { gej_add_gej(a, a, b); r = a; }       // r aliases a
+            else if (in[60] == 2u) { gej_add_gej(b, a, b); r = b; }  // r aliases b
+            else gej_add_gej(r, a, b);
+            stg_store_gej(out, r);
+            break;
+        case SV_STG_GE_SET_XO: {
+            fe x;
+            stg_load_fe(x, in);
+            out[16] = ge_set_xo(q, x, in[8] != 0) ? 1u : 0u;
+            stg_store_fe(out, q.x);
+            stg_store_fe(out + 8, q.y);
+            break;
+        }
+        case SV_STG_QTABLE_BUILD:
+            stg_load_fe(q.x, in);
+            stg_load_fe(q.y, in + 8);
+            qtable_build(tab, zc, q);
+            for (int e = 0; e < 8; e++)
+                for (int k = 0; k < 8; k++) { out[24 * e + k] = tab[e].x[k]; out[24 * e + 8 + k] = tab[e].y[k]; out[24 * e + 16 + k] = tab[e].h[k]; }
+            stg_store_fe(out + 192, zc);
+            break;
+        case SV_STG_ECMULT_LADDER_Q:
+        case SV_STG_ECMULT_HALF_LADDER:
+        case SV_STG_ECMULT_LADDER: {
+            sv_work w;
+            stg_load_work(w, in);
+            stg_load_fe(q.x, in);
+            stg_load_fe(q.y, in + 8);
+            qtable_build(tab, zc, q);
+            if (op == SV_STG_ECMULT_LADDER_Q) ecmult_ladder_q(r, &w, tab, zc);
+            else if (op == SV_STG_ECMULT_LADDER) ecmult_ladder(r, &w, gtab, tab, zc);
+            else ecmult_half_ladder(r, w.k1, in[60] != 0, tab);  // on the scaled curve: true Z = Z * zc
+            stg_store_gej(out, r);
+            stg_store_fe(out + 32, zc);
+            break;
+        }
+        case SV_STG_ECMULT_COMB_ADD: {
+            sv_work w;
+            stg_load_work(w, in);
+            stg_load_gej(r, in);
+            ecmult_comb_add(r, &w, gtab);
+            stg_store_gej(out, r);
+            break;
+        }
+        case SV_STG_SMALL_COMB: {
+            sv_small_item it;
+            stg_load_work(it.w, in);
+            small_comb(&it, gtab);
+            small_jac_load(r, &it.p3);
+            stg_store_gej(out, r);
+            break;
+        }
+        case SV_STG_NS_LINEAR_FORM: {
+            fe X1, Y1, Zs, c, rfe, D, B, ext[2];
+            stg_load_fe(X1, in);
+            stg_load_fe(Y1, in + 8);
+            stg_load_fe(Zs, in + 16);
+            stg_load_fe(c, in + 24);
+            stg_load_gej(b, in + 32);
+            stg_load_fe(rfe, in + 56);
+            out[32] = ns_linear_form(D, B, X1, Y1, Zs, b, c, rfe, ext) ? 1u : 0u;
+            stg_store_fe(out, D);
+            stg_store_fe(out + 8, B);
+            stg_store_fe(out + 16, ext[0]);
+            stg_store_fe(out + 24, ext[1]);
+            break;
+        }
+        default: break;
+    }
+}

@@ -1310,6 +1310,7 @@ SV_HD void pair_double(const pair_lane& L, gej& R) {
 SV_HD void pair_add_ge(const pair_lane& L, gej& R, const ge& p) {
     const bool r1 = L.role != 0;
     if (R.inf) {
+        SV_GE_TRACE(SV_GE_MIXED | SV_GE_ADD_A_INF);
         gej_set_ge(R, p);
         return;
     }
@@ -1327,13 +1328,17 @@ SV_HD void pair_add_ge(const pair_lane& L, gej& R, const ge& p) {
     fe_sel(H_, r1, w, h);
     fe_sel(RR_, r1, rr, w);
     if (fe_is_zero(H_)) {               // same x: double or cancel (group_impl.h:595-605); both lanes agree on the branch
-        if (fe_is_zero(RR_)) pair_double(L, R);
-        else {
+        if (fe_is_zero(RR_)) {
+            SV_GE_TRACE(SV_GE_MIXED | SV_GE_ADD_DOUBLE);
+            pair_double(L, R);
+        } else {
+            SV_GE_TRACE(SV_GE_MIXED | SV_GE_ADD_INFINITY);
             R.inf = 1;
             fe_set_zero(R.x); fe_set_zero(R.y); fe_set_zero(R.z);
         }
         return;
     }
+    SV_GE_TRACE(SV_GE_MIXED | SV_GE_ADD_GENERIC);
     fe_sel(o1, r1, RR_, H_);
     fe_sel(o2, r1, RR_, u);
     fe q;

@@ -17,6 +17,7 @@ KIND_ECDSA33 = 0
 KIND_ECDSA_XY = 1
 KIND_SCHNORR = 2
 KEY_SIZE = {KIND_ECDSA33: 33, KIND_ECDSA_XY: 64, KIND_SCHNORR: 32}
+STG_IN_WORDS, STG_OUT_WORDS = 64, 200  # SV_STG_IN_WORDS / SV_STG_OUT_WORDS: record widths of the group self test
 
 _c8 = ctypes.POINTER(ctypes.c_uint8)
 
@@ -101,6 +102,7 @@ def load_library():
     lib.sv_pubkey_parse_host.argtypes = [vp, vp, sz, vp, vp]
     lib.sv_synth_device.argtypes = [vp, i, ctypes.c_uint64, sz, vp, vp, vp, vp]
     lib.sv_selftest_host.argtypes = [vp, i, vp, vp, sz, vp]
+    lib.sv_selftest_group_host.argtypes = [vp, i, vp, sz, vp]
     lib.sv_verify_mixed_host.argtypes = [vp, vp, vp, vp, vp, sz, vp]
     lib.sv_verify_mixed_device.argtypes = [vp, vp, vp, vp, vp, sz, vp, vp]
     lib.sv_verify_schnorr_batch_host.argtypes = [vp, vp, vp, vp, sz, vp, vp, vp, vp]
@@ -445,6 +447,15 @@ class SigVerifier:
         out = np.zeros((a.shape[0], 16), dtype=np.uint32)
         self._check(self.lib.sv_selftest_host(self._ctx, int(op), a.ctypes.data, b.ctypes.data, a.shape[0], out.ctypes.data),
                     "sv_selftest_host")
+        return out
+
+    def selftest_group(self, op, rec):
+        """Run group op `op` (SV_STG_* of cln_sigverify.h) on the device for each record of rec: (n, 64) uint32; returns
+        (n, 200) uint32.  Test support."""
+        rec = np.ascontiguousarray(rec, dtype=np.uint32).reshape(-1, STG_IN_WORDS)
+        out = np.zeros((rec.shape[0], STG_OUT_WORDS), dtype=np.uint32)
+        self._check(self.lib.sv_selftest_group_host(self._ctx, int(op), rec.ctypes.data, rec.shape[0], out.ctypes.data),
+                    "sv_selftest_group_host")
         return out
 
     # ---- deferral queue --------------------------------------------------------------------

@@ -47,21 +47,27 @@ def mul(k, pt):
 G = (GX, GY)
 
 
-def craft(d, u1, u2):
-    """Return (msg32, pub33, pubxy, sig64) of a signature that verifies with scalars (+-u1, +-u2), or None."""
+def craft(d, u1, u2, exact=False, r_if_infinity=None):
+    """Return (msg32, pub33, pubxy, sig64) of a signature that verifies with scalars (+-u1, +-u2), or None.
+
+    exact: the verifier must see exactly (u1, u2): None instead of negating both when s would be high.
+    r_if_infinity: when u1*G + u2*Q is infinity, sign with this r instead (an invalid signature whose verification
+    still runs with exactly these scalars)."""
     u1 %= N
     u2 %= N
     if u2 == 0 or d % N == 0:
         return None
     Q = mul(d, G)
     R = mul((u1 + u2 * d) % N, G)
-    if R is None:
+    if R is None and r_if_infinity is None:
         return None
-    r = R[0] % N
+    r = R[0] % N if R is not None else r_if_infinity % N
     if r == 0:
         return None
     s = r * inv(u2, N) % N
     if s > N // 2:  # negating both scalars keeps x(R) and flips s
+        if exact:
+            return None
         s = N - s
         u1 = (N - u1) % N
     m = u1 * s % N

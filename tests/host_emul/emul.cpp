@@ -14,6 +14,11 @@
 #include <cstring>
 #include <vector>
 #include "../../lightning_b200/csrc/common.cuh"
+// branch log of the group law (ge.cuh SV_GE_TRACE): one byte per addition, SV_GE_MIXED / SV_GE_FULL | SV_GE_ADD_*, kept
+// per thread and only while a caller of emul_trace_* has switched it on (the second lane of a pair runs on a thread of its
+// own and is not logged: both lanes take the same branches)
+static thread_local std::vector<unsigned char>* g_trace = nullptr;
+#define SV_GE_TRACE(ev) do { if (g_trace) g_trace->push_back((unsigned char)(ev)); } while (0)
 struct fe;
 // host stand-in for the warp shuffle between the two lanes of a pair (verify.cuh pair_swap): the lanes are two threads
 // that meet at a mailbox; a sense-reversing barrier on atomics orders the exchange
@@ -189,6 +194,23 @@ void emul_gtable_build(void) { build_gtable_fast(); }
 // the self-test cases of tests/selftest_cases.py against the host forms of the primitives
 void emul_selftest(int op, const u32* a, const u32* b, size_t n, u32* out) {
     for (size_t i = 0; i < n; i++) selftest_item(op, a + 8 * i, b + 8 * i, out + 16 * i, g_table.data());
+}
+void emul_selftest_group(int op, const u32* in, size_t n, u32* out) {
+    for (size_t i = 0; i < n; i++) selftest_group_item(op, in + SV_STG_IN_WORDS * i, out + SV_STG_OUT_WORDS * i, g_table.data());
+}
+
+// Branch log: emul_trace_begin() starts logging on the calling thread, emul_trace_end(out, cap) stops it, copies up to cap
+// events to out and returns how many were logged.
+static std::vector<unsigned char> g_trace_buf;
+void emul_trace_begin(void) {
+    g_trace_buf.clear();
+    g_trace = &g_trace_buf;
+}
+size_t emul_trace_end(u8* out, size_t cap) {
+    g_trace = nullptr;
+    size_t n = g_trace_buf.size();
+    if (out) memcpy(out, g_trace_buf.data(), n < cap ? n : cap);
+    return n;
 }
 // entry computed the way the device kernel does it (double-and-add + Fermat), for cross-checking
 void emul_gtable_entry_device_algo(u32 e, u32* xy16) {
