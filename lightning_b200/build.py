@@ -29,7 +29,7 @@ NVCC_FLAGS = [
 ]
 # gcc flags of the plain-C parts: the drop-in (linked into the library) and the verifier subdaemon
 DROPIN_CFLAGS = ["-O2", "-fPIC", "-Wall", "-Wextra", "-std=c11"]
-DAEMON_CFLAGS = ["-O2", "-Wall", "-Wextra", "-std=c11"]
+DAEMON_CFLAGS = ["-O2", "-Wall", "-Wextra", "-std=c11", "-pthread"]
 
 
 def _newer(target, sources):
