@@ -255,7 +255,9 @@ int sv_verify_samekey_host(sv_ctx *ctx, int kind, const uint8_t *key, const uint
  *      bitcoin_tx_hash_for_sig (bitcoin/signature.c:120-151) -> wally_tx_get_btc_signature_hash ->
  *      bip143_signature_hash (libwally tx_io.c:660-765) + check_signed_hash.  The host passes only the fields of the
  *      preimage; scripts live in one blob.  Multi-output / multi-input transactions (the commitment transaction itself,
- *      check_tx_sig in general) pass their serialised outputs / outpoints through the SV_TX_* flags.  sighash32_out (optional, n x 32) returns the computed sighashes. ---- */
+ *      check_tx_sig in general) pass their serialised outputs / outpoints through the SV_TX_* flags.  sighash32_out (optional, n x 32) returns the computed sighashes.
+ *      A sighash_type libwally does not hash for a segwit-v0 Bitcoin input (tx_io.c:972-1009: anything but 0, 1, 2, 3,
+ *      0x81, 0x82, 0x83) gives verdict 0 and a zero sighash, whatever the signature. ---- */
 #define SV_TX_OUTPUTS_SERIALIZED 1u /* the out_script span holds the already-serialised outputs to commit to (amount ||
                                        CompactSize || script, concatenated: all outputs for SIGHASH_ALL, the one at the
                                        input's index for SIGHASH_SINGLE); output_amount is ignored */
@@ -265,7 +267,8 @@ int sv_verify_samekey_host(sv_ctx *ctx, int kind, const uint8_t *key, const uint
 #define SV_TX_OUTPUTS_ZERO 4u       /* hashOutputs is 32 zero bytes (SIGHASH_SINGLE with no output at the input's index,
                                        libwally tx_io.c:725) */
 typedef struct {
-    uint32_t version, locktime, sequence, sighash_type; /* sighash_type: SIGHASH_ALL 1 / NONE 2 / SINGLE 3, | 0x80 ANYONECANPAY */
+    uint32_t version, locktime, sequence, sighash_type; /* sighash_type: SIGHASH_ALL 1 / NONE 2 / SINGLE 3, | 0x80 ANYONECANPAY,
+                                                           or 0 (hashed as ALL); any other value is refused */
     uint8_t prev_txid[32];                              /* as serialised in the transaction (internal byte order) */
     uint32_t prev_index;
     uint32_t script_off, script_len;                    /* witness script (scriptCode) inside `scripts`, any length */
@@ -283,7 +286,8 @@ int sv_verify_tx_host(sv_ctx *ctx, int kind, const sv_tx *txs, const uint8_t *sc
  * ascending, whose fee = f*weight/1000 (common/amount.c:698-707 amount_tx_fee) makes sig64 verify under key for the
  * transaction *tx with its single output set to input_amount - fee.  A feerate whose fee equals the previous feerate's
  * is skipped; the walk ends at the first fee above input_amount, as the reference loop does.  *feerate_out = -1 when
- * none verifies (including a signature or key the reference would refuse).  tx->output_amount is ignored; tx->flags
+ * none verifies (including a signature, key or sighash type the reference would refuse: the types sv_verify_tx_host
+ * refuses give -1 without a candidate checked).  tx->output_amount is ignored; tx->flags
  * must be 0 (one input, one output); weight < 2^32.  Verdict per candidate = sv_verify_tx_host's.
  *      kind: SV_KIND_ECDSA33 or _XY.  min_feerate > max_feerate: none found, no launch.  weight 0: one candidate, fee 0.
  *      Spans out of range, a non-zero flags, weight >= 2^32 and NULL required pointers: SV_ERR_ARG.  On the device: one

@@ -223,12 +223,15 @@ SV_HD void sha_stream_final_double(sha256_stream& c, u8 out32[32]) {
 // and bip143_tail.  bip143_sighash runs them in turn; onchaind's fee grind (k_grind) runs the prefix once and the other
 // two once per candidate output amount, so both paths hash with the same code.
 //
-// Prefix: false only if the sighash type has bits above the low byte (libwally refuses those, tx_io.c:682); there is no
+// Prefix: false if the sighash type is not one libwally hashes for a Bitcoin segwit-v0 input: 0 (hashed as ALL), ALL, NONE,
+// SINGLE, each with or without ANYONECANPAY (wally_tx_get_input_signature_hash, tx_io.c:972-1009).  Every other value is
+// WALLY_EINVAL there, bits above the low byte included, and ANYPREVOUT (0x40, FORKID for Bitcoin) with them.  There is no
 // bound on script sizes.  With SV_TX_INPUTS_SERIALIZED hashPrevouts / hashSequence run over the supplied spans
 // (multi-input transactions).
+SV_HD bool bip143_sighash_type_ok(u32 t) { return t <= 3u || (t >= 0x81u && t <= 0x83u); }
 SV_HD bool bip143_prefix(sha256_stream& c, const sv_tx_item& t, const u8* blob) {
     sha_stream_init(c);
-    if (t.sighash_type & 0xffffff00u) return false;
+    if (!bip143_sighash_type_ok(t.sighash_type)) return false;
     const bool acp = (t.sighash_type & 0x80u) != 0;
     const u32 base = t.sighash_type & 0x1fu;
     const bool sh_none = base == 2, sh_single = base == 3;
