@@ -174,10 +174,13 @@ unsigned sv_last_gossip_repairs(const sv_ctx *ctx);
  *      Messages: rec_status is what sv_verify_gossip_host reports (0, 1..4, -1).  With chain_hash32, the gates of
  *      sv_verify_gossip_burst_host apply too (-4 node ids out of order, -3 another chain); NULL means no gates.  A
  *      channel_update is signed by the channel gossmap holds for its scid at the update's position: the first
- *      non-deleted channel_announcement of the scid holds it (whatever its own status, as long as it holds the fixed
- *      layout through node_id_2), a later one is redundant and never signs, a non-deleted gossip_store_delete_chan frees
- *      the scid for the next announcement.  The signer is node_id_1 or node_id_2 by channel_flags & 1.  An update whose
- *      scid has no channel at its position is -2 (after -1 and -3).
+ *      non-deleted channel_announcement of the scid holds it (whatever its own status), a later one is redundant and
+ *      never signs, a non-deleted gossip_store_delete_chan frees the scid for the next announcement.  The signer is
+ *      node_id_1 or node_id_2 by channel_flags & 1.  An update whose scid has no channel at its position is -2 (after -1
+ *      and -3).  As gossmap does, these fields are read at their fixed offsets from the message start even where the
+ *      message is shorter (an announcement through node_id_2, an update through htlc_maximum_msat, a delete_chan's
+ *      scid): the bytes come from the records after it.  Only a record whose reads would pass the end of the store, where
+ *      gossmap's load asserts, takes no part in the channel table.
  *
  *      rec_off / rec_type / rec_status (and rec_holder, optional): one entry per record the walk reads, in store order;
  *      rec_holder is the header offset of the announcement holding the channel, for a channel_update and for a redundant
@@ -205,7 +208,7 @@ typedef struct {
     uint64_t good, bad_signature, malformed, no_channel, wrong_chain, bad_order; /* messages: 0, 1..4, -1, -2, -3, -4 */
     uint64_t deleted, store_records, unknown, not_reached;
     uint64_t redundant_announcements; /* reached channel_announcements of an scid whose channel was already held */
-    uint64_t updates_without_channel; /* reached channel_updates (scid and flags present) whose scid held no channel */
+    uint64_t updates_without_channel; /* reached channel_updates (read inside the store) whose scid held no channel */
 } sv_gossip_store_summary;
 size_t sv_gossip_store_count(const uint8_t *store, size_t len);
 int sv_verify_gossip_store_host(sv_ctx *ctx, const uint8_t *store, size_t len, const uint8_t *chain_hash32,

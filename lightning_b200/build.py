@@ -6,7 +6,8 @@ Everything is built IN-TREE, so the package and the tests run from the source tr
   oracle/libsecp_port.so               the plain-C restatement oracle                 [gcc]
   oracle/_ref/libsecp_ref.so           the unmodified reference, from the Core Lightning tree at $CLN_SRC or /root/reference [gcc]
   lightning_b200/cln_sigverifyd, cln_verify_gossip_store   the verifier subdaemon and the gossip_store audit tool [gcc]
-  oracle/_ref/libcln_ref.so, libcln_bolt12.so   CLN's own plumbing and BOLT12 Merkle code from the same tree [gcc]
+  oracle/_ref/libcln_ref.so, libcln_bolt12.so, libcln_gossmap.so   CLN's own plumbing, BOLT12 Merkle code and
+                                        gossip_store loader (common/gossmap.c) from the same tree [gcc]
 """
 import os
 import shutil
@@ -115,6 +116,11 @@ def build_oracle():
                        stdin=subprocess.DEVNULL, timeout=900)
     if r.returncode != 0:
         raise RuntimeError("oracle build (bolt12.mk) failed:\n" + r.stdout + r.stderr)
+    # the reference's gossip_store loader (common/gossmap.c), with the configurator's config.h of the `cln` target
+    r = subprocess.run(["make", "-C", os.path.join(ROOT, "oracle"), "-f", "gossmap.mk", "all"], capture_output=True, text=True,
+                       stdin=subprocess.DEVNULL, timeout=900)
+    if r.returncode != 0:
+        raise RuntimeError("oracle build (gossmap.mk) failed:\n" + r.stdout + r.stderr)
 
 
 def build_all(force=False, verbose=False):

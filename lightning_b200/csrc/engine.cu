@@ -665,13 +665,13 @@ __global__ void __launch_bounds__(256) k_store_crc(const u8* store, const u64* r
     if ((threadIdx.x & 31) == 0 && bad != 0xFFFFFFFFu) atomicMin(first_bad, bad);
 }
 // one thread per channel event (announcement, delete_chan, update, listed by the host in store order): its scid as the
-// sort key and its own index as the value; a record too short to take part gets ok = 0
-__global__ void __launch_bounds__(256) k_store_events(const u8* store, const u64* ev_off, const u32* ev_len, const u8* ev_kind,
+// sort key and its own index as the value; an event whose reads would pass the end of the store (store_len) gets ok = 0
+__global__ void __launch_bounds__(256) k_store_events(const u8* store, u64 store_len, const u64* ev_off, const u8* ev_kind,
                                                       size_t n, u64* key, u32* val, u8* ok) {
     size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= n) return;
     const u8* p = store + ev_off[e];
-    const bool good = gs_event_ok(ev_kind[e], p, ev_len[e]);
+    const bool good = gs_event_ok(ev_kind[e], p, store_len - ev_off[e]);
     key[e] = good ? gs_event_scid(ev_kind[e], p) : ~0ull;
     val[e] = (u32)e;
     ok[e] = good;
@@ -2124,7 +2124,7 @@ extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, si
     int cut_status = bad < live_rec.size() ? GS_ST_BAD_CRC : 0;
     // messages (item slots laid out from the 2-byte type) and channel events before the cut, in store order
     std::vector<u64> moff, eoff;
-    std::vector<u32> mlen, base, mrec, elen, emsg, msg_of(nrec, GS_NONE);
+    std::vector<u32> mlen, base, mrec, emsg, msg_of(nrec, GS_NONE);
     std::vector<u8> ekind;
     size_t items = 0;
     for (size_t r = 0; r < cut; r++) {
@@ -2137,7 +2137,7 @@ extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, si
         }
         const int k = t == 256 ? GS_EV_ANN : t == 258 ? GS_EV_UPD : t == GS_DELETE_CHAN ? GS_EV_DEL : -1;
         if (k >= 0) {
-            eoff.push_back(rec[r].off + GS_HDR); elen.push_back(rec[r].len); ekind.push_back((u8)k);
+            eoff.push_back(rec[r].off + GS_HDR); ekind.push_back((u8)k);
             emsg.push_back(k == GS_EV_DEL ? GS_NONE : m);
         }
     }
@@ -2153,12 +2153,12 @@ extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, si
         CK(cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const u64*)nullptr, (u64*)nullptr, (const u32*)nullptr,
                                            (u32*)nullptr, (int)nev, 0, 64, st));
         // one slab: per message [off u64][len u32][item base u32][status int][holder u32][signer 33B][kind 1B], per item
-        // [keyok 1B], per event [off u64][key u64 x2][len u32][msg u32][value u32 x2][kind 1B][ok 1B], chain hash, sort scratch
+        // [keyok 1B], per event [off u64][key u64 x2][msg u32][value u32 x2][kind 1B][ok 1B], chain hash, sort scratch
         slab_layout L;
         const size_t o_moff = L.take(8 * n_msgs), o_mlen = L.take(4 * n_msgs), o_base = L.take(4 * n_msgs),
                      o_status = L.take(4 * n_msgs), o_holder = L.take(4 * n_msgs), o_sig = L.take(33 * n_msgs),
                      o_kinds = L.take(n_msgs), o_keyok = L.take(items), o_eoff = L.take(8 * nev), o_key = L.take(8 * nev),
-                     o_key2 = L.take(8 * nev), o_elen = L.take(4 * nev), o_emsg = L.take(4 * nev), o_val = L.take(4 * nev),
+                     o_key2 = L.take(8 * nev), o_emsg = L.take(4 * nev), o_val = L.take(4 * nev),
                      o_val2 = L.take(4 * nev), o_ekind = L.take(nev), o_ok = L.take(nev), o_chain = L.take(32),
                      o_cub = L.take(cub_bytes);
         dev_buf<> s;
@@ -2166,7 +2166,7 @@ extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, si
         if (rc) return rc;
         u64 *d_moff = s.at<u64>(o_moff), *d_eoff = s.at<u64>(o_eoff), *d_key = s.at<u64>(o_key), *d_key2 = s.at<u64>(o_key2);
         u32 *d_mlen = s.at<u32>(o_mlen), *d_base = s.at<u32>(o_base), *d_holder = s.at<u32>(o_holder),
-            *d_elen = s.at<u32>(o_elen), *d_emsg = s.at<u32>(o_emsg), *d_val = s.at<u32>(o_val), *d_val2 = s.at<u32>(o_val2);
+            *d_emsg = s.at<u32>(o_emsg), *d_val = s.at<u32>(o_val), *d_val2 = s.at<u32>(o_val2);
         int* d_status = s.at<int>(o_status);
         u8 *d_signers = s + o_sig, *d_kinds = chain_hash32 ? s + o_kinds : nullptr, *d_keyok = s + o_keyok,
            *d_ekind = s + o_ekind, *d_ok = s + o_ok, *d_chain = chain_hash32 ? s + o_chain : nullptr;
@@ -2182,10 +2182,9 @@ extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, si
         }
         if (nev) {
             CK(cudaMemcpyAsync(d_eoff, eoff.data(), 8 * nev, cudaMemcpyHostToDevice, st));
-            CK(cudaMemcpyAsync(d_elen, elen.data(), 4 * nev, cudaMemcpyHostToDevice, st));
             CK(cudaMemcpyAsync(d_emsg, emsg.data(), 4 * nev, cudaMemcpyHostToDevice, st));
             CK(cudaMemcpyAsync(d_ekind, ekind.data(), nev, cudaMemcpyHostToDevice, st));
-            k_store_events<<<(unsigned)((nev + 255) / 256), 256, 0, st>>>(d_store, d_eoff, d_elen, d_ekind, nev, d_key, d_val, d_ok);
+            k_store_events<<<(unsigned)((nev + 255) / 256), 256, 0, st>>>(d_store, len, d_eoff, d_ekind, nev, d_key, d_val, d_ok);
             CK(cub::DeviceRadixSort::SortPairs(s + o_cub, cub_bytes, d_key, d_key2, d_val, d_val2, (int)nev, 0, 64, st));
             k_store_resolve<<<(unsigned)((nev + 127) / 128), 128, 0, st>>>(d_store, d_key2, d_val2, d_ok, d_ekind, d_eoff, d_emsg,
                                                                             nev, d_moff, d_holder, d_signers);
@@ -2233,7 +2232,7 @@ extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, si
                 s = mstatus[m];
                 if (holder[m] != GS_NONE) h = rec[mrec[holder[m]]].off;
                 S.redundant_announcements += t == 256 && holder[m] != GS_NONE;
-                S.updates_without_channel += t == 258 && rec[r].len >= 112 && holder[m] == GS_NONE;
+                S.updates_without_channel += t == 258 && len - rec[r].off - GS_HDR >= GS_UPD_READ && holder[m] == GS_NONE;
             } else {
                 s = (t == GS_CHANNEL_AMOUNT || t == GS_DELETE_CHAN || t == GS_CHAN_DYING || t == GS_UUID) ? GS_ST_STORE_RECORD
                                                                                                           : GS_ST_UNKNOWN;

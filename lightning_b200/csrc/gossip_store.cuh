@@ -7,7 +7,10 @@
 //   checksum     csum_matches -> crc32c(timestamp, msg, len)                        common/gossmap.c:800-812, ccan/crc32c
 //   channels     add_channel (first announcement of an scid holds it, later ones are redundant; no amount record
 //                before EOF stops the walk)                                         common/gossmap.c:440-500
+//                fill_from_update                                                   common/gossmap.c:525-568
 //                remove_channel_by_deletemsg                                        common/gossmap.c:612-626
+//                gossmap reads these at fixed offsets without comparing them with the message length, so a short
+//                message takes part with the store bytes that follow it (gs_event_ok)
 //
 // The header walk is host code (it reads 12 header bytes and the 2-byte type of each record, as map_catchup does).
 // The checksum and the per-scid event rule are SV_HD: the k_store_* kernels in engine.cu call them, tests/host_emul
@@ -88,12 +91,17 @@ SV_HD u32 gs_event(u32* held, int kind, u32 msg) {
     else if (kind == GS_EV_DEL) *held = GS_NONE;
     return h;
 }
-// the byte lengths an event needs before gossmap reads it: an announcement through node_id_2, a delete_chan's scid, an
-// update's scid and channel_flags; shorter records take no part in the channel table
-SV_HD bool gs_event_ok(int kind, const u8* msg, u32 len) {
-    if (kind == GS_EV_ANN) return len >= 260 && len >= 260 + gs_be16(msg + 258) + 32 + 8 + 66;
-    if (kind == GS_EV_DEL) return len >= 10;
-    return len >= 112;
+// gossmap reads an event at fixed offsets from the message start whatever the message's own length, so a short message
+// reads on into the records after it: an announcement through node_id_2 (add_channel), a delete_chan's scid
+// (remove_channel_by_deletemsg), an update through htlc_maximum_msat (fill_from_update).  room = bytes from the message
+// start to the end of the store.  An event takes part in the channel table when those reads stay inside the store; only
+// where they would not (gossmap's map_copy asserts there and the load never returns) does it take no part.
+#define GS_DEL_READ 10u
+#define GS_UPD_READ 138u
+SV_HD bool gs_event_ok(int kind, const u8* msg, u64 room) {
+    if (kind == GS_EV_ANN) return room >= 260 && room >= 260 + (u64)gs_be16(msg + 258) + 32 + 8 + 66;
+    if (kind == GS_EV_DEL) return room >= GS_DEL_READ;
+    return room >= GS_UPD_READ;
 }
 // the scid an event is about (big-endian u64; ordering only needs it to be the same for the same 8 bytes)
 SV_HD u64 gs_event_scid(int kind, const u8* msg) {

@@ -1,6 +1,7 @@
 """Python model of how gossmap loads a gossip_store (common/gossmap.c, reference): map_catchup's record walk and
 checksums (:815-937), and the channel table that decides which announcement signs each channel_update (add_channel
-:440-500, remove_channel_by_deletemsg :612-626).  sv_verify_gossip_store_host must agree with it record for record."""
+:440-500, remove_channel_by_deletemsg :612-626).  sv_verify_gossip_store_host must agree with it record for record, and
+tests/test_gossmap.py checks both against gossmap.c itself."""
 import struct
 
 HDR = 12
@@ -71,14 +72,28 @@ def crc_ok(store, off):
     return crc32c(ts, store[off + HDR:off + HDR + ln]) == crc
 
 
-def ann_ok(m):
-    """an announcement takes part in the channel table when it holds the fixed layout through node_id_2"""
-    return len(m) >= 260 and len(m) >= 260 + struct.unpack(">H", m[258:260])[0] + 32 + 8 + 66
+# How far past a message's first byte gossmap reads it, whatever the message's own length: add_channel reads the
+# features length, then the scid and both node ids (:466-476); fill_from_update reads through htlc_maximum_msat
+# (:531-551); remove_channel_by_deletemsg reads the scid (:620).  A record takes part in the channel table when these
+# reads stay inside the store; where they do not, gossmap's map_copy asserts and the load never returns.
+UPD_READ, DEL_READ = 138, 10
 
 
-def ann_fields(m):
-    """(chain_hash, scid, node_id_1, node_id_2)"""
-    p = 260 + struct.unpack(">H", m[258:260])[0]
+def ann_read(store, p):
+    """bytes add_channel reads from message offset p on (None if even the features length lies past the store end)"""
+    return None if p + 260 > len(store) else 260 + struct.unpack(">H", store[p + 258:p + 260])[0] + 32 + 8 + 66
+
+
+def ann_ok(store, p):
+    """the announcement at message offset p takes part in the channel table"""
+    n = ann_read(store, p)
+    return n is not None and p + n <= len(store)
+
+
+def ann_fields(m, p=0):
+    """(chain_hash, scid, node_id_1, node_id_2) of the announcement at offset p of m (a message, or the store: gossmap
+    reads them where they lie, also past the end of a short message)"""
+    p += 260 + struct.unpack(">H", m[p + 258:p + 260])[0]
     return m[p:p + 32], m[p + 32:p + 40], m[p + 40:p + 73], m[p + 73:p + 106]
 
 
@@ -99,15 +114,15 @@ def audit(store, sigcheck=None):
         off, typ, ln, st = recs[i]
         if st:
             continue
-        m = store[off + HDR:off + HDR + ln]
-        if typ == 256 and ann_ok(m):
-            scid = ann_fields(m)[1]
+        p = off + HDR
+        if typ == 256 and ann_ok(store, p):
+            scid = ann_fields(store, p)[1]
             holder[i] = held.get(scid)
             held.setdefault(scid, i)
-        elif typ == DELETE_CHAN and ln >= 10:
-            held.pop(m[2:10], None)
-        elif typ == 258 and ln >= 112:
-            holder[i] = held.get(m[98:106])
+        elif typ == DELETE_CHAN and p + DEL_READ <= len(store):
+            held.pop(store[p + 2:p + 10], None)
+        elif typ == 258 and p + UPD_READ <= len(store):
+            holder[i] = held.get(store[p + 98:p + 106])
     if no_amount is not None and no_amount < cut and holder.get(no_amount) is None:
         cut, cut_status = no_amount, NO_AMOUNT
     out = []
@@ -123,11 +138,10 @@ def audit(store, sigcheck=None):
                 h = holder.get(i)
                 signer = None
                 if typ == 258 and h is not None:
-                    a = store[recs[h][0] + HDR:recs[h][0] + HDR + recs[h][2]]
-                    signer = ann_fields(a)[2 + (m[111] & 1)]
+                    signer = ann_fields(store, recs[h][0] + HDR)[2 + (store[off + HDR + 111] & 1)]
                 st = sigcheck(m, signer) if sigcheck else 0
                 s["redundant_announcements"] += typ == 256 and h is not None
-                s["updates_without_channel"] += typ == 258 and ln >= 112 and h is None
+                s["updates_without_channel"] += typ == 258 and off + HDR + UPD_READ <= len(store) and h is None
             else:
                 st = STORE_RECORD if typ in (CHANNEL_AMOUNT, DELETE_CHAN, CHAN_DYING, UUID) else UNKNOWN
         elif st == ST_ENDED and ln >= 10:

@@ -36,14 +36,15 @@ extern "C" long long emul_gs_walk(const u8* store, u64 len, u64* off, u32* type,
     return (long long)n;
 }
 
-// channel events in store order (message offsets, lengths, kinds GS_EV_*, message index per event): holder[msg] as
-// k_store_resolve writes it (GS_NONE where nothing held the scid, or for a short record)
-extern "C" void emul_gs_resolve(const u8* store, const u64* ev_off, const u32* ev_len, const u8* ev_kind, const u32* ev_msg,
-                                size_t n, u32* holder) {
+// channel events in store order (message offsets, kinds GS_EV_*, message index per event) of a store of len bytes:
+// holder[msg] as k_store_resolve writes it (GS_NONE where nothing held the scid, or where gossmap's reads of the record
+// would pass the end of the store)
+extern "C" void emul_gs_resolve(const u8* store, u64 len, const u64* ev_off, const u8* ev_kind, const u32* ev_msg, size_t n,
+                                u32* holder) {
     std::map<u64, u32> held;
     for (size_t e = 0; e < n; e++) {
         const u8* p = store + ev_off[e];
-        if (!gs_event_ok(ev_kind[e], p, ev_len[e])) continue;
+        if (!gs_event_ok(ev_kind[e], p, len - ev_off[e])) continue;
         auto it = held.emplace(gs_event_scid(ev_kind[e], p), GS_NONE).first;
         u32 h = gs_event(&it->second, ev_kind[e], ev_msg[e]);
         if (ev_kind[e] != GS_EV_DEL) holder[ev_msg[e]] = h;

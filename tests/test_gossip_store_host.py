@@ -30,7 +30,7 @@ def emul_audit(emul, store):
     emul.emul_gs_walk.restype = ctypes.c_longlong
     emul.emul_gs_walk.argtypes = [ctypes.c_char_p, ctypes.c_uint64] + [ctypes.c_void_p] * 4 + [ctypes.c_uint64, ctypes.c_void_p]
     emul.emul_gs_crc_ok.argtypes = [ctypes.c_char_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
-    emul.emul_gs_resolve.argtypes = [ctypes.c_char_p] + [ctypes.c_void_p] * 4 + [ctypes.c_size_t, ctypes.c_void_p]
+    emul.emul_gs_resolve.argtypes = [ctypes.c_char_p, ctypes.c_uint64] + [ctypes.c_void_p] * 3 + [ctypes.c_size_t, ctypes.c_void_p]
     end3 = np.zeros(3, np.uint64)
     n = emul.emul_gs_walk(store, len(store), None, None, None, None, 0, _p(end3))
     off, typ, ln, st = (np.zeros(max(n, 1), d) for d in (np.uint64, np.uint32, np.uint32, np.int32))
@@ -47,8 +47,7 @@ def emul_audit(emul, store):
     ev = [i for i in range(cut) if st[i] == 0 and typ[i] in (256, 258, gs.DELETE_CHAN)]
     kinds = np.array([{256: 0, gs.DELETE_CHAN: 1, 258: 2}[int(typ[i])] for i in ev] or [0], np.uint8)
     holder = np.full(max(len(msgs), 1), 0xFFFFFFFF, np.uint32)
-    emul.emul_gs_resolve(store, _p(np.array([off[i] + 12 for i in ev] or [0], np.uint64)),
-                         _p(np.array([ln[i] for i in ev] or [0], np.uint32)), _p(kinds),
+    emul.emul_gs_resolve(store, len(store), _p(np.array([off[i] + 12 for i in ev] or [0], np.uint64)), _p(kinds),
                          _p(np.array([midx.get(i, 0xFFFFFFFF) for i in ev] or [0], np.uint32)), len(ev), _p(holder))
     hold = {r: (None if holder[k] == 0xFFFFFFFF else msgs[holder[k]]) for r, k in midx.items()}
     if no_amount is not None and no_amount < cut and hold.get(no_amount) is None:
@@ -191,7 +190,7 @@ def test_deleted_record_with_wrong_crc_is_skipped(emul):
 
 def test_channel_rule(emul):
     """redundant announcements, delete_chan and re-announcement, a deleted announcement, an update before its
-    announcement, an announcement too short to hold its channel, both directions"""
+    announcement, short records (gossmap reads them on into the records after them), both directions"""
     a1, a2, a3 = ca(A), ca(A, N3, N4), ca(A, N2, N4)
     recs = [gs.record(cu(A)),                        # 0 before any announcement: no channel
             gs.record(a1), gs.record(amount()),      # 1 holds A
@@ -201,19 +200,19 @@ def test_channel_rule(emul):
             gs.record(cu(A)),                        # 7 no channel
             gs.record(a2, flags=gs.COMPLETED | gs.DELETED), gs.record(amount()),  # 8 deleted: takes no part
             gs.record(cu(A)),                        # 10 still no channel
-            gs.record(ca(B)[:300]), gs.record(amount()),  # 11 too short to hold B
-            gs.record(cu(B)),                        # 13 no channel
+            gs.record(ca(B)[:300]), gs.record(amount()),  # 11 ends after its scid, still holds B: node ids read on
+            gs.record(cu(B)),                        # 13 -> 11
             gs.record(a3), gs.record(amount()),      # 14 holds A again
             gs.record(cu(A, 1)),                     # 16 -> 14
             gs.record(delete(B + b"\x00")),          # 17 a delete of an unknown scid (longer than 10 bytes)
             gs.record(struct.pack(">H", 4102) + bytes(20)),  # 18 obsolete type: unknown
-            gs.record(struct.pack(">H", gs.DELETE_CHAN) + b"\x00"),  # 19 a delete_chan too short to read: ignored
+            gs.record(struct.pack(">H", gs.DELETE_CHAN) + b"\x00"),  # 19 short: its scid is read from 20's header
             gs.record(cu(A))]                        # 20 -> 14
     store = store_of(*recs)
     out, s = check_agree(emul, store)
     offs = [r[0] for r in out]
     hold = {i: (None if h is None else offs.index(h)) for i, (_, t, _, h) in enumerate(out) if t in (256, 258)}
-    assert hold == {0: None, 1: None, 3: 1, 5: 1, 7: None, 8: None, 10: None, 11: None, 13: None, 14: None, 16: 14, 20: 14}
+    assert hold == {0: None, 1: None, 3: 1, 5: 1, 7: None, 8: None, 10: None, 11: None, 13: 11, 14: None, 16: 14, 20: 14}
     assert out[18][2] == gs.UNKNOWN and out[8][2] == gs.ST_DELETED and out[19][2] == gs.STORE_RECORD
     assert s["stop"] == gs.EOF
 
