@@ -217,6 +217,68 @@ int sv_verify_gossip_store_host(sv_ctx *ctx, const uint8_t *store, size_t len, c
 /* profiling mode (sv_set_profiling): ms4 = host header walk, H2D copy of the store, checksum kernel, the rest of the call */
 int sv_get_last_gossip_store_timing(sv_ctx *ctx, float *ms4);
 
+/* ---- PRUNE a gossip_store: mark every record gossmap should not trust as deleted, so that gossipd's strict load
+ *      (gossmap_load_initial, gossipd/gossmap_manage.c:525: must_be_clean, common/gossmap.c:862, :885, :895, :922,
+ *      :1428-1438) accepts the store and keeps every record that verifies.  gossipd drops a record the same way
+ *      (gossip_store_del, gossipd/gossip_store.c:572-638): bit 0x8000 of the record's flags, set in place.  The checksum
+ *      covers the timestamp and the message only (csum_matches, common/gossmap.c:800-812), and map_catchup skips a deleted
+ *      record before it looks at its length or checksum (:844-847), so every other record reads as before.  gossmap takes
+ *      the last live channel_update per direction and the last live node_announcement per node (update_channel :585-610,
+ *      node_announcement :650-668): deleting a bad newest record makes the previous verified one current again.
+ *
+ *      out (len bytes; may equal store) differs from store only in bit 0x8000 of the flags of the deleted records.
+ *      rec_pruned[r] = 0 (kept, or deleted already) or the SV_GP_* reason record r is deleted for:
+ *        1. Walk: sv_verify_gossip_store_host's, except that a record with a bad checksum (SV_GP_BAD_CRC) or a message
+ *           under 2 bytes (SV_GP_TRUNCATED) is deleted and the walk goes on past it.  INCOMPLETE, PARTIAL and ENDED still
+ *           stop it; nothing at or after the stop is touched.
+ *        2. First round: the statuses of sv_verify_gossip_store_host (with the chain gates when chain_hash32 is given) over
+ *           the records the walk left live.  A channel_announcement or node_announcement whose status is not 0, and a
+ *           channel_update whose status is -1 or -3, is deleted (SV_GP_MESSAGE).
+ *        3. Second round: the channel table again, with the announcements of rule 2 deleted (the first live announcement
+ *           of an scid holds it, a delete_chan frees it).  An announcement redundant in it is deleted (SV_GP_REDUNDANT:
+ *           the strict load refuses one, gossmap.c:895-896).  An update whose scid holds no channel at its position is
+ *           deleted (SV_GP_NO_CHANNEL).  An update whose signer changed is verified again under the new node (same
+ *           SHA-256d digest) and deleted if it fails (SV_GP_SIGNATURE), as is one that failed under an unchanged signer.
+ *           One round is enough: updates never hold channels, and deleting a redundant announcement changes no holder.
+ *        4. The channel_amount record directly after a deleted channel_announcement is deleted with it (SV_GP_AMOUNT), as
+ *           gossip_store_del does.
+ *        5. A record of an unknown type is deleted (SV_GP_UNKNOWN: the strict load refuses one, gossmap.c:918-923).
+ *        6. Nothing else: node_announcements of nodes left without channels stay (gossmap ignores them).
+ *      An announcement kept that has no room for its amount record stops the walk as in the audit (SV_GS_NO_AMOUNT): it
+ *      and every record after it are left as they are.
+ *      rec_status[r] is the record's first-round status: sv_verify_gossip_store_host's, except SV_GS_BAD_CRC and
+ *      SV_GS_TRUNCATED for records the walk went past.  rec_capacity below sv_gossip_prune_count(store, len) (which is
+ *      sv_gossip_store_count plus the truncated records walked past), or a major version other than 0: SV_ERR_ARG,
+ *      nothing written.
+ *      On the device, besides the audit's kernels: a checksum flag per record, a mark kernel (deletions and the event
+ *      mask), k_store_resolve again over the already sorted events, the updates whose signer changed gathered into a
+ *      compact list and verified with their kept digests, and one thread per deleted record setting its flag bit. ---- */
+#define SV_GP_KEPT 0
+#define SV_GP_BAD_CRC 1
+#define SV_GP_TRUNCATED 2
+#define SV_GP_MESSAGE 3
+#define SV_GP_REDUNDANT 4
+#define SV_GP_NO_CHANNEL 5
+#define SV_GP_SIGNATURE 6
+#define SV_GP_AMOUNT 7
+#define SV_GP_UNKNOWN 8
+typedef struct {
+    uint32_t version;    /* the store's version byte */
+    int32_t stop;        /* SV_GS_EOF or the status of the record the walk stopped at */
+    uint64_t end_offset; /* where the walk stopped (the offset of that record) or ran out */
+    uint64_t records;    /* entries written */
+    uint64_t pruned;     /* records this call deleted: the sum of the reasons below */
+    uint64_t bad_crc, truncated, message, redundant, no_channel, signature, amount, unknown; /* SV_GP_1..8 */
+    uint64_t reverified; /* updates verified again under a new signer */
+} sv_gossip_prune_summary;
+size_t sv_gossip_prune_count(const uint8_t *store, size_t len);
+int sv_prune_gossip_store_host(sv_ctx *ctx, const uint8_t *store, size_t len, const uint8_t *chain_hash32, uint8_t *out,
+                               uint64_t *rec_off, uint16_t *rec_type, int *rec_status, uint8_t *rec_pruned,
+                               size_t rec_capacity, sv_gossip_prune_summary *summary);
+/* profiling mode: ms4 = host header walk, first round (H2D of the store, checksums, the audit's kernels), second round
+ * (mark, resolution, compaction, re-verification), flag write and copy back */
+int sv_get_last_gossip_prune_timing(sv_ctx *ctx, float *ms4);
+
 /* L2 residency hint for the throughput kernels (default on): the G comb table and the per-thread multiples tables are
  * marked persisting through a stream access-policy window, the rest of the stream's traffic streaming.  0 switches it off
  * for streams not yet seen (measurement aid). */

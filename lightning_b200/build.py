@@ -121,6 +121,11 @@ def build_oracle():
                        stdin=subprocess.DEVNULL, timeout=900)
     if r.returncode != 0:
         raise RuntimeError("oracle build (gossmap.mk) failed:\n" + r.stdout + r.stderr)
+    # the same loader as gossipd loads its store at start-up (strict), linked with the objects above
+    r = subprocess.run(["make", "-C", os.path.join(ROOT, "oracle"), "-f", "gossmap_strict.mk", "all"], capture_output=True,
+                       text=True, stdin=subprocess.DEVNULL, timeout=900)
+    if r.returncode != 0:
+        raise RuntimeError("oracle build (gossmap_strict.mk) failed:\n" + r.stdout + r.stderr)
 
 
 def build_all(force=False, verbose=False):

@@ -1,6 +1,6 @@
 /* cln_verify_gossip_store — audit a Core Lightning gossip_store before lightningd loads it.
  *
- *   cln_verify_gossip_store [--chain HEX] [--device N] FILE
+ *   cln_verify_gossip_store [--chain HEX] [--device N] [--prune OUT] FILE
  *
  * Walks the store as gossmap does, checks every record checksum and verifies every signature on the GPU
  * (sv_verify_gossip_store_host).  Prints a summary and one line per failing record (offset, type, status).
@@ -10,7 +10,16 @@
  *               last record (a live store's tail can look like either) or a gossip_store_ended record;
  *            1  some signature, gate or channel resolution failed;
  *            2  the walk stopped at a bad checksum, a truncated record or an announcement without its amount;
- *            3  usage, I/O or engine error. */
+ *            3  usage, I/O or engine error.
+ *
+ * --prune OUT: writes OUT, a copy of FILE with every record gossmap should not trust marked deleted
+ * (sv_prune_gossip_store_host), and never writes FILE.  Prints the deletions per reason, then audits OUT as above.
+ * Exit code: 0  OUT is clean: its audit finds no bad signature, malformed message, update without a channel, other
+ *               chain, node ids out of order, redundant announcement or unknown record, and its walk reaches the end of
+ *               the store, so gossipd's strict load accepts it;
+ *            1  OUT is written but not clean (its walk stops before the end: an incomplete, partial or ended record,
+ *               or an announcement without its amount record);
+ *            3  usage, I/O or engine error (OUT may be missing). */
 #include <errno.h>
 #include <inttypes.h>
 #include <stdio.h>
@@ -42,12 +51,58 @@ static const char *status_name(int s) {
 }
 
 static int usage(void) {
-    fprintf(stderr, "usage: cln_verify_gossip_store [--chain HEX] [--device N] FILE\n");
+    fprintf(stderr, "usage: cln_verify_gossip_store [--chain HEX] [--device N] [--prune OUT] FILE\n");
     return 3;
 }
 
+static const char *const reason_name[] = {"kept", "bad checksum", "truncated", "failing message", "redundant announcement",
+                                          "update without a channel", "bad signature under the new signer",
+                                          "amount record of a deleted announcement", "unknown record type"};
+
+/* --prune: write the pruned copy, report it, audit it; returns the exit code */
+static int prune(sv_ctx *ctx, const char *path, const uint8_t *store, size_t len, const uint8_t *chain, const char *outp) {
+    size_t n = sv_gossip_prune_count(store, len);
+    uint64_t *off = malloc((n ? n : 1) * sizeof *off);
+    uint16_t *type = malloc((n ? n : 1) * sizeof *type);
+    int *status = malloc((n ? n : 1) * sizeof *status);
+    uint8_t *why = malloc(n ? n : 1), *out = malloc(len);
+    if (!off || !type || !status || !why || !out) { fprintf(stderr, "out of memory\n"); return 3; }
+    sv_gossip_prune_summary p;
+    int rc = sv_prune_gossip_store_host(ctx, store, len, chain, out, off, type, status, why, n, &p);
+    if (rc != SV_OK) {
+        fprintf(stderr, "sv_prune_gossip_store_host: %d %s\n", rc, sv_last_error(ctx));
+        return 3;
+    }
+    for (size_t i = 0; i < n; i++)
+        if (why[i]) printf("deleted @%" PRIu64 " type %u: %s (status %d)\n", off[i], type[i], reason_name[why[i]], status[i]);
+    FILE *f = fopen(outp, "wb");
+    if (!f || fwrite(out, 1, len, f) != len || fclose(f)) { fprintf(stderr, "%s: %s\n", outp, strerror(errno)); return 3; }
+    printf("gossip_store %s: %" PRIu64 " records, walk stopped: %s at %" PRIu64 "; %" PRIu64 " deleted into %s\n", path,
+           p.records, p.stop ? status_name(p.stop) : "end of store", p.end_offset, p.pruned, outp);
+    const uint64_t count[9] = {0, p.bad_crc, p.truncated, p.message, p.redundant, p.no_channel, p.signature, p.amount, p.unknown};
+    for (int k = 1; k < 9; k++) printf("  %" PRIu64 " %s\n", count[k], reason_name[k]);
+    printf("  %" PRIu64 " updates verified again under a new signer\n", p.reverified);
+    size_t m = sv_gossip_store_count(out, len);
+    uint64_t *aoff = malloc((m ? m : 1) * sizeof *aoff);
+    uint16_t *atype = malloc((m ? m : 1) * sizeof *atype);
+    int *astatus = malloc((m ? m : 1) * sizeof *astatus);
+    if (!aoff || !atype || !astatus) { fprintf(stderr, "out of memory\n"); return 3; }
+    sv_gossip_store_summary s;
+    rc = sv_verify_gossip_store_host(ctx, out, len, chain, aoff, atype, astatus, NULL, m, &s);
+    if (rc != SV_OK) {
+        fprintf(stderr, "sv_verify_gossip_store_host: %d %s\n", rc, sv_last_error(ctx));
+        return 3;
+    }
+    const int clean = s.stop == SV_GS_EOF && s.end_offset == len && !s.bad_signature && !s.malformed && !s.no_channel &&
+                      !s.wrong_chain && !s.bad_order && !s.redundant_announcements && !s.unknown;
+    printf("%s: %s (%" PRIu64 " good messages, %" PRIu64 " deleted records)\n", outp,
+           clean ? "clean" : "NOT clean", s.good, s.deleted);
+    free(off); free(type); free(status); free(why); free(out); free(aoff); free(atype); free(astatus);
+    return clean ? 0 : 1;
+}
+
 int main(int argc, char **argv) {
-    const char *path = NULL;
+    const char *path = NULL, *prune_out = NULL;
     uint8_t chain[32];
     int have_chain = 0, device = 0;
     for (int i = 1; i < argc; i++) {
@@ -62,6 +117,8 @@ int main(int argc, char **argv) {
             have_chain = 1;
         } else if (!strcmp(argv[i], "--device") && i + 1 < argc) {
             device = atoi(argv[++i]);
+        } else if (!strcmp(argv[i], "--prune") && i + 1 < argc) {
+            prune_out = argv[++i];
         } else if (argv[i][0] == '-' || path) {
             return usage();
         } else {
@@ -69,6 +126,10 @@ int main(int argc, char **argv) {
         }
     }
     if (!path) return usage();
+    if (prune_out && !strcmp(prune_out, path)) {
+        fprintf(stderr, "--prune: OUT must be another file than %s\n", path);
+        return 3;
+    }
     FILE *f = fopen(path, "rb");
     if (!f) { fprintf(stderr, "%s: %s\n", path, strerror(errno)); return 3; }
     size_t cap = 1 << 20, len = 0, got;
@@ -79,6 +140,14 @@ int main(int argc, char **argv) {
     }
     fclose(f);
     if (!store || len == 0) { fprintf(stderr, "%s: empty or unreadable\n", path); return 3; }
+    if (prune_out) {
+        sv_ctx *pctx = NULL;
+        if (sv_create(&pctx, device) != SV_OK) { fprintf(stderr, "engine: %s\n", sv_last_error(NULL)); return 3; }
+        int code = prune(pctx, path, store, len, have_chain ? chain : NULL, prune_out);
+        sv_destroy(pctx);
+        free(store);
+        return code;
+    }
 
     size_t n = sv_gossip_store_count(store, len);
     uint64_t *off = malloc((n ? n : 1) * sizeof *off);

@@ -710,6 +710,80 @@ __global__ void __launch_bounds__(256) k_store_finish(const u8* store, const u64
     if (p[0] == 1 && p[1] == 2 && holder[m] == GS_NONE && (status[m] == 0 || status[m] == 1)) status[m] = -2;
 }
 
+// ---- gossip_store prune (sv_prune_gossip_store_host): the deletions, a second channel table and the flag writes ------
+// k_store_crc_flags: k_store_crc with a flag per record (bad[r] = 1 if its checksum fails) instead of the first bad one
+__global__ void __launch_bounds__(256) k_store_crc_flags(const u8* store, const u64* rec_off, size_t n, u8* bad) {
+    __shared__ u32 tab[2048];
+    for (u32 i = threadIdx.x; i < 256; i += blockDim.x) gs_crc_fill(tab, i);
+    __syncthreads();
+    size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < n) bad[r] = !gs_record_crc_ok(tab, store, rec_off[r]);
+}
+// k_prune_mark: thread i < n_msgs turns message i's first-round status into its deletion (an announcement that is not 0,
+// an update that is -1 or -3: SV_GP_MESSAGE); thread i < nev masks event i out of the second round if it is the
+// announcement of a deleted message
+__global__ void __launch_bounds__(256) k_prune_mark(const u8* store, const u64* msg_off, const int* status, size_t n_msgs,
+                                                    const u8* ev_kind, const u32* ev_msg, const u8* ok, size_t nev,
+                                                    u8* reason, u8* ok2) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n_msgs) {
+        const u8* p = store + msg_off[i];
+        const int st = status[i];
+        const bool upd = p[0] == 1 && p[1] == 2;
+        reason[i] = (upd ? (st == -1 || st == -3) : st != 0) ? SV_GP_MESSAGE : SV_GP_KEPT;
+    }
+    if (i < nev) ok2[i] = ok[i] && !(ev_kind[i] == GS_EV_ANN && status[ev_msg[i]] != 0);
+}
+// k_prune_select: one thread per message not yet deleted, after the second k_store_resolve (holder2, signers2).  An
+// announcement that is redundant now: SV_GP_REDUNDANT.  An update without a channel: SV_GP_NO_CHANNEL; with the same
+// holder as in the first round, its first verdict stands (SV_GP_SIGNATURE if it failed); with another holder it joins
+// the compact list (list[0] = count, warp-aggregated), its digest and signature copied from its first-round item slot
+// and the new signer's key written, in item slot tail + its list position.
+__global__ void __launch_bounds__(128) k_prune_select(const u8* store, const u64* msg_off, const int* status, size_t n_msgs,
+                                                      const u32* holder, const u32* holder2, const u32* item_base,
+                                                      const u8* signers2, u8* reason, u32* list, u32 tail, u8* msg32,
+                                                      u8* key33, u8* sig64) {
+    size_t m = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    bool moved = false;
+    if (m < n_msgs && reason[m] == SV_GP_KEPT) {
+        const u8* p = store + msg_off[m];
+        if (p[0] == 1 && p[1] == 0) {
+            if (holder2[m] != GS_NONE) reason[m] = SV_GP_REDUNDANT;
+        } else if (p[0] == 1 && p[1] == 2) {
+            if (holder2[m] == GS_NONE) reason[m] = SV_GP_NO_CHANNEL;
+            else if (holder2[m] != holder[m]) moved = true;
+            else if (status[m] != 0) reason[m] = SV_GP_SIGNATURE;
+        }
+    }
+    const unsigned mask = __ballot_sync(0xFFFFFFFFu, moved);
+    if (!mask) return;
+    const int lane = threadIdx.x & 31, leader = __ffs(mask) - 1;
+    u32 first = 0;
+    if (lane == leader) first = atomicAdd(list, (u32)__popc(mask));
+    first = __shfl_sync(0xFFFFFFFFu, first, leader);
+    if (!moved) return;
+    const u32 t = first + (u32)__popc(mask & ((1u << lane) - 1u));
+    list[1 + t] = (u32)m;
+    const size_t from = item_base[m], to = (size_t)tail + t;
+    for (int b = 0; b < 32; b++) msg32[32 * to + b] = msg32[32 * from + b];
+    for (int b = 0; b < 64; b++) sig64[64 * to + b] = sig64[64 * from + b];
+    for (int b = 0; b < 33; b++) key33[33 * to + b] = signers2[33 * (size_t)m + b];
+}
+// the compact list's verdicts (item slots tail + t): an update that fails under its new signer is SV_GP_SIGNATURE
+__global__ void __launch_bounds__(256) k_prune_settle(const u32* list, const u8* verdict, u8* reason) {
+    u32 t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < list[0] && !verdict[t]) reason[list[1 + t]] = SV_GP_SIGNATURE;
+}
+// one thread per deleted record: sets GOSSIP_STORE_DELETED_BIT (the high byte of the be16 flags) in the device copy of
+// the store and returns that byte, the only one that changes
+__global__ void __launch_bounds__(256) k_prune_flags(u8* store, const u64* rec_off, size_t n, u8* flag_hi) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const u8 v = store[rec_off[i]] | (u8)(GS_DELETED >> 8);
+    store[rec_off[i]] = v;
+    flag_hi[i] = v;
+}
+
 // ---- BOLT12 signatures (bolt12.cuh): the message hash of bolt12_check_signature on the device -----------------------
 // k_b12_count: one thread per stream walks its BigSize headers (bytes only): field count, or 0 if the parse fails
 __global__ void __launch_bounds__(128) k_b12_count(const u8* blob, const u64* off, const u32* len, size_t n, u32* cnt) {
@@ -1298,6 +1372,7 @@ struct sv_ctx {
     cudaEvent_t ev[3] = {};      // before prep, between prep and main, after main (profiling mode only)
     cudaEvent_t b12_ev[2] = {};  // around the BOLT12 parse / Merkle / sighash kernels (profiling mode only)
     float gs_ms[4] = {};         // last sv_verify_gossip_store_host: header walk, H2D, checksums, verification (profiling mode)
+    float gp_ms[4] = {};         // last sv_prune_gossip_store_host: header walk, first round, second round, flag write
     unsigned long long launches = 0;
     std::vector<sv_queue_item> queue;
     std::string err;
@@ -2074,6 +2149,119 @@ struct ev_set {  // CUDA events of one call, destroyed on every exit path
     ~ev_set() { for (cudaEvent_t x : e) if (x) cudaEventDestroy(x); }
 };
 
+// One pass over a staged store: the messages (item slots laid out from the 2-byte type) and channel events of the live
+// records before `cut` (skip[r] != 0 leaves record r out as well), sliced, resolved, hashed and verified on the device.
+// The slab stays allocated with the pass, so the prune's second round reuses the sorted events, the first holders and
+// the digests (item slots of ctx->d_msg / d_sig; ctx's staging holds extra_items more slots after them).
+struct store_pass {
+    std::vector<u64> moff, eoff;
+    std::vector<u32> mlen, base, mrec, emsg, msg_of;
+    std::vector<u8> ekind;
+    size_t items = 0, n_msgs = 0, nev = 0;
+    std::vector<int> mstatus;  // per message: the statuses of sv_verify_gossip_store_host
+    std::vector<u32> holder;   // per message: the message index of the holder the event saw, or GS_NONE
+    dev_buf<> s;
+    u64 *d_moff = nullptr, *d_eoff = nullptr, *d_key2 = nullptr;
+    u32 *d_base = nullptr, *d_holder = nullptr, *d_emsg = nullptr, *d_val2 = nullptr;
+    int* d_status = nullptr;
+    u8 *d_ekind = nullptr, *d_ok = nullptr;
+};
+static int store_pass_run(sv_ctx* ctx, const u8* d_store, size_t len, const uint8_t* chain_hash32,
+                          const std::vector<gs_rec>& rec, size_t cut, const u8* skip, size_t extra_items, store_pass& P,
+                          cudaEvent_t done) {
+    cudaStream_t st = ctx->stream;
+    P.msg_of.assign(rec.size(), GS_NONE);
+    size_t& items = P.items;
+    for (size_t r = 0; r < cut; r++) {
+        if (rec[r].status != GS_LIVE || (skip && skip[r])) continue;
+        const u32 t = rec[r].type, m = (u32)P.moff.size();
+        if (t == 256 || t == 257 || t == 258) {
+            P.msg_of[r] = m;
+            P.moff.push_back(rec[r].off + GS_HDR); P.mlen.push_back(rec[r].len); P.base.push_back((u32)items);
+            P.mrec.push_back((u32)r);
+            items += t == 256 ? 4 : 1;
+        }
+        const int k = t == 256 ? GS_EV_ANN : t == 258 ? GS_EV_UPD : t == GS_DELETE_CHAN ? GS_EV_DEL : -1;
+        if (k >= 0) {
+            P.eoff.push_back(rec[r].off + GS_HDR); P.ekind.push_back((u8)k);
+            P.emsg.push_back(k == GS_EV_DEL ? GS_NONE : m);
+        }
+    }
+    const size_t n_msgs = P.n_msgs = P.moff.size(), nev = P.nev = P.eoff.size();
+    if (items + extra_items >= 0xFFFFFFFFu || nev >= 0x7FFFFFFFu)
+        return fail(ctx, SV_ERR_ARG, "too many signatures in one store", cudaSuccess);
+    P.mstatus.assign(n_msgs, 0);
+    P.holder.assign(n_msgs, GS_NONE);
+    if (!n_msgs) {
+        if (done) {
+            CK(cudaEventRecord(done, st));
+            CK(cudaStreamSynchronize(st));
+        }
+        return SV_OK;
+    }
+    int rc = ensure_staging(ctx, items + extra_items);
+    if (!rc) rc = ensure_spans(ctx, items);
+    if (rc) return rc;
+    size_t cub_bytes = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const u64*)nullptr, (u64*)nullptr, (const u32*)nullptr,
+                                       (u32*)nullptr, (int)nev, 0, 64, st));
+    // one slab: per message [off u64][len u32][item base u32][status int][holder u32][signer 33B][kind 1B], per item
+    // [keyok 1B], per event [off u64][key u64 x2][msg u32][value u32 x2][kind 1B][ok 1B], chain hash, sort scratch
+    slab_layout L;
+    const size_t o_moff = L.take(8 * n_msgs), o_mlen = L.take(4 * n_msgs), o_base = L.take(4 * n_msgs),
+                 o_status = L.take(4 * n_msgs), o_holder = L.take(4 * n_msgs), o_sig = L.take(33 * n_msgs),
+                 o_kinds = L.take(n_msgs), o_keyok = L.take(items), o_eoff = L.take(8 * nev), o_key = L.take(8 * nev),
+                 o_key2 = L.take(8 * nev), o_emsg = L.take(4 * nev), o_val = L.take(4 * nev),
+                 o_val2 = L.take(4 * nev), o_ekind = L.take(nev), o_ok = L.take(nev), o_chain = L.take(32),
+                 o_cub = L.take(cub_bytes);
+    dev_buf<>& s = P.s;
+    rc = s.reserve(ctx, L.size, L.size);
+    if (rc) return rc;
+    u64 *d_moff = P.d_moff = s.at<u64>(o_moff), *d_eoff = P.d_eoff = s.at<u64>(o_eoff), *d_key = s.at<u64>(o_key),
+        *d_key2 = P.d_key2 = s.at<u64>(o_key2);
+    u32 *d_mlen = s.at<u32>(o_mlen), *d_base = P.d_base = s.at<u32>(o_base), *d_holder = P.d_holder = s.at<u32>(o_holder),
+        *d_emsg = P.d_emsg = s.at<u32>(o_emsg), *d_val = s.at<u32>(o_val), *d_val2 = P.d_val2 = s.at<u32>(o_val2);
+    int* d_status = P.d_status = s.at<int>(o_status);
+    u8 *d_signers = s + o_sig, *d_kinds = chain_hash32 ? s + o_kinds : nullptr, *d_keyok = s + o_keyok,
+       *d_ekind = P.d_ekind = s + o_ekind, *d_ok = P.d_ok = s + o_ok, *d_chain = chain_hash32 ? s + o_chain : nullptr;
+    CK(cudaMemcpyAsync(d_moff, P.moff.data(), 8 * n_msgs, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_mlen, P.mlen.data(), 4 * n_msgs, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_base, P.base.data(), 4 * n_msgs, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(d_holder, 0xFF, 4 * n_msgs, st));
+    CK(cudaMemsetAsync(d_signers, 0, 33 * n_msgs, st));  // an update without a channel keeps the all-zero key
+    if (chain_hash32) {
+        // with a chain hash, k_gossip_slice applies gossipd's gates (burst mode); every update's signer is given
+        CK(cudaMemsetAsync(d_kinds, 1, n_msgs, st));
+        CK(cudaMemcpyAsync(d_chain, chain_hash32, 32, cudaMemcpyHostToDevice, st));
+    }
+    if (nev) {
+        CK(cudaMemcpyAsync(d_eoff, P.eoff.data(), 8 * nev, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(d_emsg, P.emsg.data(), 4 * nev, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(d_ekind, P.ekind.data(), nev, cudaMemcpyHostToDevice, st));
+        k_store_events<<<(unsigned)((nev + 255) / 256), 256, 0, st>>>(d_store, len, d_eoff, d_ekind, nev, d_key, d_val, d_ok);
+        CK(cub::DeviceRadixSort::SortPairs(s + o_cub, cub_bytes, d_key, d_key2, d_val, d_val2, (int)nev, 0, 64, st));
+        k_store_resolve<<<(unsigned)((nev + 127) / 128), 128, 0, st>>>(d_store, d_key2, d_val2, d_ok, d_ekind, d_eoff, d_emsg,
+                                                                        nev, d_moff, d_holder, d_signers);
+        ctx->launches += 2;
+    }
+    unsigned gm = (unsigned)((n_msgs + 127) / 128);
+    k_gossip_slice<<<gm, 128, 0, st>>>(d_store, d_moff, d_mlen, d_base, d_signers, n_msgs, ctx->d_off, ctx->d_len,
+                                       ctx->d_key, ctx->d_sig, d_status, d_chain, d_kinds);
+    k_sha256d<<<(unsigned)((items + 127) / 128), 128, 0, st>>>(d_store, ctx->d_off, ctx->d_len, items, ctx->d_msg);
+    ctx->launches += 2;
+    rc = gossip_verify_items(ctx, ctx->d_msg, ctx->d_key, ctx->d_sig, items, ctx->d_verdict, st, d_keyok, &ctx->last_distinct);
+    if (rc) return rc;
+    k_gossip_status<<<gm, 128, 0, st>>>(d_store, d_moff, d_mlen, d_base, n_msgs, ctx->d_verdict, d_keyok, d_status,
+                                        d_kinds, nullptr, nullptr);
+    k_store_finish<<<(unsigned)((n_msgs + 255) / 256), 256, 0, st>>>(d_store, d_moff, d_holder, n_msgs, d_status);
+    ctx->launches += 2;
+    if (done) CK(cudaEventRecord(done, st));
+    CK(cudaMemcpyAsync(P.mstatus.data(), d_status, 4 * n_msgs, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(P.holder.data(), d_holder, 4 * n_msgs, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return SV_OK;
+}
+
 extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, size_t len, const uint8_t* chain_hash32,
                                            uint64_t* rec_off, uint16_t* rec_type, int* rec_status, uint64_t* rec_holder,
                                            size_t rec_capacity, sv_gossip_store_summary* sum) {
@@ -2122,93 +2310,11 @@ extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, si
     // the walk ends at the first bad checksum: only the records before it are verified
     size_t cut = bad < live_rec.size() ? live_rec[bad] : nrec;
     int cut_status = bad < live_rec.size() ? GS_ST_BAD_CRC : 0;
-    // messages (item slots laid out from the 2-byte type) and channel events before the cut, in store order
-    std::vector<u64> moff, eoff;
-    std::vector<u32> mlen, base, mrec, emsg, msg_of(nrec, GS_NONE);
-    std::vector<u8> ekind;
-    size_t items = 0;
-    for (size_t r = 0; r < cut; r++) {
-        if (rec[r].status != GS_LIVE) continue;
-        const u32 t = rec[r].type, m = (u32)moff.size();
-        if (t == 256 || t == 257 || t == 258) {
-            msg_of[r] = m;
-            moff.push_back(rec[r].off + GS_HDR); mlen.push_back(rec[r].len); base.push_back((u32)items); mrec.push_back((u32)r);
-            items += t == 256 ? 4 : 1;
-        }
-        const int k = t == 256 ? GS_EV_ANN : t == 258 ? GS_EV_UPD : t == GS_DELETE_CHAN ? GS_EV_DEL : -1;
-        if (k >= 0) {
-            eoff.push_back(rec[r].off + GS_HDR); ekind.push_back((u8)k);
-            emsg.push_back(k == GS_EV_DEL ? GS_NONE : m);
-        }
-    }
-    const size_t n_msgs = moff.size(), nev = eoff.size();
-    if (items >= 0xFFFFFFFFu || nev >= 0x7FFFFFFFu) return fail(ctx, SV_ERR_ARG, "too many signatures in one store", cudaSuccess);
-    std::vector<int> mstatus(n_msgs);
-    std::vector<u32> holder(n_msgs);
-    if (n_msgs) {
-        rc = ensure_staging(ctx, items);
-        if (!rc) rc = ensure_spans(ctx, items);
-        if (rc) return rc;
-        size_t cub_bytes = 0;
-        CK(cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const u64*)nullptr, (u64*)nullptr, (const u32*)nullptr,
-                                           (u32*)nullptr, (int)nev, 0, 64, st));
-        // one slab: per message [off u64][len u32][item base u32][status int][holder u32][signer 33B][kind 1B], per item
-        // [keyok 1B], per event [off u64][key u64 x2][msg u32][value u32 x2][kind 1B][ok 1B], chain hash, sort scratch
-        slab_layout L;
-        const size_t o_moff = L.take(8 * n_msgs), o_mlen = L.take(4 * n_msgs), o_base = L.take(4 * n_msgs),
-                     o_status = L.take(4 * n_msgs), o_holder = L.take(4 * n_msgs), o_sig = L.take(33 * n_msgs),
-                     o_kinds = L.take(n_msgs), o_keyok = L.take(items), o_eoff = L.take(8 * nev), o_key = L.take(8 * nev),
-                     o_key2 = L.take(8 * nev), o_emsg = L.take(4 * nev), o_val = L.take(4 * nev),
-                     o_val2 = L.take(4 * nev), o_ekind = L.take(nev), o_ok = L.take(nev), o_chain = L.take(32),
-                     o_cub = L.take(cub_bytes);
-        dev_buf<> s;
-        rc = s.reserve(ctx, L.size, L.size);
-        if (rc) return rc;
-        u64 *d_moff = s.at<u64>(o_moff), *d_eoff = s.at<u64>(o_eoff), *d_key = s.at<u64>(o_key), *d_key2 = s.at<u64>(o_key2);
-        u32 *d_mlen = s.at<u32>(o_mlen), *d_base = s.at<u32>(o_base), *d_holder = s.at<u32>(o_holder),
-            *d_emsg = s.at<u32>(o_emsg), *d_val = s.at<u32>(o_val), *d_val2 = s.at<u32>(o_val2);
-        int* d_status = s.at<int>(o_status);
-        u8 *d_signers = s + o_sig, *d_kinds = chain_hash32 ? s + o_kinds : nullptr, *d_keyok = s + o_keyok,
-           *d_ekind = s + o_ekind, *d_ok = s + o_ok, *d_chain = chain_hash32 ? s + o_chain : nullptr;
-        CK(cudaMemcpyAsync(d_moff, moff.data(), 8 * n_msgs, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(d_mlen, mlen.data(), 4 * n_msgs, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(d_base, base.data(), 4 * n_msgs, cudaMemcpyHostToDevice, st));
-        CK(cudaMemsetAsync(d_holder, 0xFF, 4 * n_msgs, st));
-        CK(cudaMemsetAsync(d_signers, 0, 33 * n_msgs, st));  // an update without a channel keeps the all-zero key
-        if (chain_hash32) {
-            // with a chain hash, k_gossip_slice applies gossipd's gates (burst mode); every update's signer is given
-            CK(cudaMemsetAsync(d_kinds, 1, n_msgs, st));
-            CK(cudaMemcpyAsync(d_chain, chain_hash32, 32, cudaMemcpyHostToDevice, st));
-        }
-        if (nev) {
-            CK(cudaMemcpyAsync(d_eoff, eoff.data(), 8 * nev, cudaMemcpyHostToDevice, st));
-            CK(cudaMemcpyAsync(d_emsg, emsg.data(), 4 * nev, cudaMemcpyHostToDevice, st));
-            CK(cudaMemcpyAsync(d_ekind, ekind.data(), nev, cudaMemcpyHostToDevice, st));
-            k_store_events<<<(unsigned)((nev + 255) / 256), 256, 0, st>>>(d_store, len, d_eoff, d_ekind, nev, d_key, d_val, d_ok);
-            CK(cub::DeviceRadixSort::SortPairs(s + o_cub, cub_bytes, d_key, d_key2, d_val, d_val2, (int)nev, 0, 64, st));
-            k_store_resolve<<<(unsigned)((nev + 127) / 128), 128, 0, st>>>(d_store, d_key2, d_val2, d_ok, d_ekind, d_eoff, d_emsg,
-                                                                            nev, d_moff, d_holder, d_signers);
-            ctx->launches += 2;
-        }
-        unsigned gm = (unsigned)((n_msgs + 127) / 128);
-        k_gossip_slice<<<gm, 128, 0, st>>>(d_store, d_moff, d_mlen, d_base, d_signers, n_msgs, ctx->d_off, ctx->d_len,
-                                           ctx->d_key, ctx->d_sig, d_status, d_chain, d_kinds);
-        k_sha256d<<<(unsigned)((items + 127) / 128), 128, 0, st>>>(d_store, ctx->d_off, ctx->d_len, items, ctx->d_msg);
-        ctx->launches += 2;
-        rc = gossip_verify_items(ctx, ctx->d_msg, ctx->d_key, ctx->d_sig, items, ctx->d_verdict, st, d_keyok, &ctx->last_distinct);
-        if (rc) return rc;
-        k_gossip_status<<<gm, 128, 0, st>>>(d_store, d_moff, d_mlen, d_base, n_msgs, ctx->d_verdict, d_keyok, d_status,
-                                            d_kinds, nullptr, nullptr);
-        k_store_finish<<<(unsigned)((n_msgs + 255) / 256), 256, 0, st>>>(d_store, d_moff, d_holder, n_msgs, d_status);
-        ctx->launches += 2;
-        if (ev.e[3]) CK(cudaEventRecord(ev.e[3], st));
-        CK(cudaMemcpyAsync(mstatus.data(), d_status, 4 * n_msgs, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(holder.data(), d_holder, 4 * n_msgs, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-    } else if (ev.e[3]) {
-        CK(cudaEventRecord(ev.e[3], st));
-        CK(cudaStreamSynchronize(st));
-    }
+    store_pass P;
+    rc = store_pass_run(ctx, d_store, len, chain_hash32, rec, cut, nullptr, 0, P, ev.e[3]);
+    if (rc) return rc;
+    const std::vector<u32>&msg_of = P.msg_of, &mrec = P.mrec, &holder = P.holder;
+    const std::vector<int>& mstatus = P.mstatus;
     // an announcement without room for its amount record stops the walk unless it is redundant (add_channel returns the
     // channel that already holds the scid before it looks for the amount)
     if (we.no_amount < cut && holder[msg_of[we.no_amount]] == GS_NONE) {
@@ -2262,6 +2368,184 @@ extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, si
 extern "C" int sv_get_last_gossip_store_timing(sv_ctx* ctx, float* ms4) {
     if (!ctx || !ctx->profiling || !ms4) return SV_ERR_ARG;
     for (int i = 0; i < 4; i++) ms4[i] = ctx->gs_ms[i];
+    return SV_OK;
+}
+
+// ---- pruning a gossip_store: the records gossmap should not trust marked deleted (see cln_sigverify.h) --------------
+extern "C" size_t sv_gossip_prune_count(const uint8_t* store, size_t len) {
+    if (!store || len < 1) return 0;
+    gs_walk_end we;
+    return (size_t)gs_walk(store, len, [](const gs_rec&) {}, &we, true);
+}
+
+extern "C" int sv_prune_gossip_store_host(sv_ctx* ctx, const uint8_t* store, size_t len, const uint8_t* chain_hash32,
+                                          uint8_t* out, uint64_t* rec_off, uint16_t* rec_type, int* rec_status,
+                                          uint8_t* rec_pruned, size_t rec_capacity, sv_gossip_prune_summary* sum) {
+    if (!ctx || !store || !out || len < 1 || !sum || (rec_capacity && (!rec_off || !rec_type || !rec_status || !rec_pruned)))
+        return SV_ERR_ARG;
+    if (store[0] >> 5) return fail(ctx, SV_ERR_ARG, "gossip_store major version is not 0", cudaSuccess);
+    const auto t0 = std::chrono::steady_clock::now();
+    gs_walk_end we;
+    std::vector<gs_rec> rec;
+    rec.reserve(len / 256 + 16);
+    const size_t nrec = gs_walk(store, len, [&rec](const gs_rec& r) { rec.push_back(r); }, &we, true);
+    if (nrec > rec_capacity) return fail(ctx, SV_ERR_ARG, "rec_capacity is below the store's record count", cudaSuccess);
+    if (nrec >= 0xFFFFFFFFu) return fail(ctx, SV_ERR_ARG, "too many records", cudaSuccess);
+    // every live record's checksum is tested (the ENDED record that stops the walk is left alone)
+    std::vector<u64> live_off;
+    std::vector<u32> live_rec;
+    size_t n_upd = 0;
+    for (size_t r = 0; r < nrec; r++)
+        if (rec[r].status == GS_LIVE) {
+            live_off.push_back(rec[r].off);
+            live_rec.push_back((u32)r);
+            n_upd += rec[r].type == 258;
+        }
+    const float walk_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    dev_guard dg__;
+    CK(dg__.enter(ctx->device));
+    cudaStream_t st = ctx->stream;
+    ev_set ev;
+    if (ctx->profiling)
+        for (cudaEvent_t& e : ev.e) CK(cudaEventCreate(&e));
+    dev_buf<> d_store, t_live;
+    const size_t nlive = live_off.size(), live_bytes = nlive * 9 + 16;
+    int rc = d_store.reserve(ctx, len, len);
+    if (!rc) rc = t_live.reserve(ctx, live_bytes, live_bytes);
+    if (rc) return rc;
+    u64* d_live = t_live.at<u64>(0);
+    u8* d_bad = t_live.at<u8>(nlive * 8);
+    if (ev.e[0]) CK(cudaEventRecord(ev.e[0], st));
+    CK(cudaMemcpyAsync(d_store, store, len, cudaMemcpyHostToDevice, st));
+    std::vector<u8> bad_live(nlive), skip(nrec, 0);
+    if (nlive) {
+        CK(cudaMemcpyAsync(d_live, live_off.data(), nlive * 8, cudaMemcpyHostToDevice, st));
+        k_store_crc_flags<<<(unsigned)((nlive + 255) / 256), 256, 0, st>>>(d_store, d_live, nlive, d_bad);
+        ctx->launches += 1;
+        CK(cudaMemcpyAsync(bad_live.data(), d_bad, nlive, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+    }
+    for (size_t k = 0; k < nlive; k++) skip[live_rec[k]] = bad_live[k];
+    // first round: the audit's statuses and channel table over the records with good checksums
+    store_pass P;
+    rc = store_pass_run(ctx, d_store, len, chain_hash32, rec, nrec, skip.data(), n_upd, P, ev.e[1]);
+    if (rc) return rc;
+    const size_t n_msgs = P.n_msgs, nev = P.nev, items = P.items;
+    std::vector<u8> reason(n_msgs, SV_GP_KEPT);
+    u32 n_moved = 0;
+    if (n_msgs) {
+        // second round: the deletions of the first, the table again over the sorted events with those announcements
+        // masked out, and the updates whose holder changed verified again under their new signer
+        slab_layout L;
+        const size_t o_reason = L.take(n_msgs), o_holder2 = L.take(4 * n_msgs), o_sig2 = L.take(33 * n_msgs),
+                     o_ok2 = L.take(nev), o_list = L.take(4 * (n_upd + 1)), o_keyok = L.take(n_upd);
+        dev_buf<> s2;
+        rc = s2.reserve(ctx, L.size, L.size);
+        if (rc) return rc;
+        u8 *d_reason = s2 + o_reason, *d_sig2 = s2 + o_sig2, *d_ok2 = s2 + o_ok2, *d_keyok = s2 + o_keyok;
+        u32 *d_holder2 = s2.at<u32>(o_holder2), *d_list = s2.at<u32>(o_list);
+        CK(cudaMemsetAsync(d_holder2, 0xFF, 4 * n_msgs, st));
+        CK(cudaMemsetAsync(d_list, 0, 4, st));
+        const size_t nmark = n_msgs > nev ? n_msgs : nev;
+        k_prune_mark<<<(unsigned)((nmark + 255) / 256), 256, 0, st>>>(d_store, P.d_moff, P.d_status, n_msgs, P.d_ekind,
+                                                                     P.d_emsg, P.d_ok, nev, d_reason, d_ok2);
+        ctx->launches += 1;
+        if (nev) {
+            k_store_resolve<<<(unsigned)((nev + 127) / 128), 128, 0, st>>>(d_store, P.d_key2, P.d_val2, d_ok2, P.d_ekind,
+                                                                            P.d_eoff, P.d_emsg, nev, P.d_moff, d_holder2,
+                                                                            d_sig2);
+            ctx->launches += 1;
+        }
+        k_prune_select<<<(unsigned)((n_msgs + 127) / 128), 128, 0, st>>>(d_store, P.d_moff, P.d_status, n_msgs, P.d_holder,
+                                                                        d_holder2, P.d_base, d_sig2, d_reason, d_list,
+                                                                        (u32)items, ctx->d_msg, ctx->d_key, ctx->d_sig);
+        ctx->launches += 1;
+        CK(cudaMemcpyAsync(&n_moved, d_list, 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        if (n_moved) {
+            rc = gossip_verify_items(ctx, ctx->d_msg + 32 * items, ctx->d_key + 33 * items, ctx->d_sig + 64 * items, n_moved,
+                                     ctx->d_verdict + items, st, d_keyok, nullptr);
+            if (rc) return rc;
+            k_prune_settle<<<(n_moved + 255) / 256, 256, 0, st>>>(d_list, ctx->d_verdict + items, d_reason);
+            ctx->launches += 1;
+        }
+        if (ev.e[2]) CK(cudaEventRecord(ev.e[2], st));
+        CK(cudaMemcpyAsync(reason.data(), d_reason, n_msgs, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+    } else if (ev.e[2]) {
+        CK(cudaEventRecord(ev.e[2], st));
+    }
+    // every record's reason, in store order
+    std::vector<u8> pr(nrec, SV_GP_KEPT);
+    for (size_t r = 0; r < nrec; r++) {
+        const u32 t = rec[r].type, m = P.msg_of[r];
+        if (rec[r].status == GS_ST_TRUNCATED) pr[r] = SV_GP_TRUNCATED;
+        else if (rec[r].status != GS_LIVE) continue;
+        else if (skip[r]) pr[r] = SV_GP_BAD_CRC;
+        else if (m != GS_NONE) pr[r] = reason[m];
+        else if (t != GS_CHANNEL_AMOUNT && t != GS_DELETE_CHAN && t != GS_CHAN_DYING && t != GS_UUID) pr[r] = SV_GP_UNKNOWN;
+        // the amount record right after a deleted announcement goes with it (gossip_store_del)
+        if (r > 0 && pr[r] == SV_GP_KEPT && t == GS_CHANNEL_AMOUNT && pr[r - 1] != SV_GP_KEPT && rec[r - 1].type == 256)
+            pr[r] = SV_GP_AMOUNT;
+    }
+    // an announcement kept without room for its amount record stops the walk: it and the records after it stay
+    size_t cut = nrec;
+    if (we.no_amount < nrec && pr[we.no_amount] == SV_GP_KEPT) cut = we.no_amount;
+    std::vector<u64> doff;
+    for (size_t r = 0; r < cut; r++)
+        if (pr[r] != SV_GP_KEPT) doff.push_back(rec[r].off);
+    // the flag writes on the device; only the changed flag bytes come back
+    const size_t nd = doff.size();
+    std::vector<u8> flag_hi(nd);
+    if (nd) {
+        dev_buf<> t_del;
+        rc = t_del.reserve(ctx, nd * 9, nd * 9);
+        if (rc) return rc;
+        u64* d_doff = t_del.at<u64>(0);
+        u8* d_hi = t_del.at<u8>(nd * 8);
+        CK(cudaMemcpyAsync(d_doff, doff.data(), nd * 8, cudaMemcpyHostToDevice, st));
+        k_prune_flags<<<(unsigned)((nd + 255) / 256), 256, 0, st>>>(d_store, d_doff, nd, d_hi);
+        ctx->launches += 1;
+        CK(cudaMemcpyAsync(flag_hi.data(), d_hi, nd, cudaMemcpyDeviceToHost, st));
+    }
+    if (ev.e[3]) CK(cudaEventRecord(ev.e[3], st));
+    CK(cudaStreamSynchronize(st));
+    if (out != store) memcpy(out, store, len);
+    for (size_t i = 0; i < nd; i++) out[doff[i]] = flag_hi[i];
+    sv_gossip_prune_summary S;
+    memset(&S, 0, sizeof S);
+    S.version = store[0];
+    S.stop = cut < nrec ? GS_ST_NO_AMOUNT : we.stop;
+    S.end_offset = cut < nrec ? rec[cut].off : we.end;
+    S.records = nrec;
+    S.reverified = n_moved;
+    uint64_t* per_reason[9] = {nullptr, &S.bad_crc, &S.truncated, &S.message, &S.redundant, &S.no_channel,
+                               &S.signature, &S.amount, &S.unknown};
+    for (size_t r = 0; r < nrec; r++) {
+        const u32 t = rec[r].type, m = P.msg_of[r];
+        int s = rec[r].status;
+        if (r >= cut) s = r == cut ? GS_ST_NO_AMOUNT : GS_ST_NOT_REACHED;
+        else if (s == GS_LIVE && skip[r]) s = GS_ST_BAD_CRC;
+        else if (s == GS_LIVE && m != GS_NONE) s = P.mstatus[m];
+        else if (s == GS_LIVE)
+            s = (t == GS_CHANNEL_AMOUNT || t == GS_DELETE_CHAN || t == GS_CHAN_DYING || t == GS_UUID) ? GS_ST_STORE_RECORD
+                                                                                                      : GS_ST_UNKNOWN;
+        const u8 why = r < cut ? pr[r] : (u8)SV_GP_KEPT;
+        rec_off[r] = rec[r].off;
+        rec_type[r] = (uint16_t)t;
+        rec_status[r] = s;
+        rec_pruned[r] = why;
+        if (why) { S.pruned++; (*per_reason[why])++; }
+    }
+    *sum = S;
+    ctx->gp_ms[0] = walk_ms;
+    if (ev.e[0])
+        for (int i = 0; i < 3; i++) CK(cudaEventElapsedTime(&ctx->gp_ms[1 + i], ev.e[i], ev.e[i + 1]));
+    return SV_OK;
+}
+extern "C" int sv_get_last_gossip_prune_timing(sv_ctx* ctx, float* ms4) {
+    if (!ctx || !ctx->profiling || !ms4) return SV_ERR_ARG;
+    for (int i = 0; i < 4; i++) ms4[i] = ctx->gp_ms[i];
     return SV_OK;
 }
 

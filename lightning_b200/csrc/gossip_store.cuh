@@ -127,9 +127,10 @@ struct gs_walk_end {
     u64 no_amount;  // entry of the first live announcement whose amount record would not fit, or ~0
 };
 // emit(const gs_rec&) receives the entries in store order: one pass, because each header's position depends on the one
-// before it (on a store larger than the caches every record costs a memory latency).
+// before it (on a store larger than the caches every record costs a memory latency).  past_truncated (the prune's walk,
+// which deletes such a record): a GS_ST_TRUNCATED record does not stop the walk.
 template <typename Emit>
-static inline u64 gs_walk(const u8* s, u64 len, Emit emit, gs_walk_end* e) {
+static inline u64 gs_walk(const u8* s, u64 len, Emit emit, gs_walk_end* e, bool past_truncated = false) {
     auto be16 = [](const u8* p) { return ((u32)p[0] << 8) | p[1]; };
     u64 off = 1, n = 0;
     e->stop = 0;
@@ -146,7 +147,7 @@ static inline u64 gs_walk(const u8* s, u64 len, Emit emit, gs_walk_end* e) {
         if (r.status == GS_LIVE && r.type == 256 && e->no_amount == ~(u64)0 && off + GS_HDR + msglen + GS_HDR + 2 + 8 > len)
             e->no_amount = n;
         emit(r);
-        if (r.status != GS_LIVE && r.status != GS_ST_DELETED) {
+        if (r.status != GS_LIVE && r.status != GS_ST_DELETED && !(past_truncated && r.status == GS_ST_TRUNCATED)) {
             e->stop = r.status;
             n++;
             break;

@@ -50,6 +50,18 @@ GS_INCOMPLETE, GS_PARTIAL, GS_TRUNCATED, GS_BAD_CRC, GS_ENDED, GS_NO_AMOUNT = 32
 GS_NO_HOLDER = (1 << 64) - 1
 
 
+class SvGossipPruneSummary(ctypes.Structure):
+    """sv_gossip_prune_summary (include/cln_sigverify.h)"""
+    _fields_ = [("version", ctypes.c_uint32), ("stop", ctypes.c_int32)] + [(f, ctypes.c_uint64) for f in (
+        "end_offset", "records", "pruned", "bad_crc", "truncated", "message", "redundant", "no_channel", "signature",
+        "amount", "unknown", "reverified")]
+
+
+# why prune_gossip_store deletes a record (include/cln_sigverify.h SV_GP_*; 0 = kept)
+GP_KEPT, GP_BAD_CRC, GP_TRUNCATED, GP_MESSAGE, GP_REDUNDANT, GP_NO_CHANNEL, GP_SIGNATURE, GP_AMOUNT, GP_UNKNOWN = range(9)
+GP_REASONS = ("kept", "bad_crc", "truncated", "message", "redundant", "no_channel", "signature", "amount", "unknown")
+
+
 class SvInfo(ctypes.Structure):
     _fields_ = [("device", ctypes.c_int), ("sm_count", ctypes.c_int), ("main_block", ctypes.c_int),
                 ("main_grid", ctypes.c_int), ("main_regs", ctypes.c_int), ("gtable_bytes", ctypes.c_size_t),
@@ -81,6 +93,10 @@ def load_library():
     lib.sv_gossip_store_count.restype = sz
     lib.sv_verify_gossip_store_host.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp, sz, ctypes.POINTER(SvGossipStoreSummary)]
     lib.sv_get_last_gossip_store_timing.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
+    lib.sv_gossip_prune_count.argtypes = [vp, sz]
+    lib.sv_gossip_prune_count.restype = sz
+    lib.sv_prune_gossip_store_host.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp, vp, sz, ctypes.POINTER(SvGossipPruneSummary)]
+    lib.sv_get_last_gossip_prune_timing.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
     lib.sv_verify_tx_host.argtypes = [vp, i, vp, vp, sz, vp, vp, sz, vp, vp]
     lib.sv_grind_tx_fee_host.argtypes = [vp, i, vp, vp, sz, vp, vp, ctypes.c_uint64, ctypes.c_uint32, ctypes.c_uint32,
                                          ctypes.POINTER(ctypes.c_int64), ctypes.POINTER(ctypes.c_uint64)]
@@ -275,6 +291,39 @@ class SigVerifier:
         """(header walk, H2D, checksums, verification) in ms of the last verify_gossip_store (profiling mode)"""
         ms = (ctypes.c_float * 4)()
         self._check(self.lib.sv_get_last_gossip_store_timing(self._ctx, ms), "sv_get_last_gossip_store_timing")
+        return tuple(ms)
+
+    def prune_gossip_store(self, store, chain_hash=None, capacity=None):
+        """Mark every record of a gossip_store that gossmap should not trust as deleted (flag bit 0x8000), so that
+        gossipd's strict load accepts the store and keeps the rest.  Returns (pruned_bytes, records, summary): the store
+        with those bits set (same length; the input is not changed), records = (rec_off uint64, rec_type uint16,
+        rec_status int32 (the first-round status), rec_pruned uint8 (GP_* reason, 0 = kept)), and the summary dict with
+        the deletions per reason.  capacity: entries to provide (default: sv_gossip_prune_count)."""
+        buf = np.frombuffer(bytes(store), dtype=np.uint8)
+        chain = None
+        if chain_hash is not None:
+            chain = np.frombuffer(bytes(chain_hash), dtype=np.uint8)
+            if chain.size != 32:
+                raise ValueError("chain_hash must be 32 bytes")
+        n = int(self.lib.sv_gossip_prune_count(buf.ctypes.data, buf.size)) if capacity is None else int(capacity)
+        out = np.empty(max(buf.size, 1), np.uint8)
+        off = np.zeros(max(n, 1), np.uint64)
+        typ = np.zeros(max(n, 1), np.uint16)
+        status = np.zeros(max(n, 1), np.int32)
+        pruned = np.zeros(max(n, 1), np.uint8)
+        s = SvGossipPruneSummary()
+        self._check(self.lib.sv_prune_gossip_store_host(
+            self._ctx, buf.ctypes.data, buf.size, chain.ctypes.data if chain is not None else None, out.ctypes.data,
+            off.ctypes.data, typ.ctypes.data, status.ctypes.data, pruned.ctypes.data, n, ctypes.byref(s)),
+            "sv_prune_gossip_store_host")
+        summary = {f: getattr(s, f) for f, _ in SvGossipPruneSummary._fields_}
+        k = s.records
+        return out[:buf.size].tobytes(), (off[:k], typ[:k], status[:k], pruned[:k]), summary
+
+    def last_gossip_prune_timing(self):
+        """(header walk, first round, second round, flag write) in ms of the last prune_gossip_store (profiling mode)"""
+        ms = (ctypes.c_float * 4)()
+        self._check(self.lib.sv_get_last_gossip_prune_timing(self._ctx, ms), "sv_get_last_gossip_prune_timing")
         return tuple(ms)
 
     def verify_samekey(self, kind, key, msg32, sig64):
