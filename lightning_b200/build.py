@@ -24,9 +24,8 @@ STORE_TOOL = os.path.join(ROOT, "lightning_b200", "cln_verify_gossip_store")
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
-    # curve-side kernel variant: inlined field arithmetic + CTA-wide re-convergence barriers (see engine.cu);
-    # in the ladder one barrier every 2 windows (tools/variants.py compares the other spacings)
-    "-DSV_FE_INLINE", "-DSV_MAIN_SYNC", "-DSV_SYNC_LEVEL=1", "-DSV_SYNC_WINDOWS=2",
+    # curve-side kernel: inlined field arithmetic + CTA-wide re-convergence barriers (see fe.cuh and common.cuh)
+    "-DSV_FE_INLINE", "-DSV_MAIN_SYNC",
 ]
 # gcc flags of the plain-C parts: the drop-in (linked into the library) and the verifier subdaemon
 DROPIN_CFLAGS = ["-O2", "-fPIC", "-Wall", "-Wextra", "-std=c11"]
@@ -47,12 +46,12 @@ def _sources(d, exts):
     return out
 
 
-def build_engine(force=False, verbose=False, extra_flags=()):
+def build_engine(force=False, verbose=False):
     srcs = _sources(CSRC, (".cu", ".cuh", ".c", ".h")) + [os.path.join(ROOT, "include", "cln_sigverify.h"),
                                                    os.path.join(ROOT, "include", "cln_dropin.h")]
-    # the flags are part of what the library is: a change of flags (or extra_flags) must rebuild, and so must a stale daemon
+    # the flags are part of what the library is: a change of flags must rebuild, and so must a stale daemon
     stamp = os.path.join(os.path.dirname(LIB), ".build_flags")
-    flags_now = " ".join(NVCC_FLAGS + list(extra_flags))
+    flags_now = " ".join(NVCC_FLAGS)
     same_flags = os.path.exists(stamp) and open(stamp).read() == flags_now
     if not force and same_flags and _newer(LIB, srcs) and _newer(DAEMON, srcs) and _newer(STORE_TOOL, srcs):
         return LIB
@@ -72,7 +71,7 @@ def build_engine(force=False, verbose=False, extra_flags=()):
         sys.stderr.write(r.stderr)
     if r.returncode != 0:
         raise RuntimeError("nvcc (batch.cu) failed:\n" + r.stdout + r.stderr)
-    cmd = [nvcc] + NVCC_FLAGS + list(extra_flags) + (["-Xptxas", "-v"] if verbose else []) + [
+    cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + [
         "-o", LIB, os.path.join(CSRC, "engine.cu"), batch_o, dropin_o]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if verbose:

@@ -38,17 +38,12 @@
 #define SV_CDATA
 #endif
 
-// CTA-wide re-convergence points of the curve-side kernel (only in the SV_MAIN_SYNC build variant, where the
+// CTA-wide re-convergence points of the curve-side kernel (only in the SV_MAIN_SYNC build, where the
 // field arithmetic is inlined and the warps of a CTA are kept at the same PC to share instruction fetches)
 #if defined(__CUDACC__) && defined(SV_MAIN_SYNC)
-#ifdef SV_MAP_INTERLEAVED
-// (variant) the last, partial round runs with fewer warps per CTA: COUNTED named barrier, count in a register
-#define SV_SYNC(n) asm volatile("bar.sync 1, %0;" ::"r"(n))
-#else
 // n = number of threads taking part (the whole CTA) or 0: no barrier (callers that run in ONE warp of a larger CTA — the
 // small-batch kernel — must not hit CTA-wide barriers)
 #define SV_SYNC(n) do { if (n) __syncthreads(); } while (0)
-#endif
 #else
 #define SV_SYNC(n) ((void)(n))
 #endif

@@ -26,8 +26,6 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <stdio.h>
 #include <chrono>
-#include <map>
-#include <mutex>
 #include <stdlib.h>
 #include <string.h>
 #include <string>
@@ -40,30 +38,15 @@
 #include "selftest.cuh"
 #include "batch.cuh"  // constants and the host-testable stages; the kernels themselves are in batch.cu
 
-// Build variants of the curve-side kernel (tools/variants.py times them at 1 M ECDSA33 verifications):
-//   default  SV_FE_INLINE + SV_MAIN_SYNC, 256 threads x 2 CTAs/SM : field arithmetic inlined, the warps of a CTA
-//            re-converge at a __syncthreads() before every point operation so that they walk the (large) code
-//            together and share instruction fetches
-//   -DSV_NO_SYNC_INLINE  fe_mul/fe_sqr as real functions, 128 x 4, no barriers
-//   (everything inlined WITHOUT barriers starves on instruction fetch)
 #if !defined(SV_NO_SYNC_INLINE) && !defined(SV_FE_INLINE)
 #error "compile with -DSV_FE_INLINE -DSV_MAIN_SYNC (default build) or -DSV_NO_SYNC_INLINE; see lightning_b200/build.py"
 #endif
-#ifndef SV_MAIN_BLOCK
 #ifdef SV_MAIN_SYNC
 #define SV_MAIN_BLOCK 256
 #else
 #define SV_MAIN_BLOCK 128
 #endif
-#endif
-#ifndef SV_MAIN_MINB
 #define SV_MAIN_MINB (512 / SV_MAIN_BLOCK)
-#endif
-#ifdef SV_COMB_SMEM
-#define SV_MAIN_SMEM (17 * 128 * 64)  // the variant's shared-memory comb table
-#else
-#define SV_MAIN_SMEM 0
-#endif
 
 // -------------------------------------------------------------------------------------------------
 // kernels
@@ -147,45 +130,11 @@ __global__ void __launch_bounds__(128) k_prep_schnorr(const u8* msg, const u8* k
 // (They must not alias a live record: the BIP-340 path overwrites records with the parked R.)
 __device__ sv_work g_idle_work = {{1, 0, 0, 0, 0}, {1, 0, 0, 0, 0}, {0}, 0, {0}};
 
-#ifdef SV_COMB_SMEM
-__device__ const ge_mem* g_t8;  // 17 x 128 entries d * 2^(8 i) * G in global memory, source of the per-CTA shared copy
-__global__ void k_t8_fill(ge_mem* t8, const ge_mem* gtab) {
-    u32 e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= 17 * 128) return;
-    u32 row = e / 128, d = e % 128 + 1;  // d * 2^(8 row) G = (d << (8 (row & 1))) * 2^(16 (row / 2)) G
-    t8[e] = gtab[(size_t)(row >> 1) * SV_GT_ROW + ((d << (8 * (row & 1))) - 1)];
-}
-#endif
 template <int KIND>
 __global__ void __launch_bounds__(SV_MAIN_BLOCK, SV_MAIN_MINB)
     k_main(sv_work* work, const u8* __restrict__ key, const u8* __restrict__ sig, size_t n,
            const ge_mem* __restrict__ gtab, qtab_entry* scratch, u8* __restrict__ verdict, u8* keyok) {
     const size_t keylen = (KIND == SV_KIND_ECDSA33 || KIND == SV_KIND_ECDSA33_NS) ? 33 : (KIND == SV_KIND_ECDSA_XY ? 64 : 32);
-#ifdef SV_COMB_SMEM
-    // VARIANT: the 17 x 128-entry 8-bit comb (136 KiB) is staged in shared memory once per (persistent) CTA by ONE bulk
-    // asynchronous copy (cp.async.bulk: the TMA engine, UBLKCP in SASS), completion signalled on an mbarrier
-    {
-        extern __shared__ __align__(16) unsigned char sv_smem_raw[];
-        __shared__ __align__(8) unsigned long long sv_bar;
-        const unsigned bytes = 17u * 128u * (unsigned)sizeof(ge_mem);
-        unsigned bar = (unsigned)__cvta_generic_to_shared(&sv_bar), dst = (unsigned)__cvta_generic_to_shared(sv_smem_raw);
-        if (threadIdx.x == 0) {
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(dst), "l"(g_t8), "r"(bytes), "r"(bar) : "memory");
-        }
-        unsigned done = 0;
-        while (!done)
-            asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                         : "=r"(done) : "r"(bar) : "memory");
-    }
-#endif
-#ifndef SV_MAP_INTERLEAVED
     size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     size_t stride = (size_t)gridDim.x * blockDim.x;
     qtab_entry* tab = scratch + tid * 8;
@@ -196,25 +145,6 @@ __global__ void __launch_bounds__(SV_MAIN_BLOCK, SV_MAIN_MINB)
         bool active = i < n;
         size_t j = active ? i : 0;
         const unsigned part = SV_MAIN_BLOCK;  // every thread of the CTA reaches every re-convergence barrier
-#else
-    // VARIANT (slower at 1 M when last measured): interleaved item mapping — in round k thread t of
-    // CTA c takes item k*T + t*G + c, so a partial last round keeps the first warps of EVERY CTA busy, the idle warps
-    // leave, and the re-convergence barrier counts only the warps taking part.
-    const unsigned G = gridDim.x, B = blockDim.x;
-    const size_t T = (size_t)G * B;
-    qtab_entry* tab = scratch + ((size_t)blockIdx.x * B + threadIdx.x) * 8;
-    const size_t r = (size_t)threadIdx.x * G + blockIdx.x;
-    for (size_t base = 0; base < n; base += T) {
-        const size_t rem = n - base;
-        unsigned act = B;
-        if (rem < T) act = (rem > blockIdx.x) ? (unsigned)(((rem - blockIdx.x + G - 1) / G) < B ? ((rem - blockIdx.x + G - 1) / G) : B) : 0u;
-        const unsigned part = (act + 31u) & ~31u;  // whole warps
-        __syncthreads();  // all warps are out of the previous round's counted barriers before the count may change
-        if (threadIdx.x >= part) return;  // only possible in the last round
-        const size_t i = base + r;
-        const bool active = r < rem;
-        const size_t j = active ? i : 0;
-#endif
         const sv_work* w = active ? (work + i) : &g_idle_work;
         if (KIND == SV_KIND_ECDSA33_NS) {
             // compressed-key ECDSA without the square root: D, B, c parked in the work record, k_final_ecdsa33 decides
@@ -1463,29 +1393,6 @@ static int ensure_spans(sv_ctx* ctx, size_t n) {
 }
 static int ensure_gbuf(sv_ctx* ctx, size_t bytes) { return ctx->g_buf.reserve(ctx, bytes, SV_GBUF_FLOOR); }
 
-#ifdef SV_COMB_SMEM
-// g_t8 is one pointer per device, read by the curve kernel of every context on that device, so the table it points to
-// belongs to the device, not to a context: the first context created on a device fills it from its G table (every
-// context's G table is the same), and it stays allocated for the life of the process.  The map is never destroyed, so
-// no cudaFree runs during static destruction.
-static int comb_t8_init(sv_ctx* ctx) {
-    struct table { dev_buf<ge_mem> t8; bool ready = false; };
-    static std::mutex mu;
-    static std::map<int, table>* tables = new std::map<int, table>;
-    std::lock_guard<std::mutex> lock(mu);
-    table& t = (*tables)[ctx->device];
-    if (t.ready) return SV_OK;
-    int rc = t.t8.reserve(ctx, 17 * 128 * sizeof(ge_mem), 17 * 128 * sizeof(ge_mem));
-    if (rc) return rc;
-    k_t8_fill<<<17, 128, 0, ctx->stream>>>(t.t8, ctx->d_gtab);
-    CK(cudaGetLastError());
-    CK(cudaMemcpyToSymbolAsync(g_t8, &t.t8.p, sizeof(t.t8.p), 0, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    t.ready = true;
-    return SV_OK;
-}
-#endif
-
 // everything sv_create sets up after the defaults, on the context's device
 static int ctx_init(sv_ctx* ctx) {
     cudaDeviceProp prop;
@@ -1501,7 +1408,7 @@ static int ctx_init(sv_ctx* ctx) {
     if (rc) return rc;
     CK(cudaHostAlloc((void**)&ctx->h_small, (size_t)SV_SMALL_CAP * (32 + 64 + 64 + 2), cudaHostAllocMapped | cudaHostAllocPortable));
     int occ = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_main<SV_KIND_ECDSA33>, SV_MAIN_BLOCK, SV_MAIN_SMEM));
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_main<SV_KIND_ECDSA33>, SV_MAIN_BLOCK, 0));
     if (occ < 1) occ = 1;
     ctx->main_grid = ctx->sm_count * occ;
     // deployment knob: leave a few CTA slots of the persistent curve kernel free for a collective's kernel that becomes
@@ -1537,14 +1444,6 @@ static int ctx_init(sv_ctx* ctx) {
     k_gtable_fill<<<(SV_GT_ENTRIES + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_gtab, ctx->d_bases);
     ctx->launches += 2;
     CK(cudaGetLastError());
-#ifdef SV_COMB_SMEM
-    rc = comb_t8_init(ctx);
-    if (rc) return rc;
-    const int smem = 17 * 128 * (int)sizeof(ge_mem);
-    CK(cudaFuncSetAttribute(k_main<SV_KIND_ECDSA33>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    CK(cudaFuncSetAttribute(k_main<SV_KIND_ECDSA_XY>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    CK(cudaFuncSetAttribute(k_main<SV_KIND_SCHNORR>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-#endif
     CK(cudaStreamSynchronize(ctx->stream));
     return SV_OK;
 }
@@ -1745,21 +1644,21 @@ static int launch_verify(sv_ctx* ctx, int kind, const u8* d_msg, const u8* d_key
     const unsigned grid = main_grid_for(ctx, n);
     if (kind == SV_KIND_ECDSA33 && ctx->nosqrt) {
         // compressed keys: the flow that skips the square root (verify.cuh "without the square root")
-        k_main<SV_KIND_ECDSA33_NS><<<grid, SV_MAIN_BLOCK, SV_MAIN_SMEM, st>>>(work, d_key, d_sig, n, ctx->d_gtab, sl->d_scratch, d_verdict, nullptr);
+        k_main<SV_KIND_ECDSA33_NS><<<grid, SV_MAIN_BLOCK, 0, st>>>(work, d_key, d_sig, n, ctx->d_gtab, sl->d_scratch, d_verdict, nullptr);
         size_t threads = (n + SV_FINAL_BATCH - 1) / SV_FINAL_BATCH;
         k_final_ecdsa33<<<(unsigned)((threads + 63) / 64), 64, 0, st>>>(work, d_key, d_sig, n, ctx->d_gtab, d_verdict, d_keyok);
         ctx->launches += 1;
     } else if (kind == SV_KIND_ECDSA33)
-        k_main<SV_KIND_ECDSA33><<<grid, SV_MAIN_BLOCK, SV_MAIN_SMEM, st>>>(work, d_key, d_sig, n, ctx->d_gtab, sl->d_scratch, d_verdict, d_keyok);
+        k_main<SV_KIND_ECDSA33><<<grid, SV_MAIN_BLOCK, 0, st>>>(work, d_key, d_sig, n, ctx->d_gtab, sl->d_scratch, d_verdict, d_keyok);
     else if (kind == SV_KIND_ECDSA_XY)
-        k_main<SV_KIND_ECDSA_XY><<<grid, SV_MAIN_BLOCK, SV_MAIN_SMEM, st>>>(work, d_key, d_sig, n, ctx->d_gtab, sl->d_scratch, d_verdict, d_keyok);
+        k_main<SV_KIND_ECDSA_XY><<<grid, SV_MAIN_BLOCK, 0, st>>>(work, d_key, d_sig, n, ctx->d_gtab, sl->d_scratch, d_verdict, d_keyok);
     else if (ctx->nosqrt) {
-        k_main<SV_KIND_SCHNORR_NS><<<grid, SV_MAIN_BLOCK, SV_MAIN_SMEM, st>>>(work, d_key, d_sig, n, ctx->d_gtab, sl->d_scratch, d_verdict, nullptr);
+        k_main<SV_KIND_SCHNORR_NS><<<grid, SV_MAIN_BLOCK, 0, st>>>(work, d_key, d_sig, n, ctx->d_gtab, sl->d_scratch, d_verdict, nullptr);
         size_t threads = (n + SV_FINAL_BATCH - 1) / SV_FINAL_BATCH;
         k_final_schnorr_ns<<<(unsigned)((threads + 63) / 64), 64, 0, st>>>(work, d_key, d_sig, n, ctx->d_gtab, d_verdict);
         ctx->launches += 1;
     } else {
-        k_main<SV_KIND_SCHNORR><<<grid, SV_MAIN_BLOCK, SV_MAIN_SMEM, st>>>(work, d_key, d_sig, n, ctx->d_gtab, sl->d_scratch, d_verdict, d_keyok);
+        k_main<SV_KIND_SCHNORR><<<grid, SV_MAIN_BLOCK, 0, st>>>(work, d_key, d_sig, n, ctx->d_gtab, sl->d_scratch, d_verdict, d_keyok);
         size_t threads = (n + SV_FINAL_BATCH - 1) / SV_FINAL_BATCH;
         k_final_schnorr<<<(unsigned)((threads + 63) / 64), 64, 0, st>>>(work, d_sig, n, d_verdict);
         ctx->launches += 1;
@@ -2718,9 +2617,6 @@ extern "C" int sv_grind_tx_fee_host(sv_ctx* ctx, int kind, const sv_tx* tx, cons
     if (weight >> 32) return fail(ctx, SV_ERR_ARG, "sv_grind_tx_fee_host: weight >= 2^32", cudaSuccess);
     if ((size_t)tx->script_off + tx->script_len > scripts_len || (size_t)tx->out_script_off + tx->out_script_len > scripts_len)
         return fail(ctx, SV_ERR_ARG, "script span out of range", cudaSuccess);
-#ifdef SV_COMB_SMEM
-    return fail(ctx, SV_ERR_ARG, "sv_grind_tx_fee_host: not available in the SV_COMB_SMEM build variant", cudaSuccess);
-#endif
     *feerate_out = -1;
     *fee_out = 0;
     if (min_feerate > max_feerate) return SV_OK;

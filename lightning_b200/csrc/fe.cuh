@@ -71,23 +71,11 @@ SV_HD void fe_add(fe& r, const fe& a, const fe& b) {
     u32 c = u256_add(r.v, a.v, b.v);
 #if SV_DEVICE_CODE
     u32 k;
-#ifdef SV_ALU_FOLDS
-    // c is 0 or 1: c * 977 as a select, so the fold stays off the multiplier pipe (the curve kernel's bottleneck)
-    asm("{\n\t.reg .pred p;\n\t.reg .u32 kc;\n\t"
-        "setp.ne.u32 p, %3, 0;\n\t"
-        "selp.u32 kc, 977, 0, p;\n\t"
-        "add.cc.u32 %0, %0, kc;\n\t"
-        "addc.cc.u32 %1, %1, %3;\n\t"
-        "addc.u32 %2, 0, 0;\n\t}"
-        : "+r"(r.v[0]), "+r"(r.v[1]), "=r"(k)
-        : "r"(c));
-#else
     asm("mad.lo.cc.u32 %0, %3, 977, %0;\n\t"
         "addc.cc.u32 %1, %1, %3;\n\t"
         "addc.u32 %2, 0, 0;"
         : "+r"(r.v[0]), "+r"(r.v[1]), "=r"(k)
         : "r"(c));
-#endif
     if (k) {
         u32 c2;
         asm("add.cc.u32 %0, %0, 1;\n\t"
@@ -124,23 +112,12 @@ SV_HD void fe_sub(fe& r, const fe& a, const fe& b) {
     // carry in fe_add and handled the same way.
 #if SV_DEVICE_CODE
     u32 k;
-#ifdef SV_ALU_FOLDS
-    asm("{\n\t.reg .pred p;\n\t.reg .u32 kc;\n\t"
-        "setp.ne.u32 p, %3, 0;\n\t"
-        "selp.u32 kc, 977, 0, p;\n\t"
-        "sub.cc.u32 %0, %0, kc;\n\t"
-        "subc.cc.u32 %1, %1, %3;\n\t"
-        "subc.u32 %2, 0, 0;\n\t}"
-        : "+r"(r.v[0]), "+r"(r.v[1]), "=r"(k)
-        : "r"(bw));
-#else
     u32 kc = bw * SV_PC;
     asm("sub.cc.u32 %0, %0, %4;\n\t"
         "subc.cc.u32 %1, %1, %3;\n\t"
         "subc.u32 %2, 0, 0;"
         : "+r"(r.v[0]), "+r"(r.v[1]), "=r"(k)
         : "r"(bw), "r"(kc));
-#endif
     if (k) {
         u32 b2;
         asm("sub.cc.u32 %0, %0, 1;\n\t"
@@ -182,117 +159,8 @@ SV_HD void fe_neg(fe& r, const fe& a) {  // reference: secp256k1_fe_negate (fiel
 SV_HD void fe_dbl(fe& r, const fe& a) { fe_add(r, a, a); }
 
 // reduce a 512-bit value t (16 limbs) mod p into weak form
-//
-// Two device variants of the first fold  lo + hi * (2^32 + 977):
-//   default           8 x IMAD.WIDE.U32 for hi * 977 (32 multiplier-pipe cycles per reduction)
-//   SV_REDUCE_SHIFTS  hi * 977 with shifts and adds only (977 = 17 + 15 * 64): no multiplier-pipe work but ~40 more
-//                     ALU instructions in long carry chains.  Measured slower: with 4 warps per sub-partition the dependent IADD3.X chains cost more
-//                     issue latency than the 8 multiplies they replace.  Kept as a tested alternative.
 SV_HD void fe_reduce512(fe& r, const u32 t[16]) {
-#if SV_DEVICE_CODE && defined(SV_REDUCE_SHIFTS)
-    u32 s[10];
-    // s = lo + (hi << 32)
-    s[0] = t[0];
-    asm("add.cc.u32 %0, %9, %17;\n\t"
-        "addc.cc.u32 %1, %10, %18;\n\t"
-        "addc.cc.u32 %2, %11, %19;\n\t"
-        "addc.cc.u32 %3, %12, %20;\n\t"
-        "addc.cc.u32 %4, %13, %21;\n\t"
-        "addc.cc.u32 %5, %14, %22;\n\t"
-        "addc.cc.u32 %6, %15, %23;\n\t"
-        "addc.cc.u32 %7, %16, 0;\n\t"
-        "addc.u32 %8, 0, 0;"
-        : "=r"(s[1]), "=r"(s[2]), "=r"(s[3]), "=r"(s[4]), "=r"(s[5]), "=r"(s[6]), "=r"(s[7]), "=r"(s[8]), "=r"(s[9])
-        : "r"(t[8]), "r"(t[9]), "r"(t[10]), "r"(t[11]), "r"(t[12]), "r"(t[13]), "r"(t[14]), "r"(t[15]),
-          "r"(t[1]), "r"(t[2]), "r"(t[3]), "r"(t[4]), "r"(t[5]), "r"(t[6]), "r"(t[7]));
-    // h4 = hi << 4 (9 limbs)
-    u32 h4[9];
-    h4[0] = t[8] << 4;
-    SV_UNROLL
-    for (int k = 1; k < 8; k++) h4[k] = __funnelshift_l(t[8 + k - 1], t[8 + k], 4);
-    h4[8] = t[15] >> 28;
-    // a17 = hi + h4 = 17*hi ; a15 = h4 - hi = 15*hi   (9 limbs each)
-    u32 a17[9], a15[9];
-    asm("add.cc.u32 %0, %9, %18;\n\t"
-        "addc.cc.u32 %1, %10, %19;\n\t"
-        "addc.cc.u32 %2, %11, %20;\n\t"
-        "addc.cc.u32 %3, %12, %21;\n\t"
-        "addc.cc.u32 %4, %13, %22;\n\t"
-        "addc.cc.u32 %5, %14, %23;\n\t"
-        "addc.cc.u32 %6, %15, %24;\n\t"
-        "addc.cc.u32 %7, %16, %25;\n\t"
-        "addc.u32 %8, %17, 0;"
-        : "=r"(a17[0]), "=r"(a17[1]), "=r"(a17[2]), "=r"(a17[3]), "=r"(a17[4]), "=r"(a17[5]), "=r"(a17[6]), "=r"(a17[7]), "=r"(a17[8])
-        : "r"(h4[0]), "r"(h4[1]), "r"(h4[2]), "r"(h4[3]), "r"(h4[4]), "r"(h4[5]), "r"(h4[6]), "r"(h4[7]), "r"(h4[8]),
-          "r"(t[8]), "r"(t[9]), "r"(t[10]), "r"(t[11]), "r"(t[12]), "r"(t[13]), "r"(t[14]), "r"(t[15]));
-    asm("sub.cc.u32 %0, %9, %18;\n\t"
-        "subc.cc.u32 %1, %10, %19;\n\t"
-        "subc.cc.u32 %2, %11, %20;\n\t"
-        "subc.cc.u32 %3, %12, %21;\n\t"
-        "subc.cc.u32 %4, %13, %22;\n\t"
-        "subc.cc.u32 %5, %14, %23;\n\t"
-        "subc.cc.u32 %6, %15, %24;\n\t"
-        "subc.cc.u32 %7, %16, %25;\n\t"
-        "subc.u32 %8, %17, 0;"
-        : "=r"(a15[0]), "=r"(a15[1]), "=r"(a15[2]), "=r"(a15[3]), "=r"(a15[4]), "=r"(a15[5]), "=r"(a15[6]), "=r"(a15[7]), "=r"(a15[8])
-        : "r"(h4[0]), "r"(h4[1]), "r"(h4[2]), "r"(h4[3]), "r"(h4[4]), "r"(h4[5]), "r"(h4[6]), "r"(h4[7]), "r"(h4[8]),
-          "r"(t[8]), "r"(t[9]), "r"(t[10]), "r"(t[11]), "r"(t[12]), "r"(t[13]), "r"(t[14]), "r"(t[15]));
-    // b = a15 << 6 = 960*hi  (a15 < 2^260 -> b < 2^266: 9 limbs)
-    u32 b[9];
-    b[0] = a15[0] << 6;
-    SV_UNROLL
-    for (int k = 1; k < 9; k++) b[k] = __funnelshift_l(a15[k - 1], a15[k], 6);
-    // s += a17 ; s += b   (s < 2^289: limb 9 stays tiny)
-    asm("add.cc.u32 %0, %0, %10;\n\t"
-        "addc.cc.u32 %1, %1, %11;\n\t"
-        "addc.cc.u32 %2, %2, %12;\n\t"
-        "addc.cc.u32 %3, %3, %13;\n\t"
-        "addc.cc.u32 %4, %4, %14;\n\t"
-        "addc.cc.u32 %5, %5, %15;\n\t"
-        "addc.cc.u32 %6, %6, %16;\n\t"
-        "addc.cc.u32 %7, %7, %17;\n\t"
-        "addc.cc.u32 %8, %8, %18;\n\t"
-        "addc.u32 %9, %9, 0;"
-        : "+r"(s[0]), "+r"(s[1]), "+r"(s[2]), "+r"(s[3]), "+r"(s[4]), "+r"(s[5]), "+r"(s[6]), "+r"(s[7]), "+r"(s[8]), "+r"(s[9])
-        : "r"(a17[0]), "r"(a17[1]), "r"(a17[2]), "r"(a17[3]), "r"(a17[4]), "r"(a17[5]), "r"(a17[6]), "r"(a17[7]), "r"(a17[8]));
-    asm("add.cc.u32 %0, %0, %10;\n\t"
-        "addc.cc.u32 %1, %1, %11;\n\t"
-        "addc.cc.u32 %2, %2, %12;\n\t"
-        "addc.cc.u32 %3, %3, %13;\n\t"
-        "addc.cc.u32 %4, %4, %14;\n\t"
-        "addc.cc.u32 %5, %5, %15;\n\t"
-        "addc.cc.u32 %6, %6, %16;\n\t"
-        "addc.cc.u32 %7, %7, %17;\n\t"
-        "addc.cc.u32 %8, %8, %18;\n\t"
-        "addc.u32 %9, %9, 0;"
-        : "+r"(s[0]), "+r"(s[1]), "+r"(s[2]), "+r"(s[3]), "+r"(s[4]), "+r"(s[5]), "+r"(s[6]), "+r"(s[7]), "+r"(s[8]), "+r"(s[9])
-        : "r"(b[0]), "r"(b[1]), "r"(b[2]), "r"(b[3]), "r"(b[4]), "r"(b[5]), "r"(b[6]), "r"(b[7]), "r"(b[8]));
-    // second fold: T = s[8] + s[9]*2^32 (< 2^35);  T*(2^32+977) < 2^68 -> three limbs f0,f1,f2
-    u64 T = ((u64)s[9] << 32) | s[8];
-    u64 m = T * SV_PC;
-    u64 mid = (m >> 32) + T;
-    u32 f0 = (u32)m, f1 = (u32)mid, f2 = (u32)(mid >> 32);
-    u32 c;
-    asm("add.cc.u32 %0, %9, %17;\n\t"
-        "addc.cc.u32 %1, %10, %18;\n\t"
-        "addc.cc.u32 %2, %11, %19;\n\t"
-        "addc.cc.u32 %3, %12, 0;\n\t"
-        "addc.cc.u32 %4, %13, 0;\n\t"
-        "addc.cc.u32 %5, %14, 0;\n\t"
-        "addc.cc.u32 %6, %15, 0;\n\t"
-        "addc.cc.u32 %7, %16, 0;\n\t"
-        "addc.u32 %8, 0, 0;"
-        : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]), "=r"(r.v[5]), "=r"(r.v[6]),
-          "=r"(r.v[7]), "=r"(c)
-        : "r"(s[0]), "r"(s[1]), "r"(s[2]), "r"(s[3]), "r"(s[4]), "r"(s[5]), "r"(s[6]), "r"(s[7]), "r"(f0), "r"(f1),
-          "r"(f2));
-    // third fold (rare): wrapped value is < 2^68, adding 2^32+977 cannot wrap again
-    asm("mad.lo.cc.u32 %0, %3, 977, %0;\n\t"
-        "addc.cc.u32 %1, %1, %3;\n\t"
-        "addc.u32 %2, %2, 0;"
-        : "+r"(r.v[0]), "+r"(r.v[1]), "+r"(r.v[2])
-        : "r"(c));
-#elif SV_DEVICE_CODE
+#if SV_DEVICE_CODE
     // s[0..8] = lo + (hi << 32)
     u32 s[10];
     s[0] = t[0];

@@ -345,32 +345,3 @@ SV_HD void sc_prepare_u1(sv_work& w, const sc& u1) {
         }
     }
 }
-
-#ifdef SV_COMB_SMEM
-// VARIANT (kept for the record): u1 = a + b*lambda with |a|, |b| < 2^128, both recoded into 17
-// signed 8-bit digits for the 131 KB shared-memory comb.  gd[k] = digit_a[k] (low 16 bits) | digit_b[k] << 16 for k < 16;
-// pad[0] = top digit of a | top digit of b << 8 | sign a << 16 | sign b << 17.
-SV_HD void sc_recode8(int dig[17], const u32 mag[5]) {
-    u32 carry = 0;
-    for (int i = 0; i < 17; i++) {
-        u32 w = (i < 16) ? ((mag[i >> 2] >> ((i & 3) * 8)) & 0xFFu) : (mag[4] & 0xFFu);
-        w += carry;
-        if (w > 128u) { dig[i] = (int)w - 256; carry = 1; } else { dig[i] = (int)w; carry = 0; }
-    }
-}
-SV_HD void sc_prepare_u1_smem(sv_work& w, const sc& u1) {
-    sc r1, r2, t;
-    sc_split_lambda(r1, r2, u1);
-    u32 m1[5], m2[5];
-    u32 n1 = sc_is_high(r1) ? 1u : 0u, n2 = sc_is_high(r2) ? 1u : 0u;
-    if (n1) sc_negate(t, r1); else t = r1;
-    for (int k = 0; k < 5; k++) m1[k] = t.v[k];
-    if (n2) sc_negate(t, r2); else t = r2;
-    for (int k = 0; k < 5; k++) m2[k] = t.v[k];
-    int da[17], db[17];
-    sc_recode8(da, m1);
-    sc_recode8(db, m2);
-    for (int k = 0; k < 16; k++) w.gd[k] = (int)(((u32)da[k] & 0xFFFFu) | ((u32)db[k] << 16));
-    w.pad[0] = ((u32)da[16] & 0xFFu) | (((u32)db[16] & 0xFFu) << 8) | (n1 << 16) | (n2 << 17);
-}
-#endif

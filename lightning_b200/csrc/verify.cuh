@@ -135,11 +135,7 @@ SV_HD void ecdsa_finish_prep(sv_work& w, bool ok, const sc& r, const sc& m, cons
     SV_UNROLL
     for (int i = 0; i < 5; i++) w.pad[i] = 0;
     sc_prepare_u2(w, u2);
-#ifdef SV_COMB_SMEM
-    sc_prepare_u1_smem(w, u1);
-#else
     sc_prepare_u1(w, u1);
-#endif
     w.flags = SV_WF_VALID | SV_WF_PARSED | ecdsa_r_plus_n_flag(r);
 }
 
@@ -163,11 +159,7 @@ SV_HD void schnorr_prep(sv_work& w, const u8* sig64, const u8* xonly32, const u8
     SV_UNROLL
     for (int i = 0; i < 5; i++) w.pad[i] = 0;
     sc_prepare_u2(w, ne);
-#ifdef SV_COMB_SMEM
-    sc_prepare_u1_smem(w, s);
-#else
     sc_prepare_u1(w, s);
-#endif
     w.flags = SV_WF_VALID;
 }
 
@@ -320,19 +312,8 @@ SV_HD void ecmult_ladder_q(gej& R, const sv_work* w, const qtab_entry* tab, cons
 #pragma unroll 1
 #endif
     for (int i = 31; i >= 0; i--) {
-#if SV_DEVICE_CODE
-#pragma unroll 1
-#endif
-#if defined(SV_SYNC_LEVEL) && SV_SYNC_LEVEL < 2
-#ifndef SV_SYNC_WINDOWS
-#define SV_SYNC_WINDOWS 1
-#endif
-        if (i % SV_SYNC_WINDOWS == 0) SV_SYNC(sync_threads);  // one re-convergence point per SV_SYNC_WINDOWS windows
-#endif
+        if (i % 2 == 0) SV_SYNC(sync_threads);  // one re-convergence point every second window
         for (int j = 0; j < 4; j++) {
-#if !defined(SV_SYNC_LEVEL) || SV_SYNC_LEVEL >= 2
-            SV_SYNC(sync_threads);
-#endif
             gej_double(R, R);
         }
 #if SV_DEVICE_CODE
@@ -340,9 +321,6 @@ SV_HD void ecmult_ladder_q(gej& R, const sv_work* w, const qtab_entry* tab, cons
 #endif
         for (int half = 0; half < 2; half++) {
             u32 v = half ? window4(m2, i) : window4(m1, i);
-#if !defined(SV_SYNC_LEVEL) || SV_SYNC_LEVEL >= 2
-            SV_SYNC(sync_threads);
-#endif
             qtable_fetch(p, tab, v, half ? s2 : s1, half != 0);
             gej_add_ge(R, R, p);
         }
@@ -354,36 +332,6 @@ SV_HD void ecmult_ladder_q(gej& R, const sv_work* w, const qtab_entry* tab, cons
 // R += u1*G through the fixed-base comb (16 mixed additions against the 34 MiB table)
 SV_HD void ecmult_comb_add(gej& R, const sv_work* w, const ge_mem* gtab, unsigned sync_threads = 0) {
     ge p;
-#if defined(SV_COMB_SMEM) && SV_DEVICE_CODE
-    // VARIANT: 8-bit GLV comb against the 131 KB table staged in shared memory (k_main copies it in with one bulk copy):
-    // 2 x 17 windows -> up to 34 mixed additions and a beta multiplication for each lambda-half point
-    {
-        extern __shared__ __align__(16) unsigned char sv_smem_raw[];
-        const ge_mem* t8 = reinterpret_cast<const ge_mem*>(sv_smem_raw);
-        fe beta;
-        SV_UNROLL
-        for (int i = 0; i < 8; i++) beta.v[i] = GE_BETA[i];
-        const u32 top = w->pad[0];
-#pragma unroll 1
-        for (int row = 0; row < 17; row++) {
-            SV_SYNC(sync_threads);
-#pragma unroll 1
-            for (int half = 0; half < 2; half++) {
-                int d;
-                if (row < 16) d = half ? (int)(short)((u32)w->gd[row] >> 16) : (int)(short)((u32)w->gd[row] & 0xFFFFu);
-                else d = (int)(signed char)((top >> (8 * half)) & 0xFFu);
-                u32 sneg = (top >> (16 + half)) & 1u;
-                if (d != 0) {
-                    u32 a = (u32)(d < 0 ? -d : d);
-                    ge_from_mem(p, t8 + (size_t)row * 128 + (a - 1));
-                    if (half) fe_mul(p.x, p.x, beta);
-                    if ((d < 0) != (sneg != 0)) fe_neg(p.y, p.y);
-                    gej_add_ge(R, R, p);
-                }
-            }
-        }
-    }
-#else
 #if SV_DEVICE_CODE
 #pragma unroll 1
 #endif
@@ -397,7 +345,6 @@ SV_HD void ecmult_comb_add(gej& R, const sv_work* w, const ge_mem* gtab, unsigne
             gej_add_ge(R, R, p);
         }
     }
-#endif
 }
 
 // R = u1*G + u2*Q in true Jacobian coordinates

@@ -11,7 +11,7 @@ import os
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("SV_LIB") or os.path.join(_HERE, "libcln_sigverify.so")  # SV_LIB: build variants (dev)
+LIB_PATH = os.environ.get("SV_LIB") or os.path.join(_HERE, "libcln_sigverify.so")  # SV_LIB: another build of the library (dev)
 
 KIND_ECDSA33 = 0
 KIND_ECDSA_XY = 1
