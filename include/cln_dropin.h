@@ -33,6 +33,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include "cln_sigverify.h" /* sv_gossip_prune_summary */
+
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -130,6 +132,8 @@ void cln_sigverify_shutdown(void);
  *   sigcheck_gossip_batch                                                               (sigverifyd_gossip_burst)
  *   sha256_double                                                                       (sigverifyd_sha256d)
  *   pubkey_from_der                                                                     (sigverifyd_pubkey)
+ *   gossip_store_prune                                                                  (sigverifyd_gossip_store_prune:
+ *                                                                                        the fd travels, not the store)
  * check_tx_sig gates the sighash type before it sends anything; the BIP143 sighash is built on the daemon's device.
  * check_tx_sigs_bip143_batch sends requests of at most 65536 transactions and 64 MiB of scripts each.  pubkey_from_der
  * returns false for a length other than 33 without sending anything.  The daemon serves the requests of all its clients
@@ -262,6 +266,17 @@ void sigcheck_channel_update_batch(const u8 *const *msgs, const size_t *lens, co
  * aborts. */
 void sigcheck_gossip_batch(const u8 *chain_hash32, const u8 *const *msgs, const size_t *lens, size_t n, const u8 *signer_kind,
                            const struct node_id *signers, int *status);
+
+/* gossipd's last resort before gossip_store_corrupt(): after a failed strict load, prune the store in place
+ * (sv_prune_gossip_store_fd in cln_sigverify.h: every record gossmap should not trust gets its deleted flag, nothing else
+ * changes) and load it again.  fd is the store opened O_RDWR, len its size (st_size), chain_hash32 the chain's genesis
+ * hash (NULL: no chain gate).  true: pruned and synced, *summary (may be NULL) says what was deleted and why.  false with
+ * errno: fd not open (EBADF), not open for writing (EBADF), not a regular file, len 0 or past its end, or a store the
+ * engine refuses (EINVAL), a store above the daemon's 4 GiB limit (EFBIG, client mode), or the errno of a failed read,
+ * write or fsync.  In client mode the descriptor goes to cln_sigverifyd (SCM_RIGHTS) and the daemon's engine reads and
+ * writes the file; the call waits for the reply as every blocking call does.  A lost daemon and engine failures abort(),
+ * as for every function of this header. */
+bool gossip_store_prune(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_prune_summary *summary);
 
 #ifdef __cplusplus
 }

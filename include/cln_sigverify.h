@@ -74,7 +74,8 @@ typedef enum {
     SV_ERR_NO_DEVICE = -1,
     SV_ERR_CUDA = -2,
     SV_ERR_NOMEM = -3,
-    SV_ERR_ARG = -4
+    SV_ERR_ARG = -4,
+    SV_ERR_IO = -5 /* sv_prune_gossip_store_fd: the file could not be read, written or synced; errno is kept */
 } sv_status;
 
 /* Create an engine on CUDA device `device` (ordinal).  Allocates the stream, builds the 34 MiB
@@ -278,6 +279,19 @@ int sv_prune_gossip_store_host(sv_ctx *ctx, const uint8_t *store, size_t len, co
 /* profiling mode: ms4 = host header walk, first round (H2D of the store, checksums, the audit's kernels), second round
  * (mark, resolution, compaction, re-verification), flag write and copy back */
 int sv_get_last_gossip_prune_timing(sv_ctx *ctx, float *ms4);
+
+/* ---- PRUNE a gossip_store FILE in place: the store is bytes [0, len) of fd, which must be a regular file opened for
+ *      reading and writing.  The store is read (pread) into host memory and pruned by sv_prune_gossip_store_host with out
+ *      == store; then, for each record it deleted, the two-byte big-endian flags field (the first two bytes of the
+ *      record's 12-byte header) is written back (pwrite) with bit 0x8000 set, as gossip_store_del does, and the file is
+ *      synced (fsync).  No other byte of the file changes, so every checksum stays valid.  *summary is the host call's.
+ *      fd not a regular file, len 0 or larger than the file: SV_ERR_ARG, nothing read, errno EINVAL.  A store the host
+ *      call refuses (a major version other than 0): SV_ERR_ARG, errno EINVAL, nothing written.  fd not open for reading
+ *      and writing: SV_ERR_IO, errno EBADF, nothing read.  A failed or short read, a failed write or fsync: SV_ERR_IO with
+ *      that errno (EIO for a short read); the flags written before a failed write stay (each is a deletion of its own).
+ *      The other engine errors (SV_ERR_NOMEM, SV_ERR_CUDA, ...) are returned as the host call returns them.  The verifier
+ *      subdaemon serves this call for its clients (sigverifyd_gossip_store_prune: the fd travels over its socket). ---- */
+int sv_prune_gossip_store_fd(sv_ctx *ctx, int fd, uint64_t len, const uint8_t *chain_hash32, sv_gossip_prune_summary *summary);
 
 /* L2 residency hint for the throughput kernels (default on): the G comb table and the per-thread multiples tables are
  * marked persisting through a stream access-policy window, the rest of the stream's traffic streaming.  0 switches it off

@@ -1,7 +1,7 @@
 """Build recipes for the engine (nvcc, sm_90a only: H100) and for the test-side artefacts.
 
 Everything is built IN-TREE, so the package and the tests run from the source tree:
-  lightning_b200/libcln_sigverify.so   the product (CUDA kernels + C ABI)            [nvcc]
+  lightning_b200/libcln_sigverify.so   the product (CUDA kernels + C ABI; its plain-C parts by gcc) [nvcc]
   tests/host_emul/libemul.so           kernel headers compiled for the host, tests only [g++]
   oracle/libsecp_port.so               the plain-C restatement oracle                 [gcc]
   oracle/_ref/libsecp_ref.so           the unmodified reference, from the Core Lightning tree at $CLN_SRC or /root/reference [gcc]
@@ -61,6 +61,12 @@ def build_engine(force=False, verbose=False):
     r = subprocess.run(["gcc"] + DROPIN_CFLAGS + ["-c", os.path.join(CSRC, "cln_dropin.c"), "-o", dropin_o], capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("gcc (cln_dropin.c) failed:\n" + r.stdout + r.stderr)
+    # pruning a gossip_store file in place (sv_prune_gossip_store_fd): plain C over the engine's prune entry points
+    store_fd_o = os.path.join(CSRC, "gossip_store_fd.o")
+    r = subprocess.run(["gcc"] + DROPIN_CFLAGS + ["-c", os.path.join(CSRC, "gossip_store_fd.c"), "-o", store_fd_o],
+                       capture_output=True, text=True)
+    if r.returncode != 0:
+        raise RuntimeError("gcc (gossip_store_fd.c) failed:\n" + r.stdout + r.stderr)
     # the batch-verification kernels are a translation unit of their own, compiled with the field multiplier as real
     # functions (see batch.cu); everything else inlines it
     batch_flags = [f for f in NVCC_FLAGS if f not in ("-shared", "-DSV_FE_INLINE", "-DSV_MAIN_SYNC")] + ["-DSV_NO_SYNC_INLINE", "-c"]
@@ -72,7 +78,7 @@ def build_engine(force=False, verbose=False):
     if r.returncode != 0:
         raise RuntimeError("nvcc (batch.cu) failed:\n" + r.stdout + r.stderr)
     cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + [
-        "-o", LIB, os.path.join(CSRC, "engine.cu"), batch_o, dropin_o]
+        "-o", LIB, os.path.join(CSRC, "engine.cu"), batch_o, dropin_o, store_fd_o]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if verbose:
         sys.stderr.write(r.stderr)

@@ -17,8 +17,11 @@
 /* weak: the library's client mode is also linked against engine builds without the fee grind (the fake engine of the
  * client-mode CPU tests); check_tx_sig_grind_fee then works through the daemon only */
 #pragma weak sv_grind_tx_fee_host
+/* likewise for the in-place prune: gossip_store_prune then works through the daemon only */
+#pragma weak sv_prune_gossip_store_fd
 
 #include <errno.h>
+#include <fcntl.h>
 #include <poll.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -51,6 +54,7 @@ struct req {
     uint64_t id;              /* req_id; a ticket's number too */
     u8 *frame;                /* be32 length + message: owned by a ticket, borrowed from a blocking call */
     size_t len, sent;
+    int pass_fd;              /* a descriptor that goes with the frame's first byte (SCM_RIGHTS), else -1 */
     bool ticket, replied;
     uint16_t type;            /* a ticket's request type, its item count and where its answer goes */
     uint32_t n;
@@ -153,7 +157,22 @@ static void reply_arrived(const u8 *r, size_t rl) {
 static void send_some(void) {
     while (g_s < g_t) {
         struct req *q = &g_q[g_s];
-        ssize_t w = send(g_sock, q->frame + q->sent, q->len - q->sent, MSG_NOSIGNAL | MSG_DONTWAIT);
+        ssize_t w;
+        if (q->pass_fd >= 0) { /* its own sendmsg, which starts at the frame's first byte */
+            union { struct cmsghdr h; char b[CMSG_SPACE(sizeof(int))]; } ctl;
+            memset(&ctl, 0, sizeof ctl);
+            struct iovec iov = {q->frame, q->len};
+            struct msghdr mh = {.msg_iov = &iov, .msg_iovlen = 1, .msg_control = ctl.b, .msg_controllen = sizeof ctl.b};
+            struct cmsghdr *cm = CMSG_FIRSTHDR(&mh);
+            cm->cmsg_level = SOL_SOCKET;
+            cm->cmsg_type = SCM_RIGHTS;
+            cm->cmsg_len = CMSG_LEN(sizeof(int));
+            memcpy(CMSG_DATA(cm), &q->pass_fd, sizeof(int));
+            w = sendmsg(g_sock, &mh, MSG_NOSIGNAL | MSG_DONTWAIT);
+            if (w > 0) q->pass_fd = -1; /* the daemon has its own copy of the descriptor now */
+        } else {
+            w = send(g_sock, q->frame + q->sent, q->len - q->sent, MSG_NOSIGNAL | MSG_DONTWAIT);
+        }
         if (w < 0 && errno == EINTR) continue;
         if (w < 0 && (errno == EAGAIN || errno == EWOULDBLOCK)) return;
         if (w <= 0) die_daemon("write failed");
@@ -226,6 +245,7 @@ static size_t push_req(uint64_t id, u8 *frame, size_t len, bool ticket) {
     q->frame = frame;
     q->len = len;
     q->ticket = ticket;
+    q->pass_fd = -1;
     g_unsent += len;
     return g_t++;
 }
@@ -1105,4 +1125,62 @@ static void ticket_reply(const struct req *q, const u8 *r, size_t rl) {
     case WIRE_SIGVERIFYD_BOLT12: *q->ok = bolt12_reply(r, rl) == 1; break;
     case WIRE_SIGVERIFYD_GOSSIP_BURST: burst_reply(r, rl, q->n, q->status); break;
     }
+}
+
+/* ---- gossip_store_prune: gossipd's store pruned in place (sv_prune_gossip_store_fd); in client mode the file's
+ * descriptor goes to the daemon with the request, never its bytes ---- */
+static bool remote_prune(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_prune_summary *summary) {
+    static const u8 zero[32];
+    size_t mlen = 2 + 8 + 1 + 32 + 8, rl;
+    u8 f[4 + 2 + 8 + 1 + 32 + 8];
+    uint64_t id = ++g_req_id;
+    towire_sigverifyd_gossip_store_prune(f + 4, mlen, id, chain_hash32 != NULL, chain_hash32 ? chain_hash32 : zero, len);
+    /* every request before it is written out first (send_some writes in order), so the fd rides on this frame's first
+     * byte: the daemon matches it to this request */
+    while (g_unsent) io_wait();
+    wire_put(f, mlen, 4);
+    size_t at = push_req(id, f, 4 + mlen, false);
+    g_q[at].pass_fd = fd;
+    send_some();
+    while (!g_q[at].replied) io_wait();
+    u8 *r = g_q[at].reply;
+    rl = g_q[at].reply_len;
+    g_t = g_s = g_r = at;
+    struct sigverifyd_gossip_store_prune_reply p;
+    if (!fromwire_sigverifyd_gossip_store_prune_reply(r, rl, &p)) die_daemon("malformed gossip_store prune reply");
+    free(r);
+    if (p.err) {
+        errno = (int)p.err;
+        return false;
+    }
+    summary->version = p.version;
+    summary->stop = (int32_t)p.stop;
+    summary->end_offset = p.end_offset;
+    summary->records = p.records;
+    summary->pruned = p.pruned;
+    summary->bad_crc = p.bad_crc;
+    summary->truncated = p.truncated;
+    summary->message = p.message;
+    summary->redundant = p.redundant;
+    summary->no_channel = p.no_channel;
+    summary->signature = p.signature;
+    summary->amount = p.amount;
+    summary->unknown = p.unknown;
+    summary->reverified = p.reverified;
+    return true;
+}
+
+bool gossip_store_prune(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_prune_summary *summary) {
+    sv_gossip_prune_summary s;
+    if (fcntl(fd, F_GETFD) < 0) return false; /* errno EBADF: nothing to send */
+    if (client()) {
+        if (!remote_prune(fd, len, chain_hash32, &s)) return false;
+    } else {
+        if (!sv_prune_gossip_store_fd) die("gossip_store_prune: this engine has no sv_prune_gossip_store_fd", SV_ERR_ARG);
+        int rc = sv_prune_gossip_store_fd(ctx(), fd, len, chain_hash32, &s);
+        if (rc == SV_ERR_ARG || rc == SV_ERR_IO) return false; /* errno says why */
+        if (rc != SV_OK) die("sv_prune_gossip_store_fd", rc);
+    }
+    if (summary) *summary = s;
+    return true;
 }

@@ -6,6 +6,7 @@ bitcoin/shadouble.h: sha256_double), batched.  There is no Python or CPU impleme
 this class: if the CUDA library or a GPU is missing, construction raises.
 """
 import ctypes
+import errno
 import os
 
 import numpy as np
@@ -13,6 +14,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SV_LIB") or os.path.join(_HERE, "libcln_sigverify.so")  # SV_LIB: another build of the library (dev)
 
+SV_ERR_ARG, SV_ERR_IO = -4, -5  # sv_status values a caller of sv_prune_gossip_store_fd tells apart
 KIND_ECDSA33 = 0
 KIND_ECDSA_XY = 1
 KIND_SCHNORR = 2
@@ -73,7 +75,7 @@ def load_library():
         raise EngineError(
             f"{LIB_PATH} is missing: build it with `python -m lightning_b200.build` "
             "(nvcc, sm_90a). There is no CPU fallback.")
-    lib = ctypes.CDLL(LIB_PATH)
+    lib = ctypes.CDLL(LIB_PATH, use_errno=True)  # errno: sv_prune_gossip_store_fd says why a file was refused
     vp, sz, i = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int
     lib.sv_create.argtypes = [ctypes.POINTER(vp), i]
     lib.sv_destroy.argtypes = [vp]
@@ -97,6 +99,7 @@ def load_library():
     lib.sv_gossip_prune_count.restype = sz
     lib.sv_prune_gossip_store_host.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp, vp, sz, ctypes.POINTER(SvGossipPruneSummary)]
     lib.sv_get_last_gossip_prune_timing.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
+    lib.sv_prune_gossip_store_fd.argtypes = [vp, i, ctypes.c_uint64, vp, ctypes.POINTER(SvGossipPruneSummary)]
     lib.sv_verify_tx_host.argtypes = [vp, i, vp, vp, sz, vp, vp, sz, vp, vp]
     lib.sv_grind_tx_fee_host.argtypes = [vp, i, vp, vp, sz, vp, vp, ctypes.c_uint64, ctypes.c_uint32, ctypes.c_uint32,
                                          ctypes.POINTER(ctypes.c_int64), ctypes.POINTER(ctypes.c_uint64)]
@@ -319,6 +322,26 @@ class SigVerifier:
         summary = {f: getattr(s, f) for f, _ in SvGossipPruneSummary._fields_}
         k = s.records
         return out[:buf.size].tobytes(), (off[:k], typ[:k], status[:k], pruned[:k]), summary
+
+    def prune_gossip_store_fd(self, fd, length, chain_hash=None):
+        """prune_gossip_store on a FILE, in place (sv_prune_gossip_store_fd): the store is bytes [0, length) of fd, a
+        regular file open for reading and writing; the flags of the records deleted are written back into it and the file
+        is synced, no other byte changes.  Returns the summary dict prune_gossip_store returns.  A file the call cannot use
+        or a store it refuses raises OSError with the call's errno (EINVAL, EBADF, or that of a failed read, write or
+        fsync); an engine failure raises EngineError."""
+        chain = None
+        if chain_hash is not None:
+            chain = np.frombuffer(bytes(chain_hash), dtype=np.uint8)
+            if chain.size != 32:
+                raise ValueError("chain_hash must be 32 bytes")
+        s = SvGossipPruneSummary()
+        rc = self.lib.sv_prune_gossip_store_fd(self._ctx, int(fd), int(length), chain.ctypes.data if chain is not None else None,
+                                               ctypes.byref(s))
+        if rc in (SV_ERR_ARG, SV_ERR_IO):
+            e = ctypes.get_errno() or errno.EINVAL
+            raise OSError(e, f"sv_prune_gossip_store_fd: {os.strerror(e)}")
+        self._check(rc, "sv_prune_gossip_store_fd")
+        return {f: getattr(s, f) for f, _ in SvGossipPruneSummary._fields_}
 
     def last_gossip_prune_timing(self):
         """(header walk, first round, second round, flag write) in ms of the last prune_gossip_store (profiling mode)"""
