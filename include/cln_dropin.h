@@ -134,6 +134,8 @@ void cln_sigverify_shutdown(void);
  *   pubkey_from_der                                                                     (sigverifyd_pubkey)
  *   gossip_store_prune                                                                  (sigverifyd_gossip_store_prune:
  *                                                                                        the fd travels, not the store)
+ *   gossip_store_repair                                                                 (sigverifyd_gossip_store_repair:
+ *                                                                                        likewise)
  * check_tx_sig gates the sighash type before it sends anything; the BIP143 sighash is built on the daemon's device.
  * check_tx_sigs_bip143_batch sends requests of at most 65536 transactions and 64 MiB of scripts each.  pubkey_from_der
  * returns false for a length other than 33 without sending anything.  The daemon serves the requests of all its clients
@@ -277,6 +279,16 @@ void sigcheck_gossip_batch(const u8 *chain_hash32, const u8 *const *msgs, const 
  * writes the file; the call waits for the reply as every blocking call does.  A lost daemon and engine failures abort(),
  * as for every function of this header. */
 bool gossip_store_prune(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_prune_summary *summary);
+
+/* gossip_store_prune, then the store's torn tail cut off (sv_repair_gossip_store_fd in cln_sigverify.h): a last record
+ * without its COMPLETED bit, one running past the end of the file, a torn header, or a channel_announcement without its
+ * channel_amount record (and an announcement the cut would leave without room for its amount record, see
+ * sv_repair_gossip_store_fd), so the second strict load then accepts the store: gossipd calls it between a failed setup_gossmap and gossip_store_corrupt(), and loads again with expected_len =
+ * *new_len.  A store that ends cleanly or in a gossip_store_ended record is only pruned (*new_len = len).  true: *summary
+ * and *new_len (each may be NULL) say what was deleted and where the file ends now.  false with errno as for
+ * gossip_store_prune, or that of a failed ftruncate; the deletions already written stay.  Client mode as for
+ * gossip_store_prune. */
+bool gossip_store_repair(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_prune_summary *summary, uint64_t *new_len);
 
 #ifdef __cplusplus
 }

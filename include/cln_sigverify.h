@@ -293,6 +293,33 @@ int sv_get_last_gossip_prune_timing(sv_ctx *ctx, float *ms4);
  *      subdaemon serves this call for its clients (sigverifyd_gossip_store_prune: the fd travels over its socket). ---- */
 int sv_prune_gossip_store_fd(sv_ctx *ctx, int fd, uint64_t len, const uint8_t *chain_hash32, sv_gossip_prune_summary *summary);
 
+/* ---- REPAIR a gossip_store FILE in place: prune it (sv_prune_gossip_store_fd, everything it does and refuses), then cut
+ *      a torn tail off it.  gossipd only appends, so a crash during gossip_store_add leaves a last record without
+ *      GOSSIP_STORE_COMPLETED_BIT, a record running past the end of the file, fewer than 13 trailing bytes, or a
+ *      channel_announcement without its channel_amount record; gossmap's strict start-up load refuses each (its walk stops
+ *      short of expected_len, common/gossmap.c:1428-1438).  The cut, where the file ends afterwards, is
+ *      sv_gossip_prune_cut(summary, pruned store, len):
+ *        stop SV_GS_INCOMPLETE, SV_GS_PARTIAL or SV_GS_NO_AMOUNT:  summary.end_offset (the record the walk stopped at);
+ *        stop SV_GS_EOF with end_offset < len (a torn header):      end_offset;
+ *        anything else, SV_GS_ENDED included (a replaced store):    len, and the call is exactly the prune.
+ *      When the cut is below len and would leave a live channel_announcement without the 22 bytes of its channel_amount
+ *      record before it (gossmap.c:488-492), the store ends at that announcement instead (repeated while that leaves
+ *      another one so).  gossipd writes a record with flags 0 and sets COMPLETED in a second one-byte write
+ *      (gossipd/gossip_store.c:64-77), so a crash between the two during the amount's append leaves a whole amount record
+ *      without COMPLETED after a complete announcement: the walk stops INCOMPLETE at the amount, and the announcement must
+ *      go with it.  A strict load with expected_len = the cut accepts the repaired store, and it holds what a load of the
+ *      pruned store holds up to its walk's stop, minus such an announcement: a lenient load of the torn store reads the
+ *      incomplete amount record's bytes and keeps that channel, the repaired store does not (gossipd learns it again
+ *      from its peers).  Order of writes: the deleted flags, fsync, then (cut < len) ftruncate(fd, cut) and fsync again,
+ *      so a crash in between leaves a store whose pruned prefix is still valid; the bytes after len go too.  *new_len (may
+ *      be NULL) = the cut, written on SV_OK only.  A failed ftruncate or fsync: SV_ERR_IO with its errno, the flags
+ *      already written stay.  The verifier subdaemon serves this call for its clients (sigverifyd_gossip_store_repair).
+ *      sv_gossip_prune_cut is that rule alone, for a store pruned in host memory (pruned: the len bytes the prune wrote,
+ *      whose deleted flags it reads; NULL summary or pruned: len). ---- */
+int sv_repair_gossip_store_fd(sv_ctx *ctx, int fd, uint64_t len, const uint8_t *chain_hash32, sv_gossip_prune_summary *summary,
+                              uint64_t *new_len);
+uint64_t sv_gossip_prune_cut(const sv_gossip_prune_summary *summary, const uint8_t *pruned, uint64_t len);
+
 /* L2 residency hint for the throughput kernels (default on): the G comb table and the per-thread multiples tables are
  * marked persisting through a stream access-policy window, the rest of the stream's traffic streaming.  0 switches it off
  * for streams not yet seen (measurement aid). */

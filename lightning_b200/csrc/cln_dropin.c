@@ -19,6 +19,7 @@
 #pragma weak sv_grind_tx_fee_host
 /* likewise for the in-place prune: gossip_store_prune then works through the daemon only */
 #pragma weak sv_prune_gossip_store_fd
+#pragma weak sv_repair_gossip_store_fd
 
 #include <errno.h>
 #include <fcntl.h>
@@ -1127,14 +1128,18 @@ static void ticket_reply(const struct req *q, const u8 *r, size_t rl) {
     }
 }
 
-/* ---- gossip_store_prune: gossipd's store pruned in place (sv_prune_gossip_store_fd); in client mode the file's
- * descriptor goes to the daemon with the request, never its bytes ---- */
-static bool remote_prune(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_prune_summary *summary) {
+/* ---- gossip_store_prune / gossip_store_repair: gossipd's store pruned in place (sv_prune_gossip_store_fd), and its
+ * torn tail cut (sv_repair_gossip_store_fd); in client mode the file's descriptor goes to the daemon with the request,
+ * never its bytes ---- */
+static bool remote_prune(bool repair, int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_prune_summary *summary,
+                         uint64_t *new_len) {
     static const u8 zero[32];
     size_t mlen = 2 + 8 + 1 + 32 + 8, rl;
     u8 f[4 + 2 + 8 + 1 + 32 + 8];
     uint64_t id = ++g_req_id;
-    towire_sigverifyd_gossip_store_prune(f + 4, mlen, id, chain_hash32 != NULL, chain_hash32 ? chain_hash32 : zero, len);
+    const u8 *chain = chain_hash32 ? chain_hash32 : zero;
+    if (repair) towire_sigverifyd_gossip_store_repair(f + 4, mlen, id, chain_hash32 != NULL, chain, len);
+    else towire_sigverifyd_gossip_store_prune(f + 4, mlen, id, chain_hash32 != NULL, chain, len);
     /* every request before it is written out first (send_some writes in order), so the fd rides on this frame's first
      * byte: the daemon matches it to this request */
     while (g_unsent) io_wait();
@@ -1146,8 +1151,18 @@ static bool remote_prune(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip
     u8 *r = g_q[at].reply;
     rl = g_q[at].reply_len;
     g_t = g_s = g_r = at;
+    /* the repair reply is the prune reply's fields, then new_len */
     struct sigverifyd_gossip_store_prune_reply p;
-    if (!fromwire_sigverifyd_gossip_store_prune_reply(r, rl, &p)) die_daemon("malformed gossip_store prune reply");
+    struct sigverifyd_gossip_store_repair_reply q;
+    if (repair) {
+        if (!fromwire_sigverifyd_gossip_store_repair_reply(r, rl, &q)) die_daemon("malformed gossip_store repair reply");
+        p = (struct sigverifyd_gossip_store_prune_reply){q.req_id, q.err, q.version, q.stop, q.end_offset, q.records,
+                                                         q.pruned, q.bad_crc, q.truncated, q.message, q.redundant,
+                                                         q.no_channel, q.signature, q.amount, q.unknown, q.reverified};
+        *new_len = q.new_len;
+    } else if (!fromwire_sigverifyd_gossip_store_prune_reply(r, rl, &p)) {
+        die_daemon("malformed gossip_store prune reply");
+    }
     free(r);
     if (p.err) {
         errno = (int)p.err;
@@ -1174,7 +1189,7 @@ bool gossip_store_prune(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_
     sv_gossip_prune_summary s;
     if (fcntl(fd, F_GETFD) < 0) return false; /* errno EBADF: nothing to send */
     if (client()) {
-        if (!remote_prune(fd, len, chain_hash32, &s)) return false;
+        if (!remote_prune(false, fd, len, chain_hash32, &s, NULL)) return false;
     } else {
         if (!sv_prune_gossip_store_fd) die("gossip_store_prune: this engine has no sv_prune_gossip_store_fd", SV_ERR_ARG);
         int rc = sv_prune_gossip_store_fd(ctx(), fd, len, chain_hash32, &s);
@@ -1182,5 +1197,22 @@ bool gossip_store_prune(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_
         if (rc != SV_OK) die("sv_prune_gossip_store_fd", rc);
     }
     if (summary) *summary = s;
+    return true;
+}
+
+bool gossip_store_repair(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_prune_summary *summary, uint64_t *new_len) {
+    sv_gossip_prune_summary s;
+    uint64_t cut = 0;
+    if (fcntl(fd, F_GETFD) < 0) return false; /* errno EBADF: nothing to send */
+    if (client()) {
+        if (!remote_prune(true, fd, len, chain_hash32, &s, &cut)) return false;
+    } else {
+        if (!sv_repair_gossip_store_fd) die("gossip_store_repair: this engine has no sv_repair_gossip_store_fd", SV_ERR_ARG);
+        int rc = sv_repair_gossip_store_fd(ctx(), fd, len, chain_hash32, &s, &cut);
+        if (rc == SV_ERR_ARG || rc == SV_ERR_IO) return false; /* errno says why */
+        if (rc != SV_OK) die("sv_repair_gossip_store_fd", rc);
+    }
+    if (summary) *summary = s;
+    if (new_len) *new_len = cut;
     return true;
 }

@@ -1,6 +1,6 @@
 /* cln_verify_gossip_store — audit a Core Lightning gossip_store before lightningd loads it.
  *
- *   cln_verify_gossip_store [--chain HEX] [--device N] [--prune OUT] FILE
+ *   cln_verify_gossip_store [--chain HEX] [--device N] [--prune OUT [--cut-tail]] FILE
  *
  * Walks the store as gossmap does, checks every record checksum and verifies every signature on the GPU
  * (sv_verify_gossip_store_host).  Prints a summary and one line per failing record (offset, type, status).
@@ -19,7 +19,12 @@
  *               the store, so gossipd's strict load accepts it;
  *            1  OUT is written but not clean (its walk stops before the end: an incomplete, partial or ended record,
  *               or an announcement without its amount record);
- *            3  usage, I/O or engine error (OUT may be missing). */
+ *            3  usage, I/O or engine error (OUT may be missing).
+ *
+ * --cut-tail (with --prune): OUT also ends where the prune's walk stopped at a torn append (sv_gossip_prune_cut: an
+ * incomplete or partial record, an announcement without its amount record, or a torn header; an announcement the cut
+ * would leave without its amount record goes too), as
+ * sv_repair_gossip_store_fd cuts a file in place.  Prints where it cut, then audits OUT as --prune does. */
 #include <errno.h>
 #include <inttypes.h>
 #include <stdio.h>
@@ -51,7 +56,7 @@ static const char *status_name(int s) {
 }
 
 static int usage(void) {
-    fprintf(stderr, "usage: cln_verify_gossip_store [--chain HEX] [--device N] [--prune OUT] FILE\n");
+    fprintf(stderr, "usage: cln_verify_gossip_store [--chain HEX] [--device N] [--prune OUT [--cut-tail]] FILE\n");
     return 3;
 }
 
@@ -59,8 +64,9 @@ static const char *const reason_name[] = {"kept", "bad checksum", "truncated", "
                                           "update without a channel", "bad signature under the new signer",
                                           "amount record of a deleted announcement", "unknown record type"};
 
-/* --prune: write the pruned copy, report it, audit it; returns the exit code */
-static int prune(sv_ctx *ctx, const char *path, const uint8_t *store, size_t len, const uint8_t *chain, const char *outp) {
+/* --prune: write the pruned copy (cut_tail: without its torn tail), report it, audit it; returns the exit code */
+static int prune(sv_ctx *ctx, const char *path, const uint8_t *store, size_t len, const uint8_t *chain, const char *outp,
+                 int cut_tail) {
     size_t n = sv_gossip_prune_count(store, len);
     uint64_t *off = malloc((n ? n : 1) * sizeof *off);
     uint16_t *type = malloc((n ? n : 1) * sizeof *type);
@@ -75,13 +81,16 @@ static int prune(sv_ctx *ctx, const char *path, const uint8_t *store, size_t len
     }
     for (size_t i = 0; i < n; i++)
         if (why[i]) printf("deleted @%" PRIu64 " type %u: %s (status %d)\n", off[i], type[i], reason_name[why[i]], status[i]);
+    const size_t wlen = cut_tail ? (size_t)sv_gossip_prune_cut(&p, out, len) : len;
     FILE *f = fopen(outp, "wb");
-    if (!f || fwrite(out, 1, len, f) != len || fclose(f)) { fprintf(stderr, "%s: %s\n", outp, strerror(errno)); return 3; }
+    if (!f || fwrite(out, 1, wlen, f) != wlen || fclose(f)) { fprintf(stderr, "%s: %s\n", outp, strerror(errno)); return 3; }
     printf("gossip_store %s: %" PRIu64 " records, walk stopped: %s at %" PRIu64 "; %" PRIu64 " deleted into %s\n", path,
            p.records, p.stop ? status_name(p.stop) : "end of store", p.end_offset, p.pruned, outp);
     const uint64_t count[9] = {0, p.bad_crc, p.truncated, p.message, p.redundant, p.no_channel, p.signature, p.amount, p.unknown};
     for (int k = 1; k < 9; k++) printf("  %" PRIu64 " %s\n", count[k], reason_name[k]);
     printf("  %" PRIu64 " updates verified again under a new signer\n", p.reverified);
+    if (cut_tail) printf("  torn tail: %zu bytes cut, %s ends at %zu\n", len - wlen, outp, wlen);
+    len = wlen;
     size_t m = sv_gossip_store_count(out, len);
     uint64_t *aoff = malloc((m ? m : 1) * sizeof *aoff);
     uint16_t *atype = malloc((m ? m : 1) * sizeof *atype);
@@ -104,7 +113,7 @@ static int prune(sv_ctx *ctx, const char *path, const uint8_t *store, size_t len
 int main(int argc, char **argv) {
     const char *path = NULL, *prune_out = NULL;
     uint8_t chain[32];
-    int have_chain = 0, device = 0;
+    int have_chain = 0, device = 0, cut_tail = 0;
     for (int i = 1; i < argc; i++) {
         if (!strcmp(argv[i], "--chain") && i + 1 < argc) {
             const char *h = argv[++i];
@@ -119,13 +128,15 @@ int main(int argc, char **argv) {
             device = atoi(argv[++i]);
         } else if (!strcmp(argv[i], "--prune") && i + 1 < argc) {
             prune_out = argv[++i];
+        } else if (!strcmp(argv[i], "--cut-tail")) {
+            cut_tail = 1;
         } else if (argv[i][0] == '-' || path) {
             return usage();
         } else {
             path = argv[i];
         }
     }
-    if (!path) return usage();
+    if (!path || (cut_tail && !prune_out)) return usage();
     if (prune_out && !strcmp(prune_out, path)) {
         fprintf(stderr, "--prune: OUT must be another file than %s\n", path);
         return 3;
@@ -143,7 +154,7 @@ int main(int argc, char **argv) {
     if (prune_out) {
         sv_ctx *pctx = NULL;
         if (sv_create(&pctx, device) != SV_OK) { fprintf(stderr, "engine: %s\n", sv_last_error(NULL)); return 3; }
-        int code = prune(pctx, path, store, len, have_chain ? chain : NULL, prune_out);
+        int code = prune(pctx, path, store, len, have_chain ? chain : NULL, prune_out, cut_tail);
         sv_destroy(pctx);
         free(store);
         return code;

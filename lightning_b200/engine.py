@@ -14,7 +14,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SV_LIB") or os.path.join(_HERE, "libcln_sigverify.so")  # SV_LIB: another build of the library (dev)
 
-SV_ERR_ARG, SV_ERR_IO = -4, -5  # sv_status values a caller of sv_prune_gossip_store_fd tells apart
+SV_ERR_ARG, SV_ERR_IO = -4, -5  # sv_status values a caller of sv_prune/repair_gossip_store_fd tells apart
 KIND_ECDSA33 = 0
 KIND_ECDSA_XY = 1
 KIND_SCHNORR = 2
@@ -100,6 +100,10 @@ def load_library():
     lib.sv_prune_gossip_store_host.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp, vp, sz, ctypes.POINTER(SvGossipPruneSummary)]
     lib.sv_get_last_gossip_prune_timing.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
     lib.sv_prune_gossip_store_fd.argtypes = [vp, i, ctypes.c_uint64, vp, ctypes.POINTER(SvGossipPruneSummary)]
+    lib.sv_repair_gossip_store_fd.argtypes = [vp, i, ctypes.c_uint64, vp, ctypes.POINTER(SvGossipPruneSummary),
+                                              ctypes.POINTER(ctypes.c_uint64)]
+    lib.sv_gossip_prune_cut.restype = ctypes.c_uint64
+    lib.sv_gossip_prune_cut.argtypes = [ctypes.POINTER(SvGossipPruneSummary), ctypes.c_char_p, ctypes.c_uint64]
     lib.sv_verify_tx_host.argtypes = [vp, i, vp, vp, sz, vp, vp, sz, vp, vp]
     lib.sv_grind_tx_fee_host.argtypes = [vp, i, vp, vp, sz, vp, vp, ctypes.c_uint64, ctypes.c_uint32, ctypes.c_uint32,
                                          ctypes.POINTER(ctypes.c_int64), ctypes.POINTER(ctypes.c_uint64)]
@@ -329,19 +333,41 @@ class SigVerifier:
         is synced, no other byte changes.  Returns the summary dict prune_gossip_store returns.  A file the call cannot use
         or a store it refuses raises OSError with the call's errno (EINVAL, EBADF, or that of a failed read, write or
         fsync); an engine failure raises EngineError."""
+        return self._store_fd(False, fd, length, chain_hash)[0]
+
+    def repair_gossip_store_fd(self, fd, length, chain_hash=None):
+        """prune_gossip_store_fd, then the file cut where a torn append begins (sv_repair_gossip_store_fd: an incomplete
+        or partial last record, an announcement without its amount record, or a torn header; see gossip_prune_cut).
+        Returns (the summary dict, new_len: where the file ends now).  Errors as prune_gossip_store_fd, and a failed
+        ftruncate raises OSError too."""
+        return self._store_fd(True, fd, length, chain_hash)
+
+    def gossip_prune_cut(self, summary, pruned):
+        """sv_gossip_prune_cut: where sv_repair_gossip_store_fd ends a store whose prune gave `summary` (a dict as
+        prune_gossip_store returns) and the bytes `pruned`"""
+        s = SvGossipPruneSummary(**{f: summary[f] for f, _ in SvGossipPruneSummary._fields_})
+        pruned = bytes(pruned)
+        return int(self.lib.sv_gossip_prune_cut(ctypes.byref(s), pruned, len(pruned)))
+
+    def _store_fd(self, repair, fd, length, chain_hash):
         chain = None
         if chain_hash is not None:
             chain = np.frombuffer(bytes(chain_hash), dtype=np.uint8)
             if chain.size != 32:
                 raise ValueError("chain_hash must be 32 bytes")
-        s = SvGossipPruneSummary()
-        rc = self.lib.sv_prune_gossip_store_fd(self._ctx, int(fd), int(length), chain.ctypes.data if chain is not None else None,
-                                               ctypes.byref(s))
+        s, new_len = SvGossipPruneSummary(), ctypes.c_uint64(0)
+        cp = chain.ctypes.data if chain is not None else None
+        if repair:
+            name = "sv_repair_gossip_store_fd"
+            rc = self.lib.sv_repair_gossip_store_fd(self._ctx, int(fd), int(length), cp, ctypes.byref(s), ctypes.byref(new_len))
+        else:
+            name = "sv_prune_gossip_store_fd"
+            rc = self.lib.sv_prune_gossip_store_fd(self._ctx, int(fd), int(length), cp, ctypes.byref(s))
         if rc in (SV_ERR_ARG, SV_ERR_IO):
             e = ctypes.get_errno() or errno.EINVAL
-            raise OSError(e, f"sv_prune_gossip_store_fd: {os.strerror(e)}")
-        self._check(rc, "sv_prune_gossip_store_fd")
-        return {f: getattr(s, f) for f, _ in SvGossipPruneSummary._fields_}
+            raise OSError(e, f"{name}: {os.strerror(e)}")
+        self._check(rc, name)
+        return {f: getattr(s, f) for f, _ in SvGossipPruneSummary._fields_}, int(new_len.value)
 
     def last_gossip_prune_timing(self):
         """(header walk, first round, second round, flag write) in ms of the last prune_gossip_store (profiling mode)"""
