@@ -148,7 +148,8 @@ int sv_verify_gossip_host(sv_ctx *ctx, const uint8_t *blob, size_t blob_len, con
  *          2  as 0; if no announcement resolves, signers33[m] is the source peer and the update is checked as gossipd's
  *             private-update path does (:1099-1110): 5 if it verifies under the peer, -2 otherwise.
  *      Every channel_announcement reports its own signatures, duplicates included.  Not decided here (policy, not
- *      signatures): timestamp_reasonable, txout confirmation, node_announcements of nodes without channels.
+ *      signatures): timestamp_reasonable, txout confirmation, node_announcements of nodes without channels.  For a
+ *      gossip_store, sv_verify_gossip_store_funding_host decides the txout from lightningd's own tables.
  *      signer_kind == NULL means all 0; signers33 (33 bytes per MESSAGE) may be NULL only when no channel_update has kind 1
  *      or 2; a signer_kind above 2 (any message) is SV_ERR_ARG.  Resolution never reaches outside the call.  On the device:
  *      an scid table of the gated announcements, one resolve thread per update and ONE verification launch for all
@@ -279,6 +280,83 @@ int sv_prune_gossip_store_host(sv_ctx *ctx, const uint8_t *store, size_t len, co
 /* profiling mode: ms4 = host header walk, first round (H2D of the store, checksums, the audit's kernels), second round
  * (mark, resolution, compaction, re-verification), flag write and copy back */
 int sv_get_last_gossip_prune_timing(sv_ctx *ctx, float *ms4);
+
+/* ---- FUNDING of a gossip_store's channels: the audit and the prune above, plus the check gossipd makes before it lets a
+ *      channel_announcement in from a peer and which a store not written by this node's gossipd never had.  gossipd asks
+ *      lightningd for the announcement's txout (gossipd/gossmap_manage.c:748-751) and drops the announcement unless an
+ *      unspent output exists and its script is the P2WSH of the 2-of-2 of the announcement's bitcoin keys; it then writes
+ *      the announcement and a channel_amount record with the output's amount (:850-852), which gossmap takes as the
+ *      channel's capacity (common/gossmap.c:1473-1499).  lightningd answers from two tables (get_txout,
+ *      lightningd/gossip_control.c:78-115): the unspent P2WSH outputs of the blocks it processed (utxoset, spendheight
+ *      NULL, wallet_outpoint_for_scid) and the heights of those blocks (blocks, wallet_have_block).  The caller passes
+ *      them as sv_funding_table; lightning_b200/funding.py reads them from lightningd.sqlite3.
+ *
+ *      One verdict per record (rec_funding).  Every live channel_announcement the walk reaches whose message status is 0
+ *      gets one of SV_GF_FUNDED..SV_GF_AMOUNT, redundant ones included; every other record SV_GF_NONE.  With
+ *      scid = block << 40 | txindex << 16 | outnum, read from the announcement:
+ *        SV_GF_DYING      the record's header has GOSSIP_STORE_DYING_BIT (0x0800): gossipd has seen the spend and deletes
+ *                         the channel at its deadline (gossipd/gossmap_manage.c:1420-1433).  Whatever the table says.
+ *        SV_GF_FUNDED     the table has an output at scid whose 34-byte script is 0x00 0x20 || SHA-256(script) of the
+ *                         2-of-2 (bitcoin_redeem_2of2, bitcoin/script.c:151-167: OP_2 <ka> <kb> OP_2 OP_CHECKMULTISIG with
+ *                         the 33-byte keys in memcmp order, pubkey_cmp bitcoin/pubkey.c:84-90), and the record directly
+ *                         after the announcement (by the header's length, whatever its flags, as gossmap_chan_get_capacity
+ *                         reads it, common/gossmap.c:1488-1495) is a channel_amount (4101) holding the output's amount.
+ *        SV_GF_UNCHECKED  no output at scid and block is not a processed height: lightningd would ask bitcoind
+ *                         (getfilteredblock, lightningd/gossip_control.c:104-112), which this call cannot.
+ *        SV_GF_NO_TXOUT   no output at scid and block is a processed height (the wallet_have_block branch, :97-103):
+ *                         gossipd ignores the announcement (gossipd/gossmap_manage.c:791-810).
+ *        SV_GF_SCRIPT     the output's script is not that P2WSH (:696-699, :812-819).
+ *        SV_GF_AMOUNT     the script matches, but the next record is not a channel_amount or holds another amount: gossipd
+ *                         would have written the txout's amount (:850-852).
+ *      The audit (sv_verify_gossip_store_funding_host) writes exactly what sv_verify_gossip_store_host writes, plus
+ *      rec_funding and *fsummary (fsummary->deleted = 0).  Records at or after a BAD_CRC or NO_AMOUNT stop get SV_GF_NONE.
+ *
+ *      The prune (sv_prune_gossip_store_funding_host) extends rule 2 of sv_prune_gossip_store_host: a channel_announcement
+ *      whose first-round status is 0 and whose verdict is SV_GF_NO_TXOUT, SV_GF_SCRIPT or SV_GF_AMOUNT is deleted
+ *      (SV_GP_FUNDING).  SV_GF_UNCHECKED and SV_GF_DYING are kept.  Rules 3 to 6 then run unchanged: the second channel
+ *      table gives the scid to a later live announcement or to none, the updates are verified again under the new holder
+ *      or deleted, and the channel_amount record goes with its announcement.  No other round is needed: a funding
+ *      deletion is one more announcement masked out of the second round, exactly as a failing one.  So when no
+ *      announcement is deleted for funding, every output equals sv_prune_gossip_store_host's; summary->pruned counts the
+ *      funding deletions as well, and fsummary->deleted says how many there were.  rec_funding is NONE at and after a
+ *      NO_AMOUNT stop.
+ *
+ *      The table: scid[n_outputs] unique (a duplicate is SV_ERR_ARG, nothing written), any order; satoshis and script34
+ *      (34 bytes) per output; blocks[n_blocks] any order.  It is staged on the device for the call and sorted there (CUB
+ *      radix sort); k_store_funding runs one thread per candidate announcement: the 2-of-2 script in registers, its
+ *      SHA-256, the scid and the block by binary search, and the amount record and the header flags read from the staged
+ *      store.  Otherwise the arguments and errors are those of the calls without the table. ---- */
+#define SV_GF_NONE 0
+#define SV_GF_FUNDED 1
+#define SV_GF_UNCHECKED 2
+#define SV_GF_DYING 3
+#define SV_GF_NO_TXOUT 4
+#define SV_GF_SCRIPT 5
+#define SV_GF_AMOUNT 6
+#define SV_GP_FUNDING 9
+typedef struct {
+    const uint64_t *scid;     /* n_outputs, unique, any order: block << 40 | txindex << 16 | outnum */
+    const uint64_t *satoshis; /* n_outputs */
+    const uint8_t *script34;  /* 34 bytes per output (lightningd keeps P2WSH outputs only) */
+    size_t n_outputs;
+    const uint32_t *blocks;   /* processed block heights, any order */
+    size_t n_blocks;
+} sv_funding_table;
+typedef struct {
+    uint64_t checked;  /* announcements given a verdict: the sum of the six below */
+    uint64_t funded, unchecked, no_txout, script, amount, dying;
+    uint64_t deleted;  /* the prune: announcements deleted for funding (SV_GP_FUNDING); the audit: 0 */
+} sv_gossip_funding_summary;
+int sv_verify_gossip_store_funding_host(sv_ctx *ctx, const uint8_t *store, size_t len, const uint8_t *chain_hash32,
+                                        const sv_funding_table *table, uint64_t *rec_off, uint16_t *rec_type,
+                                        int *rec_status, uint64_t *rec_holder, uint8_t *rec_funding, size_t rec_capacity,
+                                        sv_gossip_store_summary *summary, sv_gossip_funding_summary *fsummary);
+int sv_prune_gossip_store_funding_host(sv_ctx *ctx, const uint8_t *store, size_t len, const uint8_t *chain_hash32,
+                                       const sv_funding_table *table, uint8_t *out, uint64_t *rec_off, uint16_t *rec_type,
+                                       int *rec_status, uint8_t *rec_pruned, uint8_t *rec_funding, size_t rec_capacity,
+                                       sv_gossip_prune_summary *summary, sv_gossip_funding_summary *fsummary);
+/* profiling mode: ms2 = the last funding call's table staging and sort, and its k_store_funding (device events) */
+int sv_get_last_gossip_funding_timing(sv_ctx *ctx, float *ms2);
 
 /* ---- PRUNE a gossip_store FILE in place: the store is bytes [0, len) of fd, which must be a regular file opened for
  *      reading and writing.  The store is read (pread) into host memory and pruned by sv_prune_gossip_store_host with out

@@ -1,6 +1,6 @@
 /* cln_verify_gossip_store — audit a Core Lightning gossip_store before lightningd loads it.
  *
- *   cln_verify_gossip_store [--chain HEX] [--device N] [--prune OUT [--cut-tail]] FILE
+ *   cln_verify_gossip_store [--chain HEX] [--device N] [--funding TABLE] [--prune OUT [--cut-tail]] FILE
  *
  * Walks the store as gossmap does, checks every record checksum and verifies every signature on the GPU
  * (sv_verify_gossip_store_host).  Prints a summary and one line per failing record (offset, type, status).
@@ -24,9 +24,18 @@
  * --cut-tail (with --prune): OUT also ends where the prune's walk stopped at a torn append (sv_gossip_prune_cut: an
  * incomplete or partial record, an announcement without its amount record, or a torn header; an announcement the cut
  * would leave without its amount record goes too), as
- * sv_repair_gossip_store_fd cuts a file in place.  Prints where it cut, then audits OUT as --prune does. */
+ * sv_repair_gossip_store_fd cuts a file in place.  Prints where it cut, then audits OUT as --prune does.
+ *
+ * --funding TABLE: also checks every announcement against lightningd's funding outputs (TABLE as written by
+ * `python -m lightning_b200.funding export`; sv_verify_gossip_store_funding_host).  Prints the funding counts and one
+ * line per announcement gossipd would have refused (no unspent output, wrong script, wrong amount record).  Without
+ * --prune it exits 1 if there is one (unless a worse code applies).  With --prune it deletes them too
+ * (sv_prune_gossip_store_funding_host), and OUT's audit runs with the table: OUT is clean only if no announcement in it
+ * is refused.  Announcements in blocks lightningd never processed (unchecked) and dying channels are printed and never
+ * change the exit code. */
 #include <errno.h>
 #include <inttypes.h>
+#include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -56,27 +65,90 @@ static const char *status_name(int s) {
 }
 
 static int usage(void) {
-    fprintf(stderr, "usage: cln_verify_gossip_store [--chain HEX] [--device N] [--prune OUT [--cut-tail]] FILE\n");
+    fprintf(stderr, "usage: cln_verify_gossip_store [--chain HEX] [--device N] [--funding TABLE] [--prune OUT [--cut-tail]] "
+                    "FILE\n");
     return 3;
 }
 
 static const char *const reason_name[] = {"kept", "bad checksum", "truncated", "failing message", "redundant announcement",
                                           "update without a channel", "bad signature under the new signer",
-                                          "amount record of a deleted announcement", "unknown record type"};
+                                          "amount record of a deleted announcement", "unknown record type",
+                                          "announcement gossipd would refuse for its funding output"};
+static const char *const funding_name[] = {"-", "funded", "unchecked (block not processed)", "dying",
+                                           "no unspent output", "script is not the 2-of-2", "amount record differs"};
+
+/* the funding table file (lightning_b200/funding.py): "CLNFUND1", u64 n_outputs, u64 n_blocks (little-endian), then
+ * n_outputs x [scid u64, satoshis u64, script 34 bytes], then n_blocks x [height u32] */
+typedef struct {
+    sv_funding_table t;
+    uint64_t *scid, *sats;
+    uint8_t *script;
+    uint32_t *blocks;
+} funding_file;
+
+static uint64_t le64(const uint8_t *p) {
+    uint64_t v = 0;
+    for (int i = 7; i >= 0; i--) v = (v << 8) | p[i];
+    return v;
+}
+
+static int load_funding(const char *path, funding_file *F) {
+    FILE *f = fopen(path, "rb");
+    if (!f) { fprintf(stderr, "%s: %s\n", path, strerror(errno)); return -1; }
+    uint8_t h[24], e[50], b[4];
+    if (fread(h, 1, 24, f) != 24 || memcmp(h, "CLNFUND1", 8)) {
+        fprintf(stderr, "%s: not a funding table\n", path);
+        fclose(f);
+        return -1;
+    }
+    const uint64_t n = le64(h + 8), nb = le64(h + 16);
+    if (n > ((uint64_t)1 << 32) || nb > ((uint64_t)1 << 32)) { fprintf(stderr, "%s: not a funding table\n", path); fclose(f); return -1; }
+    F->scid = malloc((n ? n : 1) * 8);
+    F->sats = malloc((n ? n : 1) * 8);
+    F->script = malloc((n ? n : 1) * 34);
+    F->blocks = malloc((nb ? nb : 1) * 4);
+    if (!F->scid || !F->sats || !F->script || !F->blocks) { fprintf(stderr, "out of memory\n"); fclose(f); return -1; }
+    for (uint64_t i = 0; i < n; i++) {
+        if (fread(e, 1, 50, f) != 50) { fprintf(stderr, "%s: truncated\n", path); fclose(f); return -1; }
+        F->scid[i] = le64(e);
+        F->sats[i] = le64(e + 8);
+        memcpy(F->script + 34 * i, e + 16, 34);
+    }
+    for (uint64_t i = 0; i < nb; i++) {
+        if (fread(b, 1, 4, f) != 4) { fprintf(stderr, "%s: truncated\n", path); fclose(f); return -1; }
+        F->blocks[i] = (uint32_t)b[0] | (uint32_t)b[1] << 8 | (uint32_t)b[2] << 16 | (uint32_t)b[3] << 24;
+    }
+    if (fread(b, 1, 1, f) != 0) { fprintf(stderr, "%s: trailing bytes\n", path); fclose(f); return -1; }
+    fclose(f);
+    F->t = (sv_funding_table){F->scid, F->sats, F->script, (size_t)n, F->blocks, (size_t)nb};
+    return 0;
+}
+
+/* prints the funding counts; returns the number of refused announcements */
+static uint64_t print_funding(const char *what, const sv_gossip_funding_summary *g) {
+    printf("  funding (%s): %" PRIu64 " announcements checked: %" PRIu64 " funded, %" PRIu64 " unchecked, %" PRIu64
+           " dying, %" PRIu64 " no unspent output, %" PRIu64 " wrong script, %" PRIu64 " wrong amount\n",
+           what, g->checked, g->funded, g->unchecked, g->dying, g->no_txout, g->script, g->amount);
+    return g->no_txout + g->script + g->amount;
+}
 
 /* --prune: write the pruned copy (cut_tail: without its torn tail), report it, audit it; returns the exit code */
 static int prune(sv_ctx *ctx, const char *path, const uint8_t *store, size_t len, const uint8_t *chain, const char *outp,
-                 int cut_tail) {
+                 int cut_tail, const sv_funding_table *table) {
     size_t n = sv_gossip_prune_count(store, len);
     uint64_t *off = malloc((n ? n : 1) * sizeof *off);
     uint16_t *type = malloc((n ? n : 1) * sizeof *type);
     int *status = malloc((n ? n : 1) * sizeof *status);
-    uint8_t *why = malloc(n ? n : 1), *out = malloc(len);
-    if (!off || !type || !status || !why || !out) { fprintf(stderr, "out of memory\n"); return 3; }
+    uint8_t *why = malloc(n ? n : 1), *fund = malloc(n ? n : 1), *out = malloc(len);
+    if (!off || !type || !status || !why || !fund || !out) { fprintf(stderr, "out of memory\n"); return 3; }
     sv_gossip_prune_summary p;
-    int rc = sv_prune_gossip_store_host(ctx, store, len, chain, out, off, type, status, why, n, &p);
+    sv_gossip_funding_summary g;
+    int rc = table ? sv_prune_gossip_store_funding_host(ctx, store, len, chain, table, out, off, type, status, why, fund, n,
+                                                        &p, &g)
+                   : sv_prune_gossip_store_host(ctx, store, len, chain, out, off, type, status, why, n, &p);
     if (rc != SV_OK) {
-        fprintf(stderr, "sv_prune_gossip_store_host: %d %s\n", rc, sv_last_error(ctx));
+        fprintf(stderr, "%s: %d %s\n", table ? "sv_prune_gossip_store_funding_host" : "sv_prune_gossip_store_host", rc,
+                sv_last_error(ctx));
         return 3;
     }
     for (size_t i = 0; i < n; i++)
@@ -88,30 +160,36 @@ static int prune(sv_ctx *ctx, const char *path, const uint8_t *store, size_t len
            p.records, p.stop ? status_name(p.stop) : "end of store", p.end_offset, p.pruned, outp);
     const uint64_t count[9] = {0, p.bad_crc, p.truncated, p.message, p.redundant, p.no_channel, p.signature, p.amount, p.unknown};
     for (int k = 1; k < 9; k++) printf("  %" PRIu64 " %s\n", count[k], reason_name[k]);
+    if (table) printf("  %" PRIu64 " %s\n", g.deleted, reason_name[SV_GP_FUNDING]);
     printf("  %" PRIu64 " updates verified again under a new signer\n", p.reverified);
+    if (table) print_funding(path, &g);
     if (cut_tail) printf("  torn tail: %zu bytes cut, %s ends at %zu\n", len - wlen, outp, wlen);
     len = wlen;
     size_t m = sv_gossip_store_count(out, len);
     uint64_t *aoff = malloc((m ? m : 1) * sizeof *aoff);
     uint16_t *atype = malloc((m ? m : 1) * sizeof *atype);
     int *astatus = malloc((m ? m : 1) * sizeof *astatus);
-    if (!aoff || !atype || !astatus) { fprintf(stderr, "out of memory\n"); return 3; }
+    uint8_t *afund = malloc(m ? m : 1);
+    if (!aoff || !atype || !astatus || !afund) { fprintf(stderr, "out of memory\n"); return 3; }
     sv_gossip_store_summary s;
-    rc = sv_verify_gossip_store_host(ctx, out, len, chain, aoff, atype, astatus, NULL, m, &s);
+    rc = table ? sv_verify_gossip_store_funding_host(ctx, out, len, chain, table, aoff, atype, astatus, NULL, afund, m, &s, &g)
+               : sv_verify_gossip_store_host(ctx, out, len, chain, aoff, atype, astatus, NULL, m, &s);
     if (rc != SV_OK) {
-        fprintf(stderr, "sv_verify_gossip_store_host: %d %s\n", rc, sv_last_error(ctx));
+        fprintf(stderr, "%s: %d %s\n", table ? "sv_verify_gossip_store_funding_host" : "sv_verify_gossip_store_host", rc,
+                sv_last_error(ctx));
         return 3;
     }
+    const uint64_t refused = table ? print_funding(outp, &g) : 0;
     const int clean = s.stop == SV_GS_EOF && s.end_offset == len && !s.bad_signature && !s.malformed && !s.no_channel &&
-                      !s.wrong_chain && !s.bad_order && !s.redundant_announcements && !s.unknown;
+                      !s.wrong_chain && !s.bad_order && !s.redundant_announcements && !s.unknown && !refused;
     printf("%s: %s (%" PRIu64 " good messages, %" PRIu64 " deleted records)\n", outp,
            clean ? "clean" : "NOT clean", s.good, s.deleted);
-    free(off); free(type); free(status); free(why); free(out); free(aoff); free(atype); free(astatus);
+    free(off); free(type); free(status); free(why); free(fund); free(out); free(aoff); free(atype); free(astatus); free(afund);
     return clean ? 0 : 1;
 }
 
 int main(int argc, char **argv) {
-    const char *path = NULL, *prune_out = NULL;
+    const char *path = NULL, *prune_out = NULL, *funding_path = NULL;
     uint8_t chain[32];
     int have_chain = 0, device = 0, cut_tail = 0;
     for (int i = 1; i < argc; i++) {
@@ -128,6 +206,8 @@ int main(int argc, char **argv) {
             device = atoi(argv[++i]);
         } else if (!strcmp(argv[i], "--prune") && i + 1 < argc) {
             prune_out = argv[++i];
+        } else if (!strcmp(argv[i], "--funding") && i + 1 < argc) {
+            funding_path = argv[++i];
         } else if (!strcmp(argv[i], "--cut-tail")) {
             cut_tail = 1;
         } else if (argv[i][0] == '-' || path) {
@@ -140,6 +220,12 @@ int main(int argc, char **argv) {
     if (prune_out && !strcmp(prune_out, path)) {
         fprintf(stderr, "--prune: OUT must be another file than %s\n", path);
         return 3;
+    }
+    funding_file ff;
+    const sv_funding_table *table = NULL;
+    if (funding_path) {
+        if (load_funding(funding_path, &ff)) return 3;
+        table = &ff.t;
     }
     FILE *f = fopen(path, "rb");
     if (!f) { fprintf(stderr, "%s: %s\n", path, strerror(errno)); return 3; }
@@ -154,7 +240,7 @@ int main(int argc, char **argv) {
     if (prune_out) {
         sv_ctx *pctx = NULL;
         if (sv_create(&pctx, device) != SV_OK) { fprintf(stderr, "engine: %s\n", sv_last_error(NULL)); return 3; }
-        int code = prune(pctx, path, store, len, have_chain ? chain : NULL, prune_out, cut_tail);
+        int code = prune(pctx, path, store, len, have_chain ? chain : NULL, prune_out, cut_tail, table);
         sv_destroy(pctx);
         free(store);
         return code;
@@ -164,13 +250,18 @@ int main(int argc, char **argv) {
     uint64_t *off = malloc((n ? n : 1) * sizeof *off);
     uint16_t *type = malloc((n ? n : 1) * sizeof *type);
     int *status = malloc((n ? n : 1) * sizeof *status);
+    uint8_t *fund = malloc(n ? n : 1);
     sv_ctx *ctx = NULL;
-    if (!off || !type || !status) { fprintf(stderr, "out of memory\n"); return 3; }
+    if (!off || !type || !status || !fund) { fprintf(stderr, "out of memory\n"); return 3; }
     if (sv_create(&ctx, device) != SV_OK) { fprintf(stderr, "engine: %s\n", sv_last_error(NULL)); return 3; }
     sv_gossip_store_summary s;
-    int rc = sv_verify_gossip_store_host(ctx, store, len, have_chain ? chain : NULL, off, type, status, NULL, n, &s);
+    sv_gossip_funding_summary g;
+    int rc = table ? sv_verify_gossip_store_funding_host(ctx, store, len, have_chain ? chain : NULL, table, off, type, status,
+                                                         NULL, fund, n, &s, &g)
+                   : sv_verify_gossip_store_host(ctx, store, len, have_chain ? chain : NULL, off, type, status, NULL, n, &s);
     if (rc != SV_OK) {
-        fprintf(stderr, "sv_verify_gossip_store_host: %d %s\n", rc, sv_last_error(ctx));
+        fprintf(stderr, "%s: %d %s\n", table ? "sv_verify_gossip_store_funding_host" : "sv_verify_gossip_store_host", rc,
+                sv_last_error(ctx));
         sv_destroy(ctx);
         return 3;
     }
@@ -184,6 +275,8 @@ int main(int argc, char **argv) {
             printf("record @%" PRIu64 " type %u: %d (%s)\n", off[i], type[i], st, status_name(st));
             failing += st < SV_GS_DELETED;
         }
+        if (table && fund[i] != SV_GF_NONE && fund[i] != SV_GF_FUNDED)
+            printf("record @%" PRIu64 " type %u: funding %s\n", off[i], type[i], funding_name[fund[i]]);
     }
     printf("gossip_store %s: version %u, %" PRIu64 " bytes, %" PRIu64 " records, walk stopped: %s at %" PRIu64 "\n", path,
            s.version, (uint64_t)len, s.records, s.stop ? status_name(s.stop) : "end of store", s.end_offset);
@@ -195,7 +288,8 @@ int main(int argc, char **argv) {
            s.deleted, s.store_records, s.unknown, s.not_reached);
     printf("  %" PRIu64 " redundant announcements, %" PRIu64 " updates without a channel\n", s.redundant_announcements,
            s.updates_without_channel);
-    free(store); free(off); free(type); free(status);
+    const uint64_t refused = table ? print_funding(path, &g) : 0;
+    free(store); free(off); free(type); free(status); free(fund);
     if (s.stop == SV_GS_BAD_CRC || s.stop == SV_GS_TRUNCATED || s.stop == SV_GS_NO_AMOUNT) return 2;
-    return failing ? 1 : 0;
+    return failing || refused ? 1 : 0;
 }

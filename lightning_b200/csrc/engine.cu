@@ -35,6 +35,7 @@
 #include "verify.cuh"
 #include "bolt12.cuh"
 #include "gossip_store.cuh"
+#include "gossip_funding.cuh"
 #include "selftest.cuh"
 #include "batch.cuh"  // constants and the host-testable stages; the kernels themselves are in batch.cu
 
@@ -650,19 +651,23 @@ __global__ void __launch_bounds__(256) k_store_crc_flags(const u8* store, const 
     if (r < n) bad[r] = !gs_record_crc_ok(tab, store, rec_off[r]);
 }
 // k_prune_mark: thread i < n_msgs turns message i's first-round status into its deletion (an announcement that is not 0,
-// an update that is -1 or -3: SV_GP_MESSAGE); thread i < nev masks event i out of the second round if it is the
-// announcement of a deleted message
+// an update that is -1 or -3: SV_GP_MESSAGE), and with a funding verdict per message (fund, else NULL) an announcement
+// gossipd would have refused for its txout (SV_GP_FUNDING); thread i < nev masks event i out of the second round if it
+// is the announcement of a deleted message
 __global__ void __launch_bounds__(256) k_prune_mark(const u8* store, const u64* msg_off, const int* status, size_t n_msgs,
                                                     const u8* ev_kind, const u32* ev_msg, const u8* ok, size_t nev,
-                                                    u8* reason, u8* ok2) {
+                                                    const u8* fund, u8* reason, u8* ok2) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n_msgs) {
         const u8* p = store + msg_off[i];
         const int st = status[i];
         const bool upd = p[0] == 1 && p[1] == 2;
-        reason[i] = (upd ? (st == -1 || st == -3) : st != 0) ? SV_GP_MESSAGE : SV_GP_KEPT;
+        reason[i] = (upd ? (st == -1 || st == -3) : st != 0) ? SV_GP_MESSAGE
+                    : (fund && gf_refused(fund[i]))           ? SV_GP_FUNDING
+                                                               : SV_GP_KEPT;
     }
-    if (i < nev) ok2[i] = ok[i] && !(ev_kind[i] == GS_EV_ANN && status[ev_msg[i]] != 0);
+    if (i < nev)
+        ok2[i] = ok[i] && !(ev_kind[i] == GS_EV_ANN && (status[ev_msg[i]] != 0 || (fund && gf_refused(fund[ev_msg[i]]))));
 }
 // k_prune_select: one thread per message not yet deleted, after the second k_store_resolve (holder2, signers2).  An
 // announcement that is redundant now: SV_GP_REDUNDANT.  An update without a channel: SV_GP_NO_CHANNEL; with the same
@@ -712,6 +717,26 @@ __global__ void __launch_bounds__(256) k_prune_flags(u8* store, const u64* rec_o
     const u8 v = store[rec_off[i]] | (u8)(GS_DELETED >> 8);
     store[rec_off[i]] = v;
     flag_hi[i] = v;
+}
+
+// ---- gossip_store funding (gossip_funding.cuh): lightningd's funding outputs against the announcements ---------------
+// fills idx[i] = i: the values the table's scids carry through the sort
+__global__ void __launch_bounds__(256) k_funding_iota(u32* idx, size_t n) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) idx[i] = (u32)i;
+}
+// *dup = 1 if two neighbours of the sorted scids are equal
+__global__ void __launch_bounds__(256) k_funding_dups(const u64* scid, size_t n, u32* dup) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i > 0 && i < n && scid[i] == scid[i - 1]) *dup = 1;
+}
+// one thread per candidate announcement (message index cand[i]): fund[cand[i]] = its verdict (gf_verdict)
+__global__ void __launch_bounds__(128) k_store_funding(const u8* store, u64 len, const u64* msg_off, const u32* cand, size_t n,
+                                                       gf_table t, u8* fund) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const u32 m = cand[i];
+    fund[m] = (u8)gf_verdict(store, len, msg_off[m] - GS_HDR, t);
 }
 
 // ---- BOLT12 signatures (bolt12.cuh): the message hash of bolt12_check_signature on the device -----------------------
@@ -1303,6 +1328,7 @@ struct sv_ctx {
     cudaEvent_t b12_ev[2] = {};  // around the BOLT12 parse / Merkle / sighash kernels (profiling mode only)
     float gs_ms[4] = {};         // last sv_verify_gossip_store_host: header walk, H2D, checksums, verification (profiling mode)
     float gp_ms[4] = {};         // last sv_prune_gossip_store_host: header walk, first round, second round, flag write
+    float gf_ms[2] = {};         // last funding call: table staging and sort, k_store_funding
     unsigned long long launches = 0;
     std::vector<sv_queue_item> queue;
     std::string err;
@@ -2161,10 +2187,97 @@ static int store_pass_run(sv_ctx* ctx, const u8* d_store, size_t len, const uint
     return SV_OK;
 }
 
-extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, size_t len, const uint8_t* chain_hash32,
-                                           uint64_t* rec_off, uint16_t* rec_type, int* rec_status, uint64_t* rec_holder,
-                                           size_t rec_capacity, sv_gossip_store_summary* sum) {
-    if (!ctx || !store || len < 1 || !sum || (rec_capacity && (!rec_off || !rec_type || !rec_status))) return SV_ERR_ARG;
+// The funding table staged on the device for one call and sorted there: the outputs by scid (their entries carried as
+// values), the heights ascending.  A duplicate scid is SV_ERR_ARG.  ev (profiling mode): e[0], e[1] around the staging.
+struct funding_stage {
+    dev_buf<> s;
+    gf_table t{};
+};
+static int funding_stage_run(sv_ctx* ctx, const sv_funding_table* tb, funding_stage& F, const ev_set& ev) {
+    cudaStream_t st = ctx->stream;
+    const size_t n = tb->n_outputs, nb = tb->n_blocks;
+    if (n >= 0x7FFFFFFFu || nb >= 0x7FFFFFFFu) return fail(ctx, SV_ERR_ARG, "funding table too large", cudaSuccess);
+    size_t cub_pairs = 0, cub_keys = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, cub_pairs, (const u64*)nullptr, (u64*)nullptr, (const u32*)nullptr,
+                                       (u32*)nullptr, (int)n, 0, 64, st));
+    CK(cub::DeviceRadixSort::SortKeys(nullptr, cub_keys, (const u32*)nullptr, (u32*)nullptr, (int)nb, 0, 32, st));
+    // one slab: per output [scid u64 x2][entry u32 x2][amount u64][script 34B], per height [u32 x2], the duplicate
+    // flag, sort scratch
+    slab_layout L;
+    const size_t o_key = L.take(8 * n), o_key2 = L.take(8 * n), o_idx = L.take(4 * n), o_idx2 = L.take(4 * n),
+                 o_sat = L.take(8 * n), o_script = L.take(34 * n), o_blk = L.take(4 * nb), o_blk2 = L.take(4 * nb),
+                 o_dup = L.take(4), o_cub = L.take(cub_pairs > cub_keys ? cub_pairs : cub_keys);
+    int rc = F.s.reserve(ctx, L.size, L.size);
+    if (rc) return rc;
+    dev_buf<>& s = F.s;
+    u32* d_dup = s.at<u32>(o_dup);
+    if (ev.e[0]) CK(cudaEventRecord(ev.e[0], st));
+    CK(cudaMemsetAsync(d_dup, 0, 4, st));
+    if (n) {
+        CK(cudaMemcpyAsync(s.at<u64>(o_key), tb->scid, 8 * n, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(s.at<u64>(o_sat), tb->satoshis, 8 * n, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(s + o_script, tb->script34, 34 * n, cudaMemcpyHostToDevice, st));
+        k_funding_iota<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(s.at<u32>(o_idx), n);
+        CK(cub::DeviceRadixSort::SortPairs(s + o_cub, cub_pairs, s.at<u64>(o_key), s.at<u64>(o_key2), s.at<u32>(o_idx),
+                                           s.at<u32>(o_idx2), (int)n, 0, 64, st));
+        k_funding_dups<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(s.at<u64>(o_key2), n, d_dup);
+        ctx->launches += 2;
+    }
+    if (nb) {
+        CK(cudaMemcpyAsync(s.at<u32>(o_blk), tb->blocks, 4 * nb, cudaMemcpyHostToDevice, st));
+        CK(cub::DeviceRadixSort::SortKeys(s + o_cub, cub_keys, s.at<u32>(o_blk), s.at<u32>(o_blk2), (int)nb, 0, 32, st));
+    }
+    if (ev.e[1]) CK(cudaEventRecord(ev.e[1], st));
+    u32 dup = 0;
+    CK(cudaMemcpyAsync(&dup, d_dup, 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (dup) return fail(ctx, SV_ERR_ARG, "funding table: a scid appears twice", cudaSuccess);
+    F.t = gf_table{s.at<u64>(o_key2), s.at<u32>(o_idx2), s.at<u64>(o_sat), s + o_script, (u64)n, s.at<u32>(o_blk2), (u64)nb};
+    return SV_OK;
+}
+static bool funding_table_ok(const sv_funding_table* t) {
+    return t && (!t->n_outputs || (t->scid && t->satoshis && t->script34)) && (!t->n_blocks || t->blocks);
+}
+// fund[m] (n_msgs bytes, device) = the verdict of each message listed in cand (host), GF_NONE for the others; ev: e[2],
+// e[3] around the kernel
+static int funding_run(sv_ctx* ctx, const u8* d_store, size_t len, const u64* d_moff, size_t n_msgs,
+                       const std::vector<u32>& cand, const funding_stage& F, u8* d_fund, u32* d_cand, const ev_set& ev) {
+    cudaStream_t st = ctx->stream;
+    CK(cudaMemsetAsync(d_fund, GF_NONE, n_msgs, st));
+    if (ev.e[2]) CK(cudaEventRecord(ev.e[2], st));
+    if (!cand.empty()) {
+        CK(cudaMemcpyAsync(d_cand, cand.data(), 4 * cand.size(), cudaMemcpyHostToDevice, st));
+        k_store_funding<<<(unsigned)((cand.size() + 127) / 128), 128, 0, st>>>(d_store, len, d_moff, d_cand, cand.size(),
+                                                                               F.t, d_fund);
+        ctx->launches += 1;
+    }
+    if (ev.e[3]) CK(cudaEventRecord(ev.e[3], st));
+    return SV_OK;
+}
+static void funding_count(sv_gossip_funding_summary& F, u8 v) {
+    uint64_t* per[7] = {nullptr, &F.funded, &F.unchecked, &F.dying, &F.no_txout, &F.script, &F.amount};
+    if (v == GF_NONE) return;
+    F.checked++;
+    (*per[v])++;
+}
+static int funding_timing(sv_ctx* ctx, const ev_set& fev) {
+    if (fev.e[0]) {
+        CK(cudaEventElapsedTime(&ctx->gf_ms[0], fev.e[0], fev.e[1]));
+        CK(cudaEventElapsedTime(&ctx->gf_ms[1], fev.e[2], fev.e[3]));
+    }
+    return SV_OK;
+}
+
+static_assert(GF_NONE == SV_GF_NONE && GF_FUNDED == SV_GF_FUNDED && GF_UNCHECKED == SV_GF_UNCHECKED &&
+                  GF_DYING == SV_GF_DYING && GF_NO_TXOUT == SV_GF_NO_TXOUT && GF_SCRIPT == SV_GF_SCRIPT &&
+                  GF_AMOUNT == SV_GF_AMOUNT,
+              "gossip_funding.cuh and cln_sigverify.h must agree on the funding verdicts");
+
+// sv_verify_gossip_store_host, and with a table (else NULL) sv_verify_gossip_store_funding_host
+static int store_audit(sv_ctx* ctx, const uint8_t* store, size_t len, const uint8_t* chain_hash32,
+                       const sv_funding_table* table, uint64_t* rec_off, uint16_t* rec_type, int* rec_status,
+                       uint64_t* rec_holder, uint8_t* rec_funding, size_t rec_capacity, sv_gossip_store_summary* sum,
+                       sv_gossip_funding_summary* fsum) {
     if (store[0] >> 5) return fail(ctx, SV_ERR_ARG, "gossip_store major version is not 0", cudaSuccess);
     const auto t0 = std::chrono::steady_clock::now();
     gs_walk_end we;
@@ -2182,9 +2295,17 @@ extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, si
     dev_guard dg__;
     CK(dg__.enter(ctx->device));
     cudaStream_t st = ctx->stream;
-    ev_set ev;
+    ev_set ev, fev;
     if (ctx->profiling)
-        for (cudaEvent_t& e : ev.e) CK(cudaEventCreate(&e));
+        for (int i = 0; i < 4; i++) {
+            CK(cudaEventCreate(&ev.e[i]));
+            if (table) CK(cudaEventCreate(&fev.e[i]));
+        }
+    funding_stage F;
+    if (table) {
+        int rc = funding_stage_run(ctx, table, F, fev);
+        if (rc) return rc;
+    }
     // the store is staged in a buffer of its own, freed on return: a store can be hundreds of MB
     dev_buf<> d_store, t_live;
     const size_t live_bytes = live_off.size() * 8 + 16;
@@ -2220,8 +2341,27 @@ extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, si
         cut = we.no_amount;
         cut_status = GS_ST_NO_AMOUNT;
     }
+    // the funding verdicts of the reached announcements whose status is 0
+    std::vector<u8> fund;
+    if (table) {
+        std::vector<u32> cand;
+        for (size_t m = 0; m < P.n_msgs; m++)
+            if (mrec[m] < cut && rec[mrec[m]].type == 256 && mstatus[m] == 0) cand.push_back((u32)m);
+        dev_buf<> t_fund;
+        const size_t fb = P.n_msgs + 16 + 4 * cand.size();
+        rc = t_fund.reserve(ctx, fb, fb);
+        if (rc) return rc;
+        u8* d_fund = t_fund;
+        rc = funding_run(ctx, d_store, len, P.d_moff, P.n_msgs, cand, F, d_fund, t_fund.at<u32>((P.n_msgs + 15) / 16 * 16), fev);
+        if (rc) return rc;
+        fund.resize(P.n_msgs);
+        if (P.n_msgs) CK(cudaMemcpyAsync(fund.data(), d_fund, P.n_msgs, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+    }
     sv_gossip_store_summary S;
     memset(&S, 0, sizeof S);
+    sv_gossip_funding_summary FS;
+    memset(&FS, 0, sizeof FS);
     S.version = store[0];
     S.stop = cut_status ? cut_status : we.stop;
     S.end_offset = cut_status ? rec[cut].off : we.end;
@@ -2249,6 +2389,11 @@ extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, si
         rec_type[r] = (uint16_t)t;
         rec_status[r] = s;
         if (rec_holder) rec_holder[r] = h;
+        if (table) {
+            const u8 v = m != GS_NONE && !(cut_status && r >= cut) ? fund[m] : (u8)GF_NONE;
+            rec_funding[r] = v;
+            funding_count(FS, v);
+        }
         if (m != GS_NONE && s <= 4 && !(cut_status && r >= cut)) {
             S.good += s == 0; S.bad_signature += s >= 1 && s <= 4; S.malformed += s == -1; S.no_channel += s == -2;
             S.wrong_chain += s == -3; S.bad_order += s == -4;
@@ -2257,9 +2402,33 @@ extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, si
         S.not_reached += s == GS_ST_NOT_REACHED;
     }
     *sum = S;
+    if (table) *fsum = FS;
     ctx->gs_ms[0] = walk_ms;
     if (ev.e[0])
         for (int i = 0; i < 3; i++) CK(cudaEventElapsedTime(&ctx->gs_ms[1 + i], ev.e[i], ev.e[i + 1]));
+    return funding_timing(ctx, fev);
+}
+extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, size_t len, const uint8_t* chain_hash32,
+                                           uint64_t* rec_off, uint16_t* rec_type, int* rec_status, uint64_t* rec_holder,
+                                           size_t rec_capacity, sv_gossip_store_summary* sum) {
+    if (!ctx || !store || len < 1 || !sum || (rec_capacity && (!rec_off || !rec_type || !rec_status))) return SV_ERR_ARG;
+    return store_audit(ctx, store, len, chain_hash32, nullptr, rec_off, rec_type, rec_status, rec_holder, nullptr,
+                       rec_capacity, sum, nullptr);
+}
+extern "C" int sv_verify_gossip_store_funding_host(sv_ctx* ctx, const uint8_t* store, size_t len,
+                                                   const uint8_t* chain_hash32, const sv_funding_table* table,
+                                                   uint64_t* rec_off, uint16_t* rec_type, int* rec_status,
+                                                   uint64_t* rec_holder, uint8_t* rec_funding, size_t rec_capacity,
+                                                   sv_gossip_store_summary* sum, sv_gossip_funding_summary* fsum) {
+    if (!ctx || !store || len < 1 || !sum || !fsum || !funding_table_ok(table) ||
+        (rec_capacity && (!rec_off || !rec_type || !rec_status || !rec_funding)))
+        return SV_ERR_ARG;
+    return store_audit(ctx, store, len, chain_hash32, table, rec_off, rec_type, rec_status, rec_holder, rec_funding,
+                       rec_capacity, sum, fsum);
+}
+extern "C" int sv_get_last_gossip_funding_timing(sv_ctx* ctx, float* ms2) {
+    if (!ctx || !ctx->profiling || !ms2) return SV_ERR_ARG;
+    for (int i = 0; i < 2; i++) ms2[i] = ctx->gf_ms[i];
     return SV_OK;
 }
 // where the last sv_verify_gossip_store_host call spent its time (profiling mode): host header walk, H2D copy of the store,
@@ -2277,11 +2446,11 @@ extern "C" size_t sv_gossip_prune_count(const uint8_t* store, size_t len) {
     return (size_t)gs_walk(store, len, [](const gs_rec&) {}, &we, true);
 }
 
-extern "C" int sv_prune_gossip_store_host(sv_ctx* ctx, const uint8_t* store, size_t len, const uint8_t* chain_hash32,
-                                          uint8_t* out, uint64_t* rec_off, uint16_t* rec_type, int* rec_status,
-                                          uint8_t* rec_pruned, size_t rec_capacity, sv_gossip_prune_summary* sum) {
-    if (!ctx || !store || !out || len < 1 || !sum || (rec_capacity && (!rec_off || !rec_type || !rec_status || !rec_pruned)))
-        return SV_ERR_ARG;
+// sv_prune_gossip_store_host, and with a table (else NULL) sv_prune_gossip_store_funding_host
+static int store_prune(sv_ctx* ctx, const uint8_t* store, size_t len, const uint8_t* chain_hash32,
+                       const sv_funding_table* table, uint8_t* out, uint64_t* rec_off, uint16_t* rec_type, int* rec_status,
+                       uint8_t* rec_pruned, uint8_t* rec_funding, size_t rec_capacity, sv_gossip_prune_summary* sum,
+                       sv_gossip_funding_summary* fsum) {
     if (store[0] >> 5) return fail(ctx, SV_ERR_ARG, "gossip_store major version is not 0", cudaSuccess);
     const auto t0 = std::chrono::steady_clock::now();
     gs_walk_end we;
@@ -2304,9 +2473,17 @@ extern "C" int sv_prune_gossip_store_host(sv_ctx* ctx, const uint8_t* store, siz
     dev_guard dg__;
     CK(dg__.enter(ctx->device));
     cudaStream_t st = ctx->stream;
-    ev_set ev;
+    ev_set ev, fev;
     if (ctx->profiling)
-        for (cudaEvent_t& e : ev.e) CK(cudaEventCreate(&e));
+        for (int i = 0; i < 4; i++) {
+            CK(cudaEventCreate(&ev.e[i]));
+            if (table) CK(cudaEventCreate(&fev.e[i]));
+        }
+    funding_stage F;
+    if (table) {
+        int rc = funding_stage_run(ctx, table, F, fev);
+        if (rc) return rc;
+    }
     dev_buf<> d_store, t_live;
     const size_t nlive = live_off.size(), live_bytes = nlive * 9 + 16;
     int rc = d_store.reserve(ctx, len, len);
@@ -2330,24 +2507,36 @@ extern "C" int sv_prune_gossip_store_host(sv_ctx* ctx, const uint8_t* store, siz
     rc = store_pass_run(ctx, d_store, len, chain_hash32, rec, nrec, skip.data(), n_upd, P, ev.e[1]);
     if (rc) return rc;
     const size_t n_msgs = P.n_msgs, nev = P.nev, items = P.items;
-    std::vector<u8> reason(n_msgs, SV_GP_KEPT);
+    std::vector<u8> reason(n_msgs, SV_GP_KEPT), fund(table ? n_msgs : 0, GF_NONE);
     u32 n_moved = 0;
     if (n_msgs) {
+        // the funding verdicts of the announcements whose first-round status is 0: the refused ones join rule 2
+        std::vector<u32> cand;
+        if (table)
+            for (size_t m = 0; m < n_msgs; m++)
+                if (rec[P.mrec[m]].type == 256 && P.mstatus[m] == 0) cand.push_back((u32)m);
         // second round: the deletions of the first, the table again over the sorted events with those announcements
         // masked out, and the updates whose holder changed verified again under their new signer
         slab_layout L;
         const size_t o_reason = L.take(n_msgs), o_holder2 = L.take(4 * n_msgs), o_sig2 = L.take(33 * n_msgs),
-                     o_ok2 = L.take(nev), o_list = L.take(4 * (n_upd + 1)), o_keyok = L.take(n_upd);
+                     o_ok2 = L.take(nev), o_list = L.take(4 * (n_upd + 1)), o_keyok = L.take(n_upd),
+                     o_fund = L.take(table ? n_msgs : 0), o_cand = L.take(4 * cand.size());
         dev_buf<> s2;
         rc = s2.reserve(ctx, L.size, L.size);
         if (rc) return rc;
-        u8 *d_reason = s2 + o_reason, *d_sig2 = s2 + o_sig2, *d_ok2 = s2 + o_ok2, *d_keyok = s2 + o_keyok;
+        u8 *d_reason = s2 + o_reason, *d_sig2 = s2 + o_sig2, *d_ok2 = s2 + o_ok2, *d_keyok = s2 + o_keyok,
+           *d_fund = table ? s2 + o_fund : nullptr;
         u32 *d_holder2 = s2.at<u32>(o_holder2), *d_list = s2.at<u32>(o_list);
+        if (table) {
+            rc = funding_run(ctx, d_store, len, P.d_moff, n_msgs, cand, F, d_fund, s2.at<u32>(o_cand), fev);
+            if (rc) return rc;
+            CK(cudaMemcpyAsync(fund.data(), d_fund, n_msgs, cudaMemcpyDeviceToHost, st));
+        }
         CK(cudaMemsetAsync(d_holder2, 0xFF, 4 * n_msgs, st));
         CK(cudaMemsetAsync(d_list, 0, 4, st));
         const size_t nmark = n_msgs > nev ? n_msgs : nev;
         k_prune_mark<<<(unsigned)((nmark + 255) / 256), 256, 0, st>>>(d_store, P.d_moff, P.d_status, n_msgs, P.d_ekind,
-                                                                     P.d_emsg, P.d_ok, nev, d_reason, d_ok2);
+                                                                     P.d_emsg, P.d_ok, nev, d_fund, d_reason, d_ok2);
         ctx->launches += 1;
         if (nev) {
             k_store_resolve<<<(unsigned)((nev + 127) / 128), 128, 0, st>>>(d_store, P.d_key2, P.d_val2, d_ok2, P.d_ekind,
@@ -2418,8 +2607,10 @@ extern "C" int sv_prune_gossip_store_host(sv_ctx* ctx, const uint8_t* store, siz
     S.end_offset = cut < nrec ? rec[cut].off : we.end;
     S.records = nrec;
     S.reverified = n_moved;
-    uint64_t* per_reason[9] = {nullptr, &S.bad_crc, &S.truncated, &S.message, &S.redundant, &S.no_channel,
-                               &S.signature, &S.amount, &S.unknown};
+    sv_gossip_funding_summary FS;
+    memset(&FS, 0, sizeof FS);
+    uint64_t* per_reason[10] = {nullptr, &S.bad_crc, &S.truncated, &S.message, &S.redundant, &S.no_channel,
+                                &S.signature, &S.amount, &S.unknown, &FS.deleted};
     for (size_t r = 0; r < nrec; r++) {
         const u32 t = rec[r].type, m = P.msg_of[r];
         int s = rec[r].status;
@@ -2435,12 +2626,37 @@ extern "C" int sv_prune_gossip_store_host(sv_ctx* ctx, const uint8_t* store, siz
         rec_status[r] = s;
         rec_pruned[r] = why;
         if (why) { S.pruned++; (*per_reason[why])++; }
+        if (table) {
+            const u8 v = r < cut && m != GS_NONE ? fund[m] : (u8)GF_NONE;
+            rec_funding[r] = v;
+            funding_count(FS, v);
+        }
     }
     *sum = S;
+    if (table) *fsum = FS;
     ctx->gp_ms[0] = walk_ms;
     if (ev.e[0])
         for (int i = 0; i < 3; i++) CK(cudaEventElapsedTime(&ctx->gp_ms[1 + i], ev.e[i], ev.e[i + 1]));
-    return SV_OK;
+    return funding_timing(ctx, fev);
+}
+extern "C" int sv_prune_gossip_store_host(sv_ctx* ctx, const uint8_t* store, size_t len, const uint8_t* chain_hash32,
+                                          uint8_t* out, uint64_t* rec_off, uint16_t* rec_type, int* rec_status,
+                                          uint8_t* rec_pruned, size_t rec_capacity, sv_gossip_prune_summary* sum) {
+    if (!ctx || !store || !out || len < 1 || !sum || (rec_capacity && (!rec_off || !rec_type || !rec_status || !rec_pruned)))
+        return SV_ERR_ARG;
+    return store_prune(ctx, store, len, chain_hash32, nullptr, out, rec_off, rec_type, rec_status, rec_pruned, nullptr,
+                       rec_capacity, sum, nullptr);
+}
+extern "C" int sv_prune_gossip_store_funding_host(sv_ctx* ctx, const uint8_t* store, size_t len,
+                                                  const uint8_t* chain_hash32, const sv_funding_table* table, uint8_t* out,
+                                                  uint64_t* rec_off, uint16_t* rec_type, int* rec_status,
+                                                  uint8_t* rec_pruned, uint8_t* rec_funding, size_t rec_capacity,
+                                                  sv_gossip_prune_summary* sum, sv_gossip_funding_summary* fsum) {
+    if (!ctx || !store || !out || len < 1 || !sum || !fsum || !funding_table_ok(table) ||
+        (rec_capacity && (!rec_off || !rec_type || !rec_status || !rec_pruned || !rec_funding)))
+        return SV_ERR_ARG;
+    return store_prune(ctx, store, len, chain_hash32, table, out, rec_off, rec_type, rec_status, rec_pruned, rec_funding,
+                       rec_capacity, sum, fsum);
 }
 extern "C" int sv_get_last_gossip_prune_timing(sv_ctx* ctx, float* ms4) {
     if (!ctx || !ctx->profiling || !ms4) return SV_ERR_ARG;

@@ -64,6 +64,32 @@ GP_KEPT, GP_BAD_CRC, GP_TRUNCATED, GP_MESSAGE, GP_REDUNDANT, GP_NO_CHANNEL, GP_S
 GP_REASONS = ("kept", "bad_crc", "truncated", "message", "redundant", "no_channel", "signature", "amount", "unknown")
 
 
+class SvFundingTable(ctypes.Structure):
+    """sv_funding_table (include/cln_sigverify.h)"""
+    _fields_ = [("scid", ctypes.c_void_p), ("satoshis", ctypes.c_void_p), ("script34", ctypes.c_void_p),
+                ("n_outputs", ctypes.c_size_t), ("blocks", ctypes.c_void_p), ("n_blocks", ctypes.c_size_t)]
+
+
+class SvGossipFundingSummary(ctypes.Structure):
+    """sv_gossip_funding_summary (include/cln_sigverify.h)"""
+    _fields_ = [(f, ctypes.c_uint64) for f in ("checked", "funded", "unchecked", "no_txout", "script", "amount", "dying",
+                                               "deleted")]
+
+
+# the funding verdict of a channel_announcement (include/cln_sigverify.h SV_GF_*; 0 = none); GP_FUNDING: the prune's
+# reason for deleting an announcement whose verdict is NO_TXOUT, SCRIPT or AMOUNT
+GF_NONE, GF_FUNDED, GF_UNCHECKED, GF_DYING, GF_NO_TXOUT, GF_SCRIPT, GF_AMOUNT = range(7)
+GP_FUNDING = 9
+
+
+def _funding_table(funding):
+    """the sv_funding_table of a lightning_b200.funding.FundingTable (its arrays stay referenced by the table)"""
+    t = SvFundingTable(funding.scid.ctypes.data, funding.satoshis.ctypes.data, funding.script.ctypes.data, len(funding),
+                       funding.blocks.ctypes.data, funding.blocks.size)
+    t._keep = funding
+    return t
+
+
 class SvInfo(ctypes.Structure):
     _fields_ = [("device", ctypes.c_int), ("sm_count", ctypes.c_int), ("main_block", ctypes.c_int),
                 ("main_grid", ctypes.c_int), ("main_regs", ctypes.c_int), ("gtable_bytes", ctypes.c_size_t),
@@ -99,6 +125,13 @@ def load_library():
     lib.sv_gossip_prune_count.restype = sz
     lib.sv_prune_gossip_store_host.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp, vp, sz, ctypes.POINTER(SvGossipPruneSummary)]
     lib.sv_get_last_gossip_prune_timing.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
+    lib.sv_verify_gossip_store_funding_host.argtypes = [vp, vp, sz, vp, ctypes.POINTER(SvFundingTable), vp, vp, vp, vp, vp,
+                                                        sz, ctypes.POINTER(SvGossipStoreSummary),
+                                                        ctypes.POINTER(SvGossipFundingSummary)]
+    lib.sv_prune_gossip_store_funding_host.argtypes = [vp, vp, sz, vp, ctypes.POINTER(SvFundingTable), vp, vp, vp, vp, vp,
+                                                       vp, sz, ctypes.POINTER(SvGossipPruneSummary),
+                                                       ctypes.POINTER(SvGossipFundingSummary)]
+    lib.sv_get_last_gossip_funding_timing.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
     lib.sv_prune_gossip_store_fd.argtypes = [vp, i, ctypes.c_uint64, vp, ctypes.POINTER(SvGossipPruneSummary)]
     lib.sv_repair_gossip_store_fd.argtypes = [vp, i, ctypes.c_uint64, vp, ctypes.POINTER(SvGossipPruneSummary),
                                               ctypes.POINTER(ctypes.c_uint64)]
@@ -268,13 +301,16 @@ class SigVerifier:
         """updates the last gossip burst re-resolved in its repair round (their first candidate announcement failed)"""
         return int(self.lib.sv_last_gossip_repairs(self._ctx))
 
-    def verify_gossip_store(self, store, chain_hash=None, capacity=None):
+    def verify_gossip_store(self, store, chain_hash=None, capacity=None, funding=None):
         """A whole gossip_store (bytes, version byte included), walked as gossmap's map_catchup walks it, every record
         checksum and every signature checked on the device.  Returns (rec_off uint64, rec_type uint16, rec_status int32,
         rec_holder uint64, summary dict): one entry per record the walk reads; rec_status is a signature status for
         256/257/258 (0, 1..4, -1, -2 no channel, and with chain_hash -3 / -4) or a GS_* record status; rec_holder is the
         header offset of the announcement holding the channel (updates, redundant announcements), else GS_NO_HOLDER.
-        capacity: entries to provide (default: sv_gossip_store_count)."""
+        capacity: entries to provide (default: sv_gossip_store_count).
+        funding: a lightning_b200.funding.FundingTable, or None.  With a table every announcement is also checked against
+        lightningd's funding outputs (sv_verify_gossip_store_funding_host), and the call returns two more items:
+        rec_funding uint8 (GF_* verdict per record) and the funding summary dict."""
         buf = np.frombuffer(bytes(store), dtype=np.uint8)
         chain = None
         if chain_hash is not None:
@@ -287,12 +323,21 @@ class SigVerifier:
         status = np.zeros(max(n, 1), np.int32)
         holder = np.zeros(max(n, 1), np.uint64)
         s = SvGossipStoreSummary()
-        self._check(self.lib.sv_verify_gossip_store_host(
-            self._ctx, buf.ctypes.data, buf.size, chain.ctypes.data if chain is not None else None, off.ctypes.data,
-            typ.ctypes.data, status.ctypes.data, holder.ctypes.data, n, ctypes.byref(s)), "sv_verify_gossip_store_host")
+        if funding is None:
+            self._check(self.lib.sv_verify_gossip_store_host(
+                self._ctx, buf.ctypes.data, buf.size, chain.ctypes.data if chain is not None else None, off.ctypes.data,
+                typ.ctypes.data, status.ctypes.data, holder.ctypes.data, n, ctypes.byref(s)), "sv_verify_gossip_store_host")
+        else:
+            fund, fs, table = np.zeros(max(n, 1), np.uint8), SvGossipFundingSummary(), _funding_table(funding)
+            self._check(self.lib.sv_verify_gossip_store_funding_host(
+                self._ctx, buf.ctypes.data, buf.size, chain.ctypes.data if chain is not None else None, ctypes.byref(table),
+                off.ctypes.data, typ.ctypes.data, status.ctypes.data, holder.ctypes.data, fund.ctypes.data, n,
+                ctypes.byref(s), ctypes.byref(fs)), "sv_verify_gossip_store_funding_host")
         summary = {f: getattr(s, f) for f, _ in SvGossipStoreSummary._fields_}
         k = s.records
-        return off[:k], typ[:k], status[:k], holder[:k], summary
+        if funding is None:
+            return off[:k], typ[:k], status[:k], holder[:k], summary
+        return off[:k], typ[:k], status[:k], holder[:k], summary, fund[:k], {f: getattr(fs, f) for f, _ in fs._fields_}
 
     def last_gossip_store_timing(self):
         """(header walk, H2D, checksums, verification) in ms of the last verify_gossip_store (profiling mode)"""
@@ -300,12 +345,16 @@ class SigVerifier:
         self._check(self.lib.sv_get_last_gossip_store_timing(self._ctx, ms), "sv_get_last_gossip_store_timing")
         return tuple(ms)
 
-    def prune_gossip_store(self, store, chain_hash=None, capacity=None):
+    def prune_gossip_store(self, store, chain_hash=None, capacity=None, funding=None):
         """Mark every record of a gossip_store that gossmap should not trust as deleted (flag bit 0x8000), so that
         gossipd's strict load accepts the store and keeps the rest.  Returns (pruned_bytes, records, summary): the store
         with those bits set (same length; the input is not changed), records = (rec_off uint64, rec_type uint16,
         rec_status int32 (the first-round status), rec_pruned uint8 (GP_* reason, 0 = kept)), and the summary dict with
-        the deletions per reason.  capacity: entries to provide (default: sv_gossip_prune_count)."""
+        the deletions per reason.  capacity: entries to provide (default: sv_gossip_prune_count).
+        funding: a lightning_b200.funding.FundingTable, or None.  With a table the announcements gossipd would have
+        refused for their funding output are deleted too (GP_FUNDING, sv_prune_gossip_store_funding_host; summary
+        "pruned" counts them), and the call returns two more items: rec_funding uint8 (GF_* verdict per record) and
+        the funding summary dict ("deleted": the funding deletions)."""
         buf = np.frombuffer(bytes(store), dtype=np.uint8)
         chain = None
         if chain_hash is not None:
@@ -319,13 +368,23 @@ class SigVerifier:
         status = np.zeros(max(n, 1), np.int32)
         pruned = np.zeros(max(n, 1), np.uint8)
         s = SvGossipPruneSummary()
-        self._check(self.lib.sv_prune_gossip_store_host(
-            self._ctx, buf.ctypes.data, buf.size, chain.ctypes.data if chain is not None else None, out.ctypes.data,
-            off.ctypes.data, typ.ctypes.data, status.ctypes.data, pruned.ctypes.data, n, ctypes.byref(s)),
-            "sv_prune_gossip_store_host")
+        if funding is None:
+            self._check(self.lib.sv_prune_gossip_store_host(
+                self._ctx, buf.ctypes.data, buf.size, chain.ctypes.data if chain is not None else None, out.ctypes.data,
+                off.ctypes.data, typ.ctypes.data, status.ctypes.data, pruned.ctypes.data, n, ctypes.byref(s)),
+                "sv_prune_gossip_store_host")
+        else:
+            fund, fs, table = np.zeros(max(n, 1), np.uint8), SvGossipFundingSummary(), _funding_table(funding)
+            self._check(self.lib.sv_prune_gossip_store_funding_host(
+                self._ctx, buf.ctypes.data, buf.size, chain.ctypes.data if chain is not None else None, ctypes.byref(table),
+                out.ctypes.data, off.ctypes.data, typ.ctypes.data, status.ctypes.data, pruned.ctypes.data, fund.ctypes.data,
+                n, ctypes.byref(s), ctypes.byref(fs)), "sv_prune_gossip_store_funding_host")
         summary = {f: getattr(s, f) for f, _ in SvGossipPruneSummary._fields_}
         k = s.records
-        return out[:buf.size].tobytes(), (off[:k], typ[:k], status[:k], pruned[:k]), summary
+        if funding is None:
+            return out[:buf.size].tobytes(), (off[:k], typ[:k], status[:k], pruned[:k]), summary
+        return (out[:buf.size].tobytes(), (off[:k], typ[:k], status[:k], pruned[:k]), summary, fund[:k],
+                {f: getattr(fs, f) for f, _ in fs._fields_})
 
     def prune_gossip_store_fd(self, fd, length, chain_hash=None):
         """prune_gossip_store on a FILE, in place (sv_prune_gossip_store_fd): the store is bytes [0, length) of fd, a
@@ -373,6 +432,12 @@ class SigVerifier:
         """(header walk, first round, second round, flag write) in ms of the last prune_gossip_store (profiling mode)"""
         ms = (ctypes.c_float * 4)()
         self._check(self.lib.sv_get_last_gossip_prune_timing(self._ctx, ms), "sv_get_last_gossip_prune_timing")
+        return tuple(ms)
+
+    def last_gossip_funding_timing(self):
+        """(table staging and sort, k_store_funding) in ms of the last funding call (profiling mode)"""
+        ms = (ctypes.c_float * 2)()
+        self._check(self.lib.sv_get_last_gossip_funding_timing(self._ctx, ms), "sv_get_last_gossip_funding_timing")
         return tuple(ms)
 
     def verify_samekey(self, kind, key, msg32, sig64):
