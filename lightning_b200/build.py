@@ -31,6 +31,8 @@ NVCC_FLAGS = [
 # gcc flags of the plain-C parts: the drop-in (linked into the library) and the verifier subdaemon
 DROPIN_CFLAGS = ["-O2", "-fPIC", "-Wall", "-Wextra", "-std=c11"]
 DAEMON_CFLAGS = ["-O2", "-Wall", "-Wextra", "-std=c11", "-pthread"]
+# g++ line of the host build of the kernel headers (tests only; tests/invalid_curve.py builds altered copies with it)
+HOST_EMUL_CXX = ["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-pthread", "-Wall", "-Wno-unused-function"]
 
 
 def _newer(target, sources):
@@ -105,7 +107,7 @@ def build_host_emul(force=False):
     srcs = _sources(CSRC, (".cuh",)) + src
     if not force and _newer(EMUL, srcs):
         return EMUL
-    cmd = ["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-pthread", "-Wall", "-Wno-unused-function", "-o", EMUL] + src
+    cmd = HOST_EMUL_CXX + ["-o", EMUL] + src
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("g++ (host_emul) failed:\n" + r.stdout + r.stderr)
