@@ -132,6 +132,40 @@ static uint64_t print_funding(const char *what, const sv_gossip_funding_summary 
     return g->no_txout + g->script + g->amount;
 }
 
+/* one audit of a store: each record's offset, type, status and (with a table) funding verdict, and the summaries */
+typedef struct {
+    size_t n;
+    uint64_t *off;
+    uint16_t *type;
+    int *status;
+    uint8_t *fund;
+    sv_gossip_store_summary s;
+    sv_gossip_funding_summary g;
+} audit_result;
+
+/* sv_verify_gossip_store_host, or with a table sv_verify_gossip_store_funding_host; returns 0, or 3 (the exit code)
+ * after saying why it failed */
+static int audit(sv_ctx *ctx, const uint8_t *store, size_t len, const uint8_t *chain, const sv_funding_table *table,
+                 audit_result *a) {
+    const size_t n = a->n = sv_gossip_store_count(store, len);
+    a->off = malloc((n ? n : 1) * sizeof *a->off);
+    a->type = malloc((n ? n : 1) * sizeof *a->type);
+    a->status = malloc((n ? n : 1) * sizeof *a->status);
+    a->fund = malloc(n ? n : 1);
+    if (!a->off || !a->type || !a->status || !a->fund) { fprintf(stderr, "out of memory\n"); return 3; }
+    int rc = table ? sv_verify_gossip_store_funding_host(ctx, store, len, chain, table, a->off, a->type, a->status, NULL,
+                                                         a->fund, n, &a->s, &a->g)
+                   : sv_verify_gossip_store_host(ctx, store, len, chain, a->off, a->type, a->status, NULL, n, &a->s);
+    if (rc != SV_OK) {
+        fprintf(stderr, "%s: %d %s\n", table ? "sv_verify_gossip_store_funding_host" : "sv_verify_gossip_store_host", rc,
+                sv_last_error(ctx));
+        return 3;
+    }
+    return 0;
+}
+
+static void audit_free(audit_result *a) { free(a->off); free(a->type); free(a->status); free(a->fund); }
+
 /* --prune: write the pruned copy (cut_tail: without its torn tail), report it, audit it; returns the exit code */
 static int prune(sv_ctx *ctx, const char *path, const uint8_t *store, size_t len, const uint8_t *chain, const char *outp,
                  int cut_tail, const sv_funding_table *table) {
@@ -165,26 +199,16 @@ static int prune(sv_ctx *ctx, const char *path, const uint8_t *store, size_t len
     if (table) print_funding(path, &g);
     if (cut_tail) printf("  torn tail: %zu bytes cut, %s ends at %zu\n", len - wlen, outp, wlen);
     len = wlen;
-    size_t m = sv_gossip_store_count(out, len);
-    uint64_t *aoff = malloc((m ? m : 1) * sizeof *aoff);
-    uint16_t *atype = malloc((m ? m : 1) * sizeof *atype);
-    int *astatus = malloc((m ? m : 1) * sizeof *astatus);
-    uint8_t *afund = malloc(m ? m : 1);
-    if (!aoff || !atype || !astatus || !afund) { fprintf(stderr, "out of memory\n"); return 3; }
-    sv_gossip_store_summary s;
-    rc = table ? sv_verify_gossip_store_funding_host(ctx, out, len, chain, table, aoff, atype, astatus, NULL, afund, m, &s, &g)
-               : sv_verify_gossip_store_host(ctx, out, len, chain, aoff, atype, astatus, NULL, m, &s);
-    if (rc != SV_OK) {
-        fprintf(stderr, "%s: %d %s\n", table ? "sv_verify_gossip_store_funding_host" : "sv_verify_gossip_store_host", rc,
-                sv_last_error(ctx));
-        return 3;
-    }
-    const uint64_t refused = table ? print_funding(outp, &g) : 0;
+    audit_result a;
+    if (audit(ctx, out, len, chain, table, &a)) return 3;
+    const sv_gossip_store_summary s = a.s;
+    const uint64_t refused = table ? print_funding(outp, &a.g) : 0;
     const int clean = s.stop == SV_GS_EOF && s.end_offset == len && !s.bad_signature && !s.malformed && !s.no_channel &&
                       !s.wrong_chain && !s.bad_order && !s.redundant_announcements && !s.unknown && !refused;
     printf("%s: %s (%" PRIu64 " good messages, %" PRIu64 " deleted records)\n", outp,
            clean ? "clean" : "NOT clean", s.good, s.deleted);
-    free(off); free(type); free(status); free(why); free(fund); free(out); free(aoff); free(atype); free(astatus); free(afund);
+    free(off); free(type); free(status); free(why); free(fund); free(out);
+    audit_free(&a);
     return clean ? 0 : 1;
 }
 
@@ -237,47 +261,31 @@ int main(int argc, char **argv) {
     }
     fclose(f);
     if (!store || len == 0) { fprintf(stderr, "%s: empty or unreadable\n", path); return 3; }
+    sv_ctx *ctx = NULL;
+    if (sv_create(&ctx, device) != SV_OK) { fprintf(stderr, "engine: %s\n", sv_last_error(NULL)); return 3; }
     if (prune_out) {
-        sv_ctx *pctx = NULL;
-        if (sv_create(&pctx, device) != SV_OK) { fprintf(stderr, "engine: %s\n", sv_last_error(NULL)); return 3; }
-        int code = prune(pctx, path, store, len, have_chain ? chain : NULL, prune_out, cut_tail, table);
-        sv_destroy(pctx);
+        int code = prune(ctx, path, store, len, have_chain ? chain : NULL, prune_out, cut_tail, table);
+        sv_destroy(ctx);
         free(store);
         return code;
     }
-
-    size_t n = sv_gossip_store_count(store, len);
-    uint64_t *off = malloc((n ? n : 1) * sizeof *off);
-    uint16_t *type = malloc((n ? n : 1) * sizeof *type);
-    int *status = malloc((n ? n : 1) * sizeof *status);
-    uint8_t *fund = malloc(n ? n : 1);
-    sv_ctx *ctx = NULL;
-    if (!off || !type || !status || !fund) { fprintf(stderr, "out of memory\n"); return 3; }
-    if (sv_create(&ctx, device) != SV_OK) { fprintf(stderr, "engine: %s\n", sv_last_error(NULL)); return 3; }
-    sv_gossip_store_summary s;
-    sv_gossip_funding_summary g;
-    int rc = table ? sv_verify_gossip_store_funding_host(ctx, store, len, have_chain ? chain : NULL, table, off, type, status,
-                                                         NULL, fund, n, &s, &g)
-                   : sv_verify_gossip_store_host(ctx, store, len, have_chain ? chain : NULL, off, type, status, NULL, n, &s);
-    if (rc != SV_OK) {
-        fprintf(stderr, "%s: %d %s\n", table ? "sv_verify_gossip_store_funding_host" : "sv_verify_gossip_store_host", rc,
-                sv_last_error(ctx));
-        sv_destroy(ctx);
-        return 3;
-    }
+    audit_result a;
+    int rc = audit(ctx, store, len, have_chain ? chain : NULL, table, &a);
     sv_destroy(ctx);
+    if (rc) return rc;
 
     int failing = 0;
-    for (size_t i = 0; i < n; i++) {
-        int st = status[i];
+    for (size_t i = 0; i < a.n; i++) {
+        int st = a.status[i];
         int bad = (st != 0 && st < SV_GS_DELETED) || st == SV_GS_BAD_CRC || st == SV_GS_TRUNCATED || st == SV_GS_NO_AMOUNT;
         if (bad) {
-            printf("record @%" PRIu64 " type %u: %d (%s)\n", off[i], type[i], st, status_name(st));
+            printf("record @%" PRIu64 " type %u: %d (%s)\n", a.off[i], a.type[i], st, status_name(st));
             failing += st < SV_GS_DELETED;
         }
-        if (table && fund[i] != SV_GF_NONE && fund[i] != SV_GF_FUNDED)
-            printf("record @%" PRIu64 " type %u: funding %s\n", off[i], type[i], funding_name[fund[i]]);
+        if (table && a.fund[i] != SV_GF_NONE && a.fund[i] != SV_GF_FUNDED)
+            printf("record @%" PRIu64 " type %u: funding %s\n", a.off[i], a.type[i], funding_name[a.fund[i]]);
     }
+    const sv_gossip_store_summary s = a.s;
     printf("gossip_store %s: version %u, %" PRIu64 " bytes, %" PRIu64 " records, walk stopped: %s at %" PRIu64 "\n", path,
            s.version, (uint64_t)len, s.records, s.stop ? status_name(s.stop) : "end of store", s.end_offset);
     if (s.stop == SV_GS_ENDED) printf("  gossip_store_ended: equivalent_offset %" PRIu64 "\n", s.ended_equivalent_offset);
@@ -288,8 +296,9 @@ int main(int argc, char **argv) {
            s.deleted, s.store_records, s.unknown, s.not_reached);
     printf("  %" PRIu64 " redundant announcements, %" PRIu64 " updates without a channel\n", s.redundant_announcements,
            s.updates_without_channel);
-    const uint64_t refused = table ? print_funding(path, &g) : 0;
-    free(store); free(off); free(type); free(status); free(fund);
+    const uint64_t refused = table ? print_funding(path, &a.g) : 0;
+    free(store);
+    audit_free(&a);
     if (s.stop == SV_GS_BAD_CRC || s.stop == SV_GS_TRUNCATED || s.stop == SV_GS_NO_AMOUNT) return 2;
     return failing || refused ? 1 : 0;
 }

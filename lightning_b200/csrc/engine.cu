@@ -584,16 +584,14 @@ __global__ void __launch_bounds__(128) k_gossip_status(const u8* blob, const u64
 }
 
 // ---- gossip_store (gossip_store.cuh): record checksums and the channel each update is signed for ---------------------
-// k_store_crc: one thread per live record the host walk read (header offsets), slice-by-8 tables in shared memory.
-// *first_bad = the lowest entry whose checksum fails: map_catchup stops there.
-__global__ void __launch_bounds__(256) k_store_crc(const u8* store, const u64* rec_off, size_t n, u32* first_bad) {
+// k_store_crc_flags: one thread per record the host walk listed (header offsets), slice-by-8 tables in shared memory;
+// bad[r] = 1 if its checksum fails
+__global__ void __launch_bounds__(256) k_store_crc_flags(const u8* store, const u64* rec_off, size_t n, u8* bad) {
     __shared__ u32 tab[2048];
     for (u32 i = threadIdx.x; i < 256; i += blockDim.x) gs_crc_fill(tab, i);
     __syncthreads();
     size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    u32 bad = (r < n && !gs_record_crc_ok(tab, store, rec_off[r])) ? (u32)r : 0xFFFFFFFFu;
-    bad = __reduce_min_sync(0xFFFFFFFFu, bad);
-    if ((threadIdx.x & 31) == 0 && bad != 0xFFFFFFFFu) atomicMin(first_bad, bad);
+    if (r < n) bad[r] = !gs_record_crc_ok(tab, store, rec_off[r]);
 }
 // one thread per channel event (announcement, delete_chan, update, listed by the host in store order): its scid as the
 // sort key and its own index as the value; an event whose reads would pass the end of the store (store_len) gets ok = 0
@@ -642,14 +640,6 @@ __global__ void __launch_bounds__(256) k_store_finish(const u8* store, const u64
 }
 
 // ---- gossip_store prune (sv_prune_gossip_store_host): the deletions, a second channel table and the flag writes ------
-// k_store_crc_flags: k_store_crc with a flag per record (bad[r] = 1 if its checksum fails) instead of the first bad one
-__global__ void __launch_bounds__(256) k_store_crc_flags(const u8* store, const u64* rec_off, size_t n, u8* bad) {
-    __shared__ u32 tab[2048];
-    for (u32 i = threadIdx.x; i < 256; i += blockDim.x) gs_crc_fill(tab, i);
-    __syncthreads();
-    size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r < n) bad[r] = !gs_record_crc_ok(tab, store, rec_off[r]);
-}
 // k_prune_mark: thread i < n_msgs turns message i's first-round status into its deletion (an announcement that is not 0,
 // an update that is -1 or -3: SV_GP_MESSAGE), and with a funding verdict per message (fund, else NULL) an announcement
 // gossipd would have refused for its txout (SV_GP_FUNDING); thread i < nev masks event i out of the second round if it
@@ -2070,7 +2060,7 @@ static_assert(GS_ST_DELETED == SV_GS_DELETED && GS_ST_STORE_RECORD == SV_GS_STOR
               "gossip_store.cuh and cln_sigverify.h must agree on the record statuses");
 
 struct ev_set {  // CUDA events of one call, destroyed on every exit path
-    cudaEvent_t e[4] = {};
+    cudaEvent_t e[6] = {};
     ~ev_set() { for (cudaEvent_t x : e) if (x) cudaEventDestroy(x); }
 };
 
@@ -2238,22 +2228,6 @@ static int funding_stage_run(sv_ctx* ctx, const sv_funding_table* tb, funding_st
 static bool funding_table_ok(const sv_funding_table* t) {
     return t && (!t->n_outputs || (t->scid && t->satoshis && t->script34)) && (!t->n_blocks || t->blocks);
 }
-// fund[m] (n_msgs bytes, device) = the verdict of each message listed in cand (host), GF_NONE for the others; ev: e[2],
-// e[3] around the kernel
-static int funding_run(sv_ctx* ctx, const u8* d_store, size_t len, const u64* d_moff, size_t n_msgs,
-                       const std::vector<u32>& cand, const funding_stage& F, u8* d_fund, u32* d_cand, const ev_set& ev) {
-    cudaStream_t st = ctx->stream;
-    CK(cudaMemsetAsync(d_fund, GF_NONE, n_msgs, st));
-    if (ev.e[2]) CK(cudaEventRecord(ev.e[2], st));
-    if (!cand.empty()) {
-        CK(cudaMemcpyAsync(d_cand, cand.data(), 4 * cand.size(), cudaMemcpyHostToDevice, st));
-        k_store_funding<<<(unsigned)((cand.size() + 127) / 128), 128, 0, st>>>(d_store, len, d_moff, d_cand, cand.size(),
-                                                                               F.t, d_fund);
-        ctx->launches += 1;
-    }
-    if (ev.e[3]) CK(cudaEventRecord(ev.e[3], st));
-    return SV_OK;
-}
 static void funding_count(sv_gossip_funding_summary& F, u8 v) {
     uint64_t* per[7] = {nullptr, &F.funded, &F.unchecked, &F.dying, &F.no_txout, &F.script, &F.amount};
     if (v == GF_NONE) return;
@@ -2273,68 +2247,133 @@ static_assert(GF_NONE == SV_GF_NONE && GF_FUNDED == SV_GF_FUNDED && GF_UNCHECKED
                   GF_AMOUNT == SV_GF_AMOUNT,
               "gossip_funding.cuh and cln_sigverify.h must agree on the funding verdicts");
 
+// What the audit and the prune share: gossmap's header walk (past_truncated: the prune's), the funding table staged
+// (with a table), the store staged in a buffer of its own (a store can be hundreds of MB) and the checksum of every live
+// record and of the ENDED record tested on the device.  ev (profiling mode): e[0] before the store's copy, e[1] after
+// it, e[2] after the checksums; e[3..5] are the caller's.  fev: the funding step's (funding_stage_run, store_funding_run).
+struct store_front {
+    dev_guard dg;  // the first member: the buffers below are freed on the context's device
+    std::vector<gs_rec> rec;
+    gs_walk_end we;
+    float walk_ms = 0;
+    ev_set ev, fev;
+    funding_stage F;
+    dev_buf<> d_store, d_crc;
+    std::vector<u8> bad;  // per record: 1 if its checksum was tested and failed
+};
+static int store_front_run(sv_ctx* ctx, const uint8_t* store, size_t len, const sv_funding_table* table,
+                           size_t rec_capacity, bool past_truncated, store_front& G) {
+    if (store[0] >> 5) return fail(ctx, SV_ERR_ARG, "gossip_store major version is not 0", cudaSuccess);
+    const auto t0 = std::chrono::steady_clock::now();
+    std::vector<gs_rec>& rec = G.rec;
+    rec.reserve(len / 256 + 16);
+    const size_t nrec = gs_walk(store, len, [&rec](const gs_rec& r) { rec.push_back(r); }, &G.we, past_truncated);
+    if (nrec > rec_capacity) return fail(ctx, SV_ERR_ARG, "rec_capacity is below the store's record count", cudaSuccess);
+    if (nrec >= 0xFFFFFFFFu) return fail(ctx, SV_ERR_ARG, "too many records", cudaSuccess);
+    // the records whose checksum map_catchup tests: every live one the walk reached, the ENDED record included
+    std::vector<u64> crc_off;
+    std::vector<u32> crc_rec;
+    for (size_t r = 0; r < nrec; r++)
+        if (rec[r].status == GS_LIVE || rec[r].status == GS_ST_ENDED) { crc_off.push_back(rec[r].off); crc_rec.push_back((u32)r); }
+    G.walk_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    CK(G.dg.enter(ctx->device));
+    cudaStream_t st = ctx->stream;
+    if (ctx->profiling)
+        for (int i = 0; i < 6; i++) {
+            CK(cudaEventCreate(&G.ev.e[i]));
+            if (table && i < 4) CK(cudaEventCreate(&G.fev.e[i]));
+        }
+    if (table) {
+        int rc = funding_stage_run(ctx, table, G.F, G.fev);
+        if (rc) return rc;
+    }
+    const size_t n = crc_off.size(), crc_bytes = n * 9 + 16;
+    int rc = G.d_store.reserve(ctx, len, len);
+    if (!rc) rc = G.d_crc.reserve(ctx, crc_bytes, crc_bytes);
+    if (rc) return rc;
+    u64* d_off = G.d_crc.at<u64>(0);
+    u8* d_bad = G.d_crc.at<u8>(n * 8);
+    const cudaEvent_t* ev = G.ev.e;
+    if (ev[0]) CK(cudaEventRecord(ev[0], st));
+    CK(cudaMemcpyAsync(G.d_store, store, len, cudaMemcpyHostToDevice, st));
+    if (n) CK(cudaMemcpyAsync(d_off, crc_off.data(), n * 8, cudaMemcpyHostToDevice, st));
+    if (ev[1]) CK(cudaEventRecord(ev[1], st));
+    if (n) {
+        k_store_crc_flags<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(G.d_store, d_off, n, d_bad);
+        ctx->launches += 1;
+    }
+    if (ev[2]) CK(cudaEventRecord(ev[2], st));
+    std::vector<u8> bad(n);
+    if (n) CK(cudaMemcpyAsync(bad.data(), d_bad, n, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    G.bad.assign(nrec, 0);
+    for (size_t k = 0; k < n; k++) G.bad[crc_rec[k]] = bad[k];
+    return SV_OK;
+}
+
+// The funding verdicts of P's announcements whose status is 0 and whose record lies before cut, GF_NONE for every other
+// message: in d_fund on the device (n_msgs bytes at its start, which k_prune_mark reads) and in fund on the host once the
+// stream is synchronised.  fev: e[2], e[3] around the kernel.
+static int store_funding_run(sv_ctx* ctx, const store_front& G, size_t len, const store_pass& P, size_t cut,
+                             dev_buf<>& d_fund, std::vector<u8>& fund) {
+    cudaStream_t st = ctx->stream;
+    const size_t n = P.n_msgs;
+    std::vector<u32> cand;
+    for (size_t m = 0; m < n; m++)
+        if (P.mrec[m] < cut && G.rec[P.mrec[m]].type == 256 && P.mstatus[m] == 0) cand.push_back((u32)m);
+    slab_layout L;
+    L.take(n);
+    const size_t o_cand = L.take(4 * cand.size());
+    int rc = d_fund.reserve(ctx, L.size, L.size);
+    if (rc) return rc;
+    u32* d_cand = d_fund.at<u32>(o_cand);
+    const cudaEvent_t* fev = G.fev.e;
+    CK(cudaMemsetAsync(d_fund, GF_NONE, n, st));
+    if (fev[2]) CK(cudaEventRecord(fev[2], st));
+    if (!cand.empty()) {
+        CK(cudaMemcpyAsync(d_cand, cand.data(), 4 * cand.size(), cudaMemcpyHostToDevice, st));
+        k_store_funding<<<(unsigned)((cand.size() + 127) / 128), 128, 0, st>>>(G.d_store, len, P.d_moff, d_cand, cand.size(),
+                                                                               G.F.t, d_fund);
+        ctx->launches += 1;
+    }
+    if (fev[3]) CK(cudaEventRecord(fev[3], st));
+    fund.resize(n);
+    if (n) CK(cudaMemcpyAsync(fund.data(), d_fund, n, cudaMemcpyDeviceToHost, st));
+    return SV_OK;
+}
+
+// gossmap's store-only records: a load passes over them; a record of any other type it does not know is unknown
+static bool gs_store_record(u32 t) {
+    return t == GS_CHANNEL_AMOUNT || t == GS_DELETE_CHAN || t == GS_CHAN_DYING || t == GS_UUID;
+}
+// a reached record's status: the walk's if it is not live, else GS_ST_BAD_CRC if its checksum failed, else its message's
+// status (m: its message in P), else GS_ST_STORE_RECORD or GS_ST_UNKNOWN
+static int store_status(const gs_rec& r, u8 bad, u32 m, const store_pass& P) {
+    if (r.status != GS_LIVE) return r.status;
+    if (bad) return GS_ST_BAD_CRC;
+    if (m != GS_NONE) return P.mstatus[m];
+    return gs_store_record(r.type) ? GS_ST_STORE_RECORD : GS_ST_UNKNOWN;
+}
+
 // sv_verify_gossip_store_host, and with a table (else NULL) sv_verify_gossip_store_funding_host
 static int store_audit(sv_ctx* ctx, const uint8_t* store, size_t len, const uint8_t* chain_hash32,
                        const sv_funding_table* table, uint64_t* rec_off, uint16_t* rec_type, int* rec_status,
                        uint64_t* rec_holder, uint8_t* rec_funding, size_t rec_capacity, sv_gossip_store_summary* sum,
                        sv_gossip_funding_summary* fsum) {
-    if (store[0] >> 5) return fail(ctx, SV_ERR_ARG, "gossip_store major version is not 0", cudaSuccess);
-    const auto t0 = std::chrono::steady_clock::now();
-    gs_walk_end we;
-    std::vector<gs_rec> rec;
-    rec.reserve(len / 256 + 16);
-    const size_t nrec = gs_walk(store, len, [&rec](const gs_rec& r) { rec.push_back(r); }, &we);
-    if (nrec > rec_capacity) return fail(ctx, SV_ERR_ARG, "rec_capacity is below the store's record count", cudaSuccess);
-    if (nrec >= 0xFFFFFFFFu) return fail(ctx, SV_ERR_ARG, "too many records", cudaSuccess);
-    // the records whose checksum map_catchup tests: every live one the walk reached, the ENDED record included
-    std::vector<u64> live_off;
-    std::vector<u32> live_rec;
-    for (size_t r = 0; r < nrec; r++)
-        if (rec[r].status == GS_LIVE || rec[r].status == GS_ST_ENDED) { live_off.push_back(rec[r].off); live_rec.push_back((u32)r); }
-    const float walk_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    dev_guard dg__;
-    CK(dg__.enter(ctx->device));
-    cudaStream_t st = ctx->stream;
-    ev_set ev, fev;
-    if (ctx->profiling)
-        for (int i = 0; i < 4; i++) {
-            CK(cudaEventCreate(&ev.e[i]));
-            if (table) CK(cudaEventCreate(&fev.e[i]));
-        }
-    funding_stage F;
-    if (table) {
-        int rc = funding_stage_run(ctx, table, F, fev);
-        if (rc) return rc;
-    }
-    // the store is staged in a buffer of its own, freed on return: a store can be hundreds of MB
-    dev_buf<> d_store, t_live;
-    const size_t live_bytes = live_off.size() * 8 + 16;
-    int rc = d_store.reserve(ctx, len, len);
-    if (!rc) rc = t_live.reserve(ctx, live_bytes, live_bytes);
+    store_front G;
+    int rc = store_front_run(ctx, store, len, table, rec_capacity, false, G);
     if (rc) return rc;
-    u64* d_live = t_live.at<u64>(0);
-    u32* d_bad = t_live.at<u32>(live_off.size() * 8);
-    if (ev.e[0]) CK(cudaEventRecord(ev.e[0], st));
-    CK(cudaMemcpyAsync(d_store, store, len, cudaMemcpyHostToDevice, st));
-    if (!live_off.empty()) CK(cudaMemcpyAsync(d_live, live_off.data(), live_off.size() * 8, cudaMemcpyHostToDevice, st));
-    if (ev.e[1]) CK(cudaEventRecord(ev.e[1], st));
-    CK(cudaMemsetAsync(d_bad, 0xFF, 4, st));
-    if (!live_off.empty()) {
-        k_store_crc<<<(unsigned)((live_off.size() + 255) / 256), 256, 0, st>>>(d_store, d_live, live_off.size(), d_bad);
-        ctx->launches += 1;
-    }
-    if (ev.e[2]) CK(cudaEventRecord(ev.e[2], st));
-    u32 bad = 0xFFFFFFFFu;
-    CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    const std::vector<gs_rec>& rec = G.rec;
+    const size_t nrec = rec.size();
+    const gs_walk_end& we = G.we;
     // the walk ends at the first bad checksum: only the records before it are verified
-    size_t cut = bad < live_rec.size() ? live_rec[bad] : nrec;
-    int cut_status = bad < live_rec.size() ? GS_ST_BAD_CRC : 0;
+    size_t cut = 0;
+    while (cut < nrec && !G.bad[cut]) cut++;
+    int cut_status = cut < nrec ? GS_ST_BAD_CRC : 0;
     store_pass P;
-    rc = store_pass_run(ctx, d_store, len, chain_hash32, rec, cut, nullptr, 0, P, ev.e[3]);
+    rc = store_pass_run(ctx, G.d_store, len, chain_hash32, rec, cut, nullptr, 0, P, G.ev.e[3]);
     if (rc) return rc;
     const std::vector<u32>&msg_of = P.msg_of, &mrec = P.mrec, &holder = P.holder;
-    const std::vector<int>& mstatus = P.mstatus;
     // an announcement without room for its amount record stops the walk unless it is redundant (add_channel returns the
     // channel that already holds the scid before it looks for the amount)
     if (we.no_amount < cut && holder[msg_of[we.no_amount]] == GS_NONE) {
@@ -2342,21 +2381,12 @@ static int store_audit(sv_ctx* ctx, const uint8_t* store, size_t len, const uint
         cut_status = GS_ST_NO_AMOUNT;
     }
     // the funding verdicts of the reached announcements whose status is 0
+    dev_buf<> d_fund;
     std::vector<u8> fund;
     if (table) {
-        std::vector<u32> cand;
-        for (size_t m = 0; m < P.n_msgs; m++)
-            if (mrec[m] < cut && rec[mrec[m]].type == 256 && mstatus[m] == 0) cand.push_back((u32)m);
-        dev_buf<> t_fund;
-        const size_t fb = P.n_msgs + 16 + 4 * cand.size();
-        rc = t_fund.reserve(ctx, fb, fb);
+        rc = store_funding_run(ctx, G, len, P, cut, d_fund, fund);
         if (rc) return rc;
-        u8* d_fund = t_fund;
-        rc = funding_run(ctx, d_store, len, P.d_moff, P.n_msgs, cand, F, d_fund, t_fund.at<u32>((P.n_msgs + 15) / 16 * 16), fev);
-        if (rc) return rc;
-        fund.resize(P.n_msgs);
-        if (P.n_msgs) CK(cudaMemcpyAsync(fund.data(), d_fund, P.n_msgs, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
+        CK(cudaStreamSynchronize(ctx->stream));
     }
     sv_gossip_store_summary S;
     memset(&S, 0, sizeof S);
@@ -2368,45 +2398,36 @@ static int store_audit(sv_ctx* ctx, const uint8_t* store, size_t len, const uint
     S.records = nrec;
     for (size_t r = 0; r < nrec; r++) {
         const u32 t = rec[r].type, m = msg_of[r];
-        int s = rec[r].status;
+        const bool reached = !(cut_status && r >= cut);
+        const int s = reached ? store_status(rec[r], G.bad[r], m, P) : r == cut ? cut_status : GS_ST_NOT_REACHED;
         u64 h = ~(u64)0;
-        if (cut_status && r >= cut) {
-            s = r == cut ? cut_status : GS_ST_NOT_REACHED;
-        } else if (s == GS_LIVE) {
-            if (m != GS_NONE) {
-                s = mstatus[m];
-                if (holder[m] != GS_NONE) h = rec[mrec[holder[m]]].off;
-                S.redundant_announcements += t == 256 && holder[m] != GS_NONE;
-                S.updates_without_channel += t == 258 && len - rec[r].off - GS_HDR >= GS_UPD_READ && holder[m] == GS_NONE;
-            } else {
-                s = (t == GS_CHANNEL_AMOUNT || t == GS_DELETE_CHAN || t == GS_CHAN_DYING || t == GS_UUID) ? GS_ST_STORE_RECORD
-                                                                                                          : GS_ST_UNKNOWN;
-            }
-        } else if (s == GS_ST_ENDED && rec[r].len >= 10) {
-            for (int b = 0; b < 8; b++) S.ended_equivalent_offset = (S.ended_equivalent_offset << 8) | store[rec[r].off + GS_HDR + 2 + b];
+        if (reached && m != GS_NONE) {
+            if (holder[m] != GS_NONE) h = rec[mrec[holder[m]]].off;
+            S.redundant_announcements += t == 256 && holder[m] != GS_NONE;
+            S.updates_without_channel += t == 258 && len - rec[r].off - GS_HDR >= GS_UPD_READ && holder[m] == GS_NONE;
+            S.good += s == 0; S.bad_signature += s >= 1 && s <= 4; S.malformed += s == -1; S.no_channel += s == -2;
+            S.wrong_chain += s == -3; S.bad_order += s == -4;
         }
+        if (s == GS_ST_ENDED && rec[r].len >= 10)
+            for (int b = 0; b < 8; b++) S.ended_equivalent_offset = (S.ended_equivalent_offset << 8) | store[rec[r].off + GS_HDR + 2 + b];
         rec_off[r] = rec[r].off;
         rec_type[r] = (uint16_t)t;
         rec_status[r] = s;
         if (rec_holder) rec_holder[r] = h;
         if (table) {
-            const u8 v = m != GS_NONE && !(cut_status && r >= cut) ? fund[m] : (u8)GF_NONE;
+            const u8 v = reached && m != GS_NONE ? fund[m] : (u8)GF_NONE;
             rec_funding[r] = v;
             funding_count(FS, v);
-        }
-        if (m != GS_NONE && s <= 4 && !(cut_status && r >= cut)) {
-            S.good += s == 0; S.bad_signature += s >= 1 && s <= 4; S.malformed += s == -1; S.no_channel += s == -2;
-            S.wrong_chain += s == -3; S.bad_order += s == -4;
         }
         S.deleted += s == GS_ST_DELETED; S.store_records += s == GS_ST_STORE_RECORD; S.unknown += s == GS_ST_UNKNOWN;
         S.not_reached += s == GS_ST_NOT_REACHED;
     }
     *sum = S;
     if (table) *fsum = FS;
-    ctx->gs_ms[0] = walk_ms;
-    if (ev.e[0])
-        for (int i = 0; i < 3; i++) CK(cudaEventElapsedTime(&ctx->gs_ms[1 + i], ev.e[i], ev.e[i + 1]));
-    return funding_timing(ctx, fev);
+    ctx->gs_ms[0] = G.walk_ms;
+    if (G.ev.e[0])
+        for (int i = 0; i < 3; i++) CK(cudaEventElapsedTime(&ctx->gs_ms[1 + i], G.ev.e[i], G.ev.e[i + 1]));
+    return funding_timing(ctx, G.fev);
 }
 extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, size_t len, const uint8_t* chain_hash32,
                                            uint64_t* rec_off, uint16_t* rec_type, int* rec_status, uint64_t* rec_holder,
@@ -2451,87 +2472,44 @@ static int store_prune(sv_ctx* ctx, const uint8_t* store, size_t len, const uint
                        const sv_funding_table* table, uint8_t* out, uint64_t* rec_off, uint16_t* rec_type, int* rec_status,
                        uint8_t* rec_pruned, uint8_t* rec_funding, size_t rec_capacity, sv_gossip_prune_summary* sum,
                        sv_gossip_funding_summary* fsum) {
-    if (store[0] >> 5) return fail(ctx, SV_ERR_ARG, "gossip_store major version is not 0", cudaSuccess);
-    const auto t0 = std::chrono::steady_clock::now();
-    gs_walk_end we;
-    std::vector<gs_rec> rec;
-    rec.reserve(len / 256 + 16);
-    const size_t nrec = gs_walk(store, len, [&rec](const gs_rec& r) { rec.push_back(r); }, &we, true);
-    if (nrec > rec_capacity) return fail(ctx, SV_ERR_ARG, "rec_capacity is below the store's record count", cudaSuccess);
-    if (nrec >= 0xFFFFFFFFu) return fail(ctx, SV_ERR_ARG, "too many records", cudaSuccess);
-    // every live record's checksum is tested (the ENDED record that stops the walk is left alone)
-    std::vector<u64> live_off;
-    std::vector<u32> live_rec;
-    size_t n_upd = 0;
-    for (size_t r = 0; r < nrec; r++)
-        if (rec[r].status == GS_LIVE) {
-            live_off.push_back(rec[r].off);
-            live_rec.push_back((u32)r);
-            n_upd += rec[r].type == 258;
-        }
-    const float walk_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    dev_guard dg__;
-    CK(dg__.enter(ctx->device));
-    cudaStream_t st = ctx->stream;
-    ev_set ev, fev;
-    if (ctx->profiling)
-        for (int i = 0; i < 4; i++) {
-            CK(cudaEventCreate(&ev.e[i]));
-            if (table) CK(cudaEventCreate(&fev.e[i]));
-        }
-    funding_stage F;
-    if (table) {
-        int rc = funding_stage_run(ctx, table, F, fev);
-        if (rc) return rc;
-    }
-    dev_buf<> d_store, t_live;
-    const size_t nlive = live_off.size(), live_bytes = nlive * 9 + 16;
-    int rc = d_store.reserve(ctx, len, len);
-    if (!rc) rc = t_live.reserve(ctx, live_bytes, live_bytes);
+    store_front G;
+    int rc = store_front_run(ctx, store, len, table, rec_capacity, true, G);
     if (rc) return rc;
-    u64* d_live = t_live.at<u64>(0);
-    u8* d_bad = t_live.at<u8>(nlive * 8);
-    if (ev.e[0]) CK(cudaEventRecord(ev.e[0], st));
-    CK(cudaMemcpyAsync(d_store, store, len, cudaMemcpyHostToDevice, st));
-    std::vector<u8> bad_live(nlive), skip(nrec, 0);
-    if (nlive) {
-        CK(cudaMemcpyAsync(d_live, live_off.data(), nlive * 8, cudaMemcpyHostToDevice, st));
-        k_store_crc_flags<<<(unsigned)((nlive + 255) / 256), 256, 0, st>>>(d_store, d_live, nlive, d_bad);
-        ctx->launches += 1;
-        CK(cudaMemcpyAsync(bad_live.data(), d_bad, nlive, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-    }
-    for (size_t k = 0; k < nlive; k++) skip[live_rec[k]] = bad_live[k];
+    const std::vector<gs_rec>& rec = G.rec;
+    const std::vector<u8>& skip = G.bad;  // a live record whose checksum fails is deleted and left out of both rounds
+    const size_t nrec = rec.size();
+    const gs_walk_end& we = G.we;
+    const cudaEvent_t* ev = G.ev.e;
+    u8* d_store = G.d_store;
+    cudaStream_t st = ctx->stream;
+    size_t n_upd = 0;
+    for (const gs_rec& r : rec) n_upd += r.status == GS_LIVE && r.type == 258;
     // first round: the audit's statuses and channel table over the records with good checksums
     store_pass P;
-    rc = store_pass_run(ctx, d_store, len, chain_hash32, rec, nrec, skip.data(), n_upd, P, ev.e[1]);
+    rc = store_pass_run(ctx, d_store, len, chain_hash32, rec, nrec, skip.data(), n_upd, P, ev[3]);
     if (rc) return rc;
     const size_t n_msgs = P.n_msgs, nev = P.nev, items = P.items;
-    std::vector<u8> reason(n_msgs, SV_GP_KEPT), fund(table ? n_msgs : 0, GF_NONE);
+    // the funding verdicts of the announcements whose first-round status is 0: the refused ones join rule 2.  Without a
+    // table d_fund stays empty, and k_prune_mark reads no verdicts.
+    dev_buf<> d_fund;
+    std::vector<u8> fund;
+    if (table) {
+        rc = store_funding_run(ctx, G, len, P, nrec, d_fund, fund);
+        if (rc) return rc;
+    }
+    std::vector<u8> reason(n_msgs, SV_GP_KEPT);
     u32 n_moved = 0;
     if (n_msgs) {
-        // the funding verdicts of the announcements whose first-round status is 0: the refused ones join rule 2
-        std::vector<u32> cand;
-        if (table)
-            for (size_t m = 0; m < n_msgs; m++)
-                if (rec[P.mrec[m]].type == 256 && P.mstatus[m] == 0) cand.push_back((u32)m);
         // second round: the deletions of the first, the table again over the sorted events with those announcements
         // masked out, and the updates whose holder changed verified again under their new signer
         slab_layout L;
         const size_t o_reason = L.take(n_msgs), o_holder2 = L.take(4 * n_msgs), o_sig2 = L.take(33 * n_msgs),
-                     o_ok2 = L.take(nev), o_list = L.take(4 * (n_upd + 1)), o_keyok = L.take(n_upd),
-                     o_fund = L.take(table ? n_msgs : 0), o_cand = L.take(4 * cand.size());
+                     o_ok2 = L.take(nev), o_list = L.take(4 * (n_upd + 1)), o_keyok = L.take(n_upd);
         dev_buf<> s2;
         rc = s2.reserve(ctx, L.size, L.size);
         if (rc) return rc;
-        u8 *d_reason = s2 + o_reason, *d_sig2 = s2 + o_sig2, *d_ok2 = s2 + o_ok2, *d_keyok = s2 + o_keyok,
-           *d_fund = table ? s2 + o_fund : nullptr;
+        u8 *d_reason = s2 + o_reason, *d_sig2 = s2 + o_sig2, *d_ok2 = s2 + o_ok2, *d_keyok = s2 + o_keyok;
         u32 *d_holder2 = s2.at<u32>(o_holder2), *d_list = s2.at<u32>(o_list);
-        if (table) {
-            rc = funding_run(ctx, d_store, len, P.d_moff, n_msgs, cand, F, d_fund, s2.at<u32>(o_cand), fev);
-            if (rc) return rc;
-            CK(cudaMemcpyAsync(fund.data(), d_fund, n_msgs, cudaMemcpyDeviceToHost, st));
-        }
         CK(cudaMemsetAsync(d_holder2, 0xFF, 4 * n_msgs, st));
         CK(cudaMemsetAsync(d_list, 0, 4, st));
         const size_t nmark = n_msgs > nev ? n_msgs : nev;
@@ -2557,11 +2535,11 @@ static int store_prune(sv_ctx* ctx, const uint8_t* store, size_t len, const uint
             k_prune_settle<<<(n_moved + 255) / 256, 256, 0, st>>>(d_list, ctx->d_verdict + items, d_reason);
             ctx->launches += 1;
         }
-        if (ev.e[2]) CK(cudaEventRecord(ev.e[2], st));
+        if (ev[4]) CK(cudaEventRecord(ev[4], st));
         CK(cudaMemcpyAsync(reason.data(), d_reason, n_msgs, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
-    } else if (ev.e[2]) {
-        CK(cudaEventRecord(ev.e[2], st));
+    } else if (ev[4]) {
+        CK(cudaEventRecord(ev[4], st));
     }
     // every record's reason, in store order
     std::vector<u8> pr(nrec, SV_GP_KEPT);
@@ -2571,7 +2549,7 @@ static int store_prune(sv_ctx* ctx, const uint8_t* store, size_t len, const uint
         else if (rec[r].status != GS_LIVE) continue;
         else if (skip[r]) pr[r] = SV_GP_BAD_CRC;
         else if (m != GS_NONE) pr[r] = reason[m];
-        else if (t != GS_CHANNEL_AMOUNT && t != GS_DELETE_CHAN && t != GS_CHAN_DYING && t != GS_UUID) pr[r] = SV_GP_UNKNOWN;
+        else if (!gs_store_record(t)) pr[r] = SV_GP_UNKNOWN;
         // the amount record right after a deleted announcement goes with it (gossip_store_del)
         if (r > 0 && pr[r] == SV_GP_KEPT && t == GS_CHANNEL_AMOUNT && pr[r - 1] != SV_GP_KEPT && rec[r - 1].type == 256)
             pr[r] = SV_GP_AMOUNT;
@@ -2596,7 +2574,7 @@ static int store_prune(sv_ctx* ctx, const uint8_t* store, size_t len, const uint
         ctx->launches += 1;
         CK(cudaMemcpyAsync(flag_hi.data(), d_hi, nd, cudaMemcpyDeviceToHost, st));
     }
-    if (ev.e[3]) CK(cudaEventRecord(ev.e[3], st));
+    if (ev[5]) CK(cudaEventRecord(ev[5], st));
     CK(cudaStreamSynchronize(st));
     if (out != store) memcpy(out, store, len);
     for (size_t i = 0; i < nd; i++) out[doff[i]] = flag_hi[i];
@@ -2613,13 +2591,7 @@ static int store_prune(sv_ctx* ctx, const uint8_t* store, size_t len, const uint
                                 &S.signature, &S.amount, &S.unknown, &FS.deleted};
     for (size_t r = 0; r < nrec; r++) {
         const u32 t = rec[r].type, m = P.msg_of[r];
-        int s = rec[r].status;
-        if (r >= cut) s = r == cut ? GS_ST_NO_AMOUNT : GS_ST_NOT_REACHED;
-        else if (s == GS_LIVE && skip[r]) s = GS_ST_BAD_CRC;
-        else if (s == GS_LIVE && m != GS_NONE) s = P.mstatus[m];
-        else if (s == GS_LIVE)
-            s = (t == GS_CHANNEL_AMOUNT || t == GS_DELETE_CHAN || t == GS_CHAN_DYING || t == GS_UUID) ? GS_ST_STORE_RECORD
-                                                                                                      : GS_ST_UNKNOWN;
+        const int s = r < cut ? store_status(rec[r], skip[r], m, P) : r == cut ? GS_ST_NO_AMOUNT : GS_ST_NOT_REACHED;
         const u8 why = r < cut ? pr[r] : (u8)SV_GP_KEPT;
         rec_off[r] = rec[r].off;
         rec_type[r] = (uint16_t)t;
@@ -2634,10 +2606,13 @@ static int store_prune(sv_ctx* ctx, const uint8_t* store, size_t len, const uint
     }
     *sum = S;
     if (table) *fsum = FS;
-    ctx->gp_ms[0] = walk_ms;
-    if (ev.e[0])
-        for (int i = 0; i < 3; i++) CK(cudaEventElapsedTime(&ctx->gp_ms[1 + i], ev.e[i], ev.e[i + 1]));
-    return funding_timing(ctx, fev);
+    ctx->gp_ms[0] = G.walk_ms;
+    if (ev[0]) {
+        CK(cudaEventElapsedTime(&ctx->gp_ms[1], ev[0], ev[3]));
+        CK(cudaEventElapsedTime(&ctx->gp_ms[2], ev[3], ev[4]));
+        CK(cudaEventElapsedTime(&ctx->gp_ms[3], ev[4], ev[5]));
+    }
+    return funding_timing(ctx, G.fev);
 }
 extern "C" int sv_prune_gossip_store_host(sv_ctx* ctx, const uint8_t* store, size_t len, const uint8_t* chain_hash32,
                                           uint8_t* out, uint64_t* rec_off, uint16_t* rec_type, int* rec_status,

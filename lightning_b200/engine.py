@@ -188,6 +188,13 @@ def _u8(a, shape_tail):
     return a
 
 
+def _chain_hash(h):
+    chain = np.frombuffer(bytes(h), dtype=np.uint8)
+    if chain.size != 32:
+        raise ValueError("chain_hash must be 32 bytes")
+    return chain
+
+
 class SigVerifier:
     """One engine context on one GPU (sv_ctx)."""
 
@@ -281,9 +288,7 @@ class SigVerifier:
         lens = np.array([len(m) for m in msgs], dtype=np.uint32)
         offs = np.concatenate([[0], np.cumsum(lens[:-1], dtype=np.uint64)]).astype(np.uint64) if n else np.zeros(0, np.uint64)
         blob = np.frombuffer(b"".join(bytes(m) for m in msgs), dtype=np.uint8)
-        chain = np.frombuffer(bytes(chain_hash), dtype=np.uint8)
-        if chain.size != 32:
-            raise ValueError("chain_hash must be 32 bytes")
+        chain = _chain_hash(chain_hash)
         kinds = None if signer_kind is None else np.ascontiguousarray(signer_kind, dtype=np.uint8).reshape(-1)
         if kinds is not None and kinds.size != n:
             raise ValueError("signer_kind: one byte per message")
@@ -312,11 +317,7 @@ class SigVerifier:
         lightningd's funding outputs (sv_verify_gossip_store_funding_host), and the call returns two more items:
         rec_funding uint8 (GF_* verdict per record) and the funding summary dict."""
         buf = np.frombuffer(bytes(store), dtype=np.uint8)
-        chain = None
-        if chain_hash is not None:
-            chain = np.frombuffer(bytes(chain_hash), dtype=np.uint8)
-            if chain.size != 32:
-                raise ValueError("chain_hash must be 32 bytes")
+        chain = None if chain_hash is None else _chain_hash(chain_hash)
         n = int(self.lib.sv_gossip_store_count(buf.ctypes.data, buf.size)) if capacity is None else int(capacity)
         off = np.zeros(max(n, 1), np.uint64)
         typ = np.zeros(max(n, 1), np.uint16)
@@ -356,11 +357,7 @@ class SigVerifier:
         "pruned" counts them), and the call returns two more items: rec_funding uint8 (GF_* verdict per record) and
         the funding summary dict ("deleted": the funding deletions)."""
         buf = np.frombuffer(bytes(store), dtype=np.uint8)
-        chain = None
-        if chain_hash is not None:
-            chain = np.frombuffer(bytes(chain_hash), dtype=np.uint8)
-            if chain.size != 32:
-                raise ValueError("chain_hash must be 32 bytes")
+        chain = None if chain_hash is None else _chain_hash(chain_hash)
         n = int(self.lib.sv_gossip_prune_count(buf.ctypes.data, buf.size)) if capacity is None else int(capacity)
         out = np.empty(max(buf.size, 1), np.uint8)
         off = np.zeros(max(n, 1), np.uint64)
@@ -409,11 +406,7 @@ class SigVerifier:
         return int(self.lib.sv_gossip_prune_cut(ctypes.byref(s), pruned, len(pruned)))
 
     def _store_fd(self, repair, fd, length, chain_hash):
-        chain = None
-        if chain_hash is not None:
-            chain = np.frombuffer(bytes(chain_hash), dtype=np.uint8)
-            if chain.size != 32:
-                raise ValueError("chain_hash must be 32 bytes")
+        chain = None if chain_hash is None else _chain_hash(chain_hash)
         s, new_len = SvGossipPruneSummary(), ctypes.c_uint64(0)
         cp = chain.ctypes.data if chain is not None else None
         if repair:

@@ -1,7 +1,7 @@
 // tests/host_emul/gossip_store_emul.cpp — TEST-ONLY host build of lightning_b200/csrc/gossip_store.cuh (linked into
 // libemul.so).
 //
-// The checksum the k_store_crc kernel computes per record, the header walk sv_verify_gossip_store_host runs, and the
+// The checksum the k_store_crc_flags kernel computes per record, the header walk sv_verify_gossip_store_host runs, and the
 // per-scid event rule of k_store_resolve applied in store order (the kernel applies it per scid after a stable sort by
 // scid, which gives each scid the same sequence).  The sort and the thread layout are checked on the device by
 // tests/test_gpu_gossip_store.py.
