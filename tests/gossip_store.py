@@ -10,6 +10,7 @@ CHANNEL_AMOUNT, DELETE_CHAN, ENDED, CHAN_DYING, UUID = 4101, 4103, 4105, 4106, 4
 # record statuses besides the signature statuses (include/cln_sigverify.h SV_GS_*)
 EOF, ST_DELETED, STORE_RECORD, UNKNOWN, NOT_REACHED = 0, 16, 17, 18, 19
 INCOMPLETE, PARTIAL, TRUNCATED, BAD_CRC, ST_ENDED, NO_AMOUNT = 32, 33, 34, 35, 36, 37
+STORE_TYPES = (CHANNEL_AMOUNT, DELETE_CHAN, CHAN_DYING, UUID)  # the store's own records: status STORE_RECORD
 NONE = None
 
 
@@ -39,9 +40,10 @@ def record(msg, ts=0, flags=COMPLETED, crc=None):
     return struct.pack(">HHII", flags, len(msg), crc32c(ts, msg) if crc is None else crc, ts) + msg
 
 
-def walk(store):
+def walk(store, truncated_stops=True):
     """map_catchup's header walk -> (records [(off, type, len, status)], map_end, stop, no_amount entry or None);
-    status 0 = live, to be judged by checksum and content"""
+    status 0 = live, to be judged by checksum and content.  The prune's walk (truncated_stops=False) steps over a
+    TRUNCATED record instead of stopping at it."""
     recs, off, stop, no_amount = [], 1, EOF, None
     while off + HDR < len(store):
         flags, ln = struct.unpack(">HH", store[off:off + 4])
@@ -60,7 +62,7 @@ def walk(store):
         if st == 0 and typ == 256 and no_amount is None and off + HDR + ln + HDR + 2 + 8 > len(store):
             no_amount = len(recs)
         recs.append((off, typ, ln, st))
-        if st not in (0, ST_DELETED):
+        if st not in (0, ST_DELETED) and (truncated_stops or st != TRUNCATED):
             stop = st
             break
         off += HDR + ln
@@ -70,6 +72,12 @@ def walk(store):
 def crc_ok(store, off):
     ln, crc, ts = struct.unpack(">HII", store[off + 2:off + 12])
     return crc32c(ts, store[off + HDR:off + HDR + ln]) == crc
+
+
+def reseal(store, off):
+    """recompute the checksum of the record at header offset off of the bytearray store"""
+    ln, ts = struct.unpack(">H", store[off + 2:off + 4])[0], struct.unpack(">I", store[off + 8:off + 12])[0]
+    struct.pack_into(">I", store, off + 4, crc32c(ts, bytes(store[off + 12:off + 12 + ln])))
 
 
 # How far past a message's first byte gossmap reads it, whatever the message's own length: add_channel reads the
@@ -97,6 +105,30 @@ def ann_fields(m, p=0):
     return m[p:p + 32], m[p + 32:p + 40], m[p + 40:p + 73], m[p + 73:p + 106]
 
 
+def holders(store, recs, live):
+    """the channel table over the records `live` (indices, store order): {entry: the entry of the announcement its event
+    saw, or None} for announcements and updates whose reads stay inside the store"""
+    held, holder = {}, {}
+    for i in live:
+        off, typ = recs[i][0], recs[i][1]
+        p = off + HDR
+        if typ == 256 and ann_ok(store, p):
+            scid = ann_fields(store, p)[1]
+            holder[i] = held.get(scid)
+            held.setdefault(scid, i)
+        elif typ == DELETE_CHAN and p + DEL_READ <= len(store):
+            held.pop(store[p + 2:p + 10], None)
+        elif typ == 258 and p + UPD_READ <= len(store):
+            holder[i] = held.get(store[p + 98:p + 106])
+    return holder
+
+
+def signer(store, recs, i, h):
+    """the node key an update at entry i is checked under when entry h holds its channel: node_id_1 or node_id_2 of
+    that announcement by the update's direction bit; None without a holder"""
+    return None if h is None else ann_fields(store, recs[h][0] + HDR)[2 + (store[recs[i][0] + HDR + 111] & 1)]
+
+
 def audit(store, sigcheck=None):
     """The whole call: -> (list of (off, type, status, holder_off or None), summary dict).
     sigcheck(msg, signer33 or None) gives a message's status (the signature statuses with whatever gates the caller
@@ -109,20 +141,7 @@ def audit(store, sigcheck=None):
         if st in (0, ST_ENDED) and not crc_ok(store, off):
             cut, cut_status = i, BAD_CRC
             break
-    held, holder = {}, {}
-    for i in range(cut):
-        off, typ, ln, st = recs[i]
-        if st:
-            continue
-        p = off + HDR
-        if typ == 256 and ann_ok(store, p):
-            scid = ann_fields(store, p)[1]
-            holder[i] = held.get(scid)
-            held.setdefault(scid, i)
-        elif typ == DELETE_CHAN and p + DEL_READ <= len(store):
-            held.pop(store[p + 2:p + 10], None)
-        elif typ == 258 and p + UPD_READ <= len(store):
-            holder[i] = held.get(store[p + 98:p + 106])
+    holder = holders(store, recs, [i for i in range(cut) if recs[i][3] == 0])
     if no_amount is not None and no_amount < cut and holder.get(no_amount) is None:
         cut, cut_status = no_amount, NO_AMOUNT
     out = []
@@ -136,14 +155,11 @@ def audit(store, sigcheck=None):
             m = store[off + HDR:off + HDR + ln]
             if typ in (256, 257, 258):
                 h = holder.get(i)
-                signer = None
-                if typ == 258 and h is not None:
-                    signer = ann_fields(store, recs[h][0] + HDR)[2 + (store[off + HDR + 111] & 1)]
-                st = sigcheck(m, signer) if sigcheck else 0
+                st = sigcheck(m, signer(store, recs, i, h) if typ == 258 else None) if sigcheck else 0
                 s["redundant_announcements"] += typ == 256 and h is not None
                 s["updates_without_channel"] += typ == 258 and off + HDR + UPD_READ <= len(store) and h is None
             else:
-                st = STORE_RECORD if typ in (CHANNEL_AMOUNT, DELETE_CHAN, CHAN_DYING, UUID) else UNKNOWN
+                st = STORE_RECORD if typ in STORE_TYPES else UNKNOWN
         elif st == ST_ENDED and ln >= 10:
             s["ended_equivalent_offset"] = struct.unpack(">Q", store[off + HDR + 2:off + HDR + 10])[0]
         out.append((off, typ, st, None if h is None else recs[h][0]))

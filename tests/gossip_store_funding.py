@@ -1,19 +1,17 @@
 """Python model of the funding check of a gossip_store (sv_verify_gossip_store_funding_host and
 sv_prune_gossip_store_funding_host, include/cln_sigverify.h): one verdict per channel_announcement from lightningd's
 funding outputs, following get_txout (lightningd/gossip_control.c:78-115) and gossipd's txout reply
-(gossipd/gossmap_manage.c:696-699, :791-819, :850-852), and the prune with those refused deleted in rule 2.  Built on
-the audit's model (tests/gossip_store.py) and the prune's (tests/gossip_store_prune.py)."""
+(gossipd/gossmap_manage.c:696-699, :791-819, :850-852).  Built on the audit's model (tests/gossip_store.py); the
+prune with those refused deleted in rule 2 is tests/gossip_store_prune.py prune with a table."""
 import hashlib
 import struct
 
 from tests import gossip_store as gs
-from tests import gossip_store_prune as gp
-from tests.gossip_store import CHANNEL_AMOUNT, HDR, ann_fields, crc_ok
+from tests.gossip_store import CHANNEL_AMOUNT, HDR
 
-# verdicts (include/cln_sigverify.h SV_GF_*) and the prune's reason for a funding deletion (SV_GP_FUNDING)
+# verdicts (include/cln_sigverify.h SV_GF_*)
 GF_NONE, GF_FUNDED, GF_UNCHECKED, GF_DYING, GF_NO_TXOUT, GF_SCRIPT, GF_AMOUNT = range(7)
 REFUSED = (GF_NO_TXOUT, GF_SCRIPT, GF_AMOUNT)
-GP_FUNDING = 9
 DYING = 0x0800
 NAMES = {GF_FUNDED: "funded", GF_UNCHECKED: "unchecked", GF_DYING: "dying", GF_NO_TXOUT: "no_txout",
          GF_SCRIPT: "script", GF_AMOUNT: "amount"}
@@ -82,81 +80,6 @@ def audit(store, table, sigcheck=None):
     return rows, s, fund, summary(fund)
 
 
-def prune(store, table, sigcheck=None):
-    """tests/gossip_store_prune.py prune with rule 2 extended: an announcement whose first-round status is 0 and whose
-    verdict is refused is deleted (GP_FUNDING).  -> (pruned bytes, rows (off, type, status, reason), summary, verdict per
-    row, funding summary)"""
-    if store[0] >> 5:
-        raise ValueError("major version")
-    recs, end, stop, no_amount = gp.walk(store)
-    bad = {i for i, (off, typ, ln, st) in enumerate(recs) if st == 0 and not crc_ok(store, off)}
-    live = [i for i, r in enumerate(recs) if r[3] == 0 and i not in bad]
-
-    def signer(i, h):
-        return None if h is None else ann_fields(store, recs[h][0] + HDR)[2 + (store[recs[i][0] + HDR + 111] & 1)]
-
-    def check(i, h):
-        off, ln = recs[i][0], recs[i][2]
-        return sigcheck(store[off + HDR:off + HDR + ln], signer(i, h)) if sigcheck else 0
-
-    h1 = gp.holders(store, recs, live)
-    status = {i: check(i, h1.get(i)) for i in live if recs[i][1] in (256, 257, 258)}
-    fund = {i: verdict(store, recs[i][0], table) for i in live if recs[i][1] == 256 and status[i] == 0}
-    reason = {i: gp.GP_TRUNCATED for i, r in enumerate(recs) if r[3] == gs.TRUNCATED}
-    reason.update({i: gp.GP_BAD_CRC for i in bad})
-    for i, st in status.items():
-        if (st in (-1, -3)) if recs[i][1] == 258 else st != 0:
-            reason[i] = gp.GP_MESSAGE
-        elif fund.get(i) in REFUSED:
-            reason[i] = GP_FUNDING
-    h2 = gp.holders(store, recs, [i for i in live if not (recs[i][1] == 256 and i in reason)])
-    reverified = 0
-    for i in live:
-        typ = recs[i][1]
-        if i in reason:
-            continue
-        if typ == 256:
-            if h2.get(i) is not None:
-                reason[i] = gp.GP_REDUNDANT
-        elif typ == 258:
-            h = h2.get(i)
-            if h is None:
-                reason[i] = gp.GP_NO_CHANNEL
-            elif h != h1.get(i):
-                reverified += 1
-                if check(i, h) != 0:
-                    reason[i] = gp.GP_SIGNATURE
-            elif status[i] != 0:
-                reason[i] = gp.GP_SIGNATURE
-        elif typ not in (257,) + gp.STORE_TYPES:
-            reason[i] = gp.GP_UNKNOWN
-    for i in range(1, len(recs)):
-        if recs[i][3] == 0 and i not in reason and recs[i][1] == CHANNEL_AMOUNT and recs[i - 1][1] == 256 and i - 1 in reason:
-            reason[i] = gp.GP_AMOUNT
-    cut = no_amount if no_amount is not None and no_amount not in reason else len(recs)
-    out = bytearray(store)
-    rows, fv = [], []
-    for i, (off, typ, ln, st) in enumerate(recs):
-        if i >= cut:
-            st = gs.NO_AMOUNT if i == cut else gs.NOT_REACHED
-        elif st == 0:
-            st = gs.BAD_CRC if i in bad else status[i] if i in status else (
-                gs.STORE_RECORD if typ in gp.STORE_TYPES else gs.UNKNOWN)
-        why = reason.get(i, gp.GP_KEPT) if i < cut else gp.GP_KEPT
-        if why:
-            out[off] |= gs.DELETED >> 8
-        rows.append((off, typ, st, why))
-        fv.append(fund.get(i, GF_NONE) if i < cut else GF_NONE)
-    whys = [w for _, _, _, w in rows]
-    s = dict(version=store[0], stop=gs.NO_AMOUNT if cut < len(recs) else stop,
-             end_offset=recs[cut][0] if cut < len(recs) else end, records=len(recs),
-             pruned=sum(w != gp.GP_KEPT for w in whys), reverified=reverified)
-    for k, name in enumerate(("bad_crc", "truncated", "message", "redundant", "no_channel", "signature", "amount",
-                              "unknown"), 1):
-        s[name] = whys.count(k)
-    return bytes(out), rows, s, fv, summary(fv, whys.count(GP_FUNDING))
-
-
 def table_of_store(store):
     """the table that funds every channel of a store as its own amount records say: for each live announcement (first of
     its scid) followed by a channel_amount, an output at its scid with the 2-of-2 script and that amount; every block
@@ -175,11 +98,6 @@ def table_of_store(store):
 
 
 # ---- the committed store fixture, funded by a table built from its own announcements, and one mutation per verdict ----
-def _reseal(store, off):
-    ln, ts = struct.unpack(">H", store[off + 2:off + 4])[0], struct.unpack(">I", store[off + 8:off + 12])[0]
-    struct.pack_into(">I", store, off + 4, gs.crc32c(ts, bytes(store[off + 12:off + 12 + ln])))
-
-
 def fixture_cases(fx):
     """name -> (store bytes, (scids, satoshis, scripts, blocks)), from the fixture fx: the table funds every channel as
     its amount records say, then one change per verdict"""
@@ -240,7 +158,7 @@ def fixture_cases(fx):
     a = recs[i + 1]
     st = bytearray(fx)
     struct.pack_into(">Q", st, a[0] + HDR + 2, sats[pos[s]] + 1)
-    _reseal(st, a[0])
+    gs.reseal(st, a[0])
     mine = [j for j, r in enumerate(recs) if r[1] == 258 and r[3] == 0 and
             fx[r[0] + HDR + 98:r[0] + HDR + 106] == struct.pack(">Q", s)]
     out["refused_holder_then_funded_copy"] = (bytes(st) + rec(i) + rec(i + 1) + b"".join(rec(j) for j in mine), table())

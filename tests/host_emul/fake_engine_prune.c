@@ -1,15 +1,21 @@
 /*
  * fake_engine_prune.c — a stand-in for the engine's gossip_store prune (sv_gossip_prune_count, sv_prune_gossip_store_host
- * of cln_sigverify.h), linked beside fake_engine.c or fake_engine_timed.c so that sv_prune_gossip_store_fd
- * (lightning_b200/csrc/gossip_store_fd.c), the verifier subdaemon's prune requests and the drop-in's gossip_store_prune
- * can be tested without a GPU (tests/test_sigverifyd_prune_fake.py).  It deletes a fixed set of records for fixed reasons,
- * which the test recomputes:
- *   walk    from offset 1 while a whole 12-byte header fits; a record whose message runs past the end stops it
- *           (stop SV_GS_PARTIAL, end_offset its offset), else the walk ends at the end (SV_GS_EOF)
- *   delete  record r (0-based, in walk order) when r % 3 == 1 and its flags do not have bit 0x8000 yet, for reason
- *           1 + (r / 3) % 8 (SV_GP_BAD_CRC .. SV_GP_UNKNOWN); reverified counts the SV_GP_SIGNATURE deletions
- * A major version other than 0, len 0 or rec_capacity below the record count: SV_ERR_ARG, nothing written.  Each call
- * appends "sv_prune_gossip_store_host 0 <records> <len>" to $FAKE_ENGINE_LOG.  Like fake_engine_timed.c, a
+ * of cln_sigverify.h) whose walk stops where gossmap's does on a torn store, linked beside fake_engine.c or
+ * fake_engine_timed.c so that sv_prune_gossip_store_fd and sv_repair_gossip_store_fd
+ * (lightning_b200/csrc/gossip_store_fd.c), the verifier subdaemon's prune and repair requests and the drop-in's
+ * gossip_store_prune and gossip_store_repair can be tested without a GPU (tests/test_sigverifyd_prune_fake.py,
+ * tests/test_sigverifyd_repair_fake.py).  It deletes a fixed set of records for fixed reasons, which the tests recompute:
+ *   walk    from offset 1 while 13 bytes are left (a shorter tail is a torn header: stop SV_GS_EOF, end_offset < len).
+ *           A record without bit 0x2000 stops it (SV_GS_INCOMPLETE); one with bit 0x8000 is stepped over (so a deleted
+ *           record running past the end leaves end_offset > len); one running past the end stops it (SV_GS_PARTIAL), as
+ *           does a type 4105 (SV_GS_ENDED) and a type 256 with fewer than 22 bytes after it (SV_GS_NO_AMOUNT).  The
+ *           record it stops at is not an entry, so summary.records counts one record fewer than the engine's walk
+ *           gives for a stopped store (gs_walk emits the record it stops at too); the cut does not read it.
+ *           end_offset is the stop's offset, or where the walk ran out.
+ *   delete  entry r (0-based, in walk order) when r % 3 == 1 and it is not deleted yet, for reason 1 + (r / 3) % 8
+ *           (SV_GP_BAD_CRC .. SV_GP_UNKNOWN); reverified counts the SV_GP_SIGNATURE deletions
+ * A major version other than 0, len 0 or rec_capacity below the entry count: SV_ERR_ARG, nothing written.  Each call
+ * appends "sv_prune_gossip_store_host 0 <entries> <len>" to $FAKE_ENGINE_LOG.  Like fake_engine_timed.c, a
  * "sv_prune_gossip_store_host=<ms>" entry in $FAKE_ENGINE_DELAY holds each call that long, between a
  * "begin sv_prune_gossip_store_host 0" and an "end sv_prune_gossip_store_host 0" line in $FAKE_ENGINE_TRACE.
  */
@@ -41,18 +47,26 @@ static long prune_delay_ms(void) {
     return 0;
 }
 
-/* the walk: each record's offset into offs (if given); returns the record count, *end and *stop where it ended */
+/* the walk: each entry's offset into offs (if given); returns the entry count, *end and *stop where it ended */
 static size_t walk(const uint8_t *s, size_t len, uint64_t *end, int32_t *stop, uint64_t *offs) {
-    size_t off = 1, r = 0;
+    uint64_t off = 1;
+    size_t r = 0;
     *stop = SV_GS_EOF;
-    while (off + 12 <= len) {
-        size_t mlen = ((size_t)s[off + 2] << 8) | s[off + 3];
-        if (off + 12 + mlen > len) { *stop = SV_GS_PARTIAL; break; }
+    while (off + 12 < len) {
+        const unsigned flags = ((unsigned)s[off] << 8) | s[off + 1];
+        const uint64_t mlen = ((uint64_t)s[off + 2] << 8) | s[off + 3];
+        const unsigned type = off + 14 <= len ? ((unsigned)s[off + 12] << 8) | s[off + 13] : 0;
+        if (!(flags & 0x2000)) { *stop = SV_GS_INCOMPLETE; break; }
+        if (!(flags & 0x8000)) {
+            if (off + 12 + mlen > len) { *stop = SV_GS_PARTIAL; break; }
+            if (type == 4105) { *stop = SV_GS_ENDED; break; }
+            if (type == 256 && off + 12 + mlen + 22 > len) { *stop = SV_GS_NO_AMOUNT; break; }
+        }
         if (offs) offs[r] = off;
         r++;
         off += 12 + mlen;
     }
-    *end = off < len ? off : len;
+    *end = off;
     return r;
 }
 

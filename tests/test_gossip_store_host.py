@@ -61,7 +61,7 @@ def emul_audit(emul, store):
             if i in midx:
                 h = None if hold[i] is None else int(off[hold[i]])
             else:
-                s = gs.STORE_RECORD if typ[i] in (4101, 4103, 4106, 4107) else gs.UNKNOWN
+                s = gs.STORE_RECORD if typ[i] in gs.STORE_TYPES else gs.UNKNOWN
         out.append((int(off[i]), int(typ[i]), s, h))
     return out, dict(stop=cut_status or stop, end_offset=int(off[cut]) if cut_status else int(end3[0]))
 

@@ -1,10 +1,11 @@
 """GPU: the funding check of a gossip_store (sv_verify_gossip_store_funding_host, sv_prune_gossip_store_funding_host).
 The committed store fixture with a table built from its own announcements and amount records, then one deterministic
-mutation per verdict, each checked on the device against the model (tests/gossip_store_funding.py, with CLN's own
-gossipd/sigcheck.c as its sigcheck).  The pruned store must load under Core Lightning's gossmap.c strictly, as gossipd
-loads it at start-up (oracle/gossmap_strict_harness.c), and every channel it holds must be funded, unchecked or dying
-in the table, with the capacity the table gives.  Then the same on the fixture tiled x53 with 1 % of the table wrong,
-the Python binding without a table, and the command line's exit codes."""
+mutation per verdict, each checked on the device against the model (tests/gossip_store_funding.py, and
+tests/gossip_store_prune.py with the table, with CLN's own gossipd/sigcheck.c as their sigcheck).  The pruned store must
+load under Core Lightning's gossmap.c strictly, as gossipd loads it at start-up (oracle/gossmap_strict_harness.c), and
+every channel it holds must be funded, unchecked or dying in the table, with the capacity the table gives.  Then the same
+on the fixture tiled x53 with 1 % of the table wrong, the Python binding without a table, and the command line's exit
+codes."""
 import ctypes
 import os
 import struct
@@ -16,6 +17,7 @@ import pytest
 from lightning_b200.funding import FundingTable
 from tests import gossip_store as gs
 from tests import gossip_store_funding as gf
+from tests import gossip_store_prune as gp
 from tests import oracle_replay
 from tests.test_gossip_store_host import load_fixture
 from tests.test_gossip_store_prune_host import strict_load
@@ -65,7 +67,7 @@ def check(engine, store, t, chain=TESTNET):
     # the prune
     out, (poff, ptyp, pst, why), ps, pfund, pfs = engine.prune_gossip_store(store, chain, funding=ft)
     assert store == before
-    want, wrows, ws, wpfund, wpfs = gf.prune(store, table, sig)
+    want, wrows, ws, wpfund, wpfs = gp.prune(store, sig, table)
     assert out == want
     assert [(int(a), int(b), int(c), int(d)) for a, b, c, d in zip(poff, ptyp, pst, why)] == wrows
     assert [int(x) for x in pfund] == wpfund

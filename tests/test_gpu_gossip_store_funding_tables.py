@@ -29,6 +29,7 @@ from lightning_b200.funding import FundingTable
 from tests import funding_tables as ftab
 from tests import gossip_store as gs
 from tests import gossip_store_funding as gf
+from tests import gossip_store_prune as gp
 from tests.test_gossip_store_funding_host import make_db
 from tests.test_gossip_store_host import load_fixture
 from tests.test_gpu_gossip_burst import TESTNET
@@ -76,7 +77,7 @@ def model_results(store, t):
     key = (hash(store), tuple(sorted(t.outputs.items())), frozenset(t.blocks))
     if key not in _MODEL:
         _, _, fund, fs = gf.audit(store, t)
-        out, rows, s, pfund, pfs = gf.prune(store, t)
+        out, rows, s, pfund, pfs = gp.prune(store, table=t)
         _MODEL[key] = (fund, fs, out, rows, s, pfund, pfs)
     return _MODEL[key]
 

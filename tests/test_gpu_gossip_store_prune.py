@@ -63,17 +63,11 @@ def memo(f):
     return g
 
 
-def reseal(store, off):
-    """recompute the checksum of the record at header offset off"""
-    ln, ts = struct.unpack(">H", store[off + 2:off + 4])[0], struct.unpack(">I", store[off + 8:off + 12])[0]
-    struct.pack_into(">I", store, off + 4, gs.crc32c(ts, bytes(store[off + 12:off + 12 + ln])))
-
-
 def flip_sig(rec_bytes, k=0):
     """a record with bit 0 of signature k's byte 10 flipped, checksum recomputed"""
     r = bytearray(rec_bytes)
     r[12 + 2 + 64 * k + 10] ^= 1
-    reseal(r, 0)
+    gs.reseal(r, 0)
     return bytes(r)
 
 
@@ -137,12 +131,12 @@ def corrupted_x53():
         k = int(rng.integers(0, 3))
         if k == 0 and t in (256, 257, 258):
             store[off + 12 + 2 + int(rng.integers(0, 64))] ^= 1 << int(rng.integers(0, 8))
-            reseal(store, off)
+            gs.reseal(store, off)
         elif k == 1:
             store[off + 12 + int(rng.integers(2, ln))] ^= 1
         else:
             store[off + 12:off + 14] = struct.pack(">H", 4999)
-            reseal(store, off)
+            gs.reseal(store, off)
     return bytes(store)
 
 

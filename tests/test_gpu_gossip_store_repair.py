@@ -39,7 +39,8 @@ from tests.test_gossmap import gossmap_load
 from tests.test_gpu_gossip_burst import PUB, SK, TESTNET, _ordered, _sha256d, make_ca, make_cu
 from tests.test_gpu_gossip_store import TOOL
 from tests.test_gpu_gossip_store_prune import corrupted_x53
-from tests.test_sigverifyd_repair_fake import case, cut_rule, run_client
+from tests.test_sigverifyd_prune_fake import case, run_client
+from tests.test_sigverifyd_repair_fake import cut_rule
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -275,7 +276,7 @@ def test_repair_through_the_daemon(expected, tmp_path, name):
             part = tests[i:i + batch]
             for k in part:
                 (d / k).write_bytes(torn(name, k))
-            got = run_client(tmp_path, build.LIB, "sock:" + sock, [case(d / k) for k in part])
+            got = run_client(tmp_path, build.LIB, "sock:" + sock, [case(d / k, op="repair") for k in part])
             for k, g in zip(part, got):
                 t, pruned, s, cut = expected(name, k)
                 assert g == [True, 0, s, cut], k
@@ -320,7 +321,7 @@ def test_ended_and_untorn_stores_are_only_pruned(engine, tmp_path):
             assert sp["stop"] == gs.ST_ENDED and sp["end_offset"] < len(st)
         b.write_bytes(st)
         with sigverifyd_daemon.running(tmp_path) as sock:
-            got = run_client(tmp_path, build.LIB, "sock:" + sock, [case(b)])
+            got = run_client(tmp_path, build.LIB, "sock:" + sock, [case(b, op="repair")])
         assert got == [[True, 0, sp, len(st)]] and b.read_bytes() == a.read_bytes(), k
         dst = tmp_path / (k + ".cli")
         r = subprocess.run([TOOL, "--chain", TESTNET.hex(), "--prune", str(dst), "--cut-tail", str(b)], capture_output=True,

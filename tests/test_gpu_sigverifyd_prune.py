@@ -100,7 +100,7 @@ def test_dropin_in_process_and_through_the_daemon(host, tmp_path):
             pruned, s = host[name]
             assert (d / name).read_bytes() == pruned, (how, name)
             first, second = got[how][2 * k], got[how][2 * k + 1]
-            assert first == [True, 0, s], (how, name)
+            assert first == [True, 0, s, None], (how, name)
             assert second[:2] == [True, 0] and second[2] == _nothing_more(second[2]), (how, name)
 
 

@@ -1,17 +1,19 @@
 """CPU: pruning a gossip_store FILE in place — sv_prune_gossip_store_fd (lightning_b200/csrc/gossip_store_fd.c), the
 verifier subdaemon's sigverifyd_gossip_store_prune (the store's fd passed over the socket with SCM_RIGHTS) and the drop-in's
 gossip_store_prune in both modes — built with gcc against a fake prune (tests/host_emul/fake_engine_prune.c) that deletes a
-fixed set of records.  Checked: the file changes only in bit 0x8000 of the flags of the records the fake deleted, the same
-way in-process, through a daemon on a socket and through `--fd N`; a client-mode process never creates a context; every
-refused file or frame is answered without the daemon exiting, leaves the file as it was, and leaves the daemon with no
-descriptor more than before; a prune runs beside channel checks and never beside another prune; the codec of the new
-messages."""
+fixed set of records.  The builds, the client process and the fake's Python statement serve the repair's tests
+(tests/test_sigverifyd_repair_fake.py) too.  Checked: the file changes only in bit 0x8000 of the flags of the records the
+fake deleted, the same way in-process, through a daemon on a socket and through `--fd N`; a client-mode process never
+creates a context; every refused file or frame is answered without the daemon exiting, leaves the file as it was, and
+leaves the daemon with no descriptor more than before; a prune runs beside channel checks and never beside another prune;
+the codec of the new messages."""
 import contextlib
 import ctypes
 import errno
 import json
 import os
 import socket
+import struct
 import subprocess
 import sys
 import time
@@ -22,6 +24,8 @@ import pytest
 from lightning_b200 import build
 from lightning_b200 import sigverifyd_wire as W
 from lightning_b200.engine import SvGossipPruneSummary
+from tests.gossip_store import EOF, INCOMPLETE, NO_AMOUNT, PARTIAL, ST_ENDED
+from tests.gossip_store_prune import REASONS
 from tests.test_sigverifyd_fake_engine import verify_req
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -29,10 +33,8 @@ HE = os.path.join(ROOT, "tests", "host_emul")
 STORE_FD = os.path.join(build.CSRC, "gossip_store_fd.c")
 PRUNE = "sv_prune_gossip_store_host"
 FIELDS = [f for f, _ in SvGossipPruneSummary._fields_]
-REASONS = ("bad_crc", "truncated", "message", "redundant", "no_channel", "signature", "amount", "unknown")  # SV_GP_1..8
 TESTNET = bytes.fromhex("43497fd7f826957108f4a30fd9cec3aeba79972084e90ead01ea330900000000")
 MAX_PRUNE_STORE = 4 << 30  # sigverifyd_proto.h
-GS_EOF, GS_PARTIAL = 0, 33
 
 
 # ---- stores and what the fake prune makes of them (fake_engine_prune.c) ----------------------------------------------
@@ -53,12 +55,19 @@ def fake_prune(store):
     """(the pruned store, the summary dict) the fake engine gives"""
     out, s = bytearray(store), dict.fromkeys(FIELDS, 0)
     off, r = 1, 0
-    s["version"], s["stop"] = store[0], GS_EOF
-    while off + 12 <= len(store):
-        mlen = int.from_bytes(store[off + 2:off + 4], "big")
-        if off + 12 + mlen > len(store):
-            s["stop"] = GS_PARTIAL
+    s["version"], s["stop"] = store[0], EOF
+    while off + 12 < len(store):
+        flags, mlen = struct.unpack(">HH", store[off:off + 4])
+        typ = struct.unpack(">H", store[off + 12:off + 14])[0] if off + 14 <= len(store) else 0
+        if not flags & 0x2000:
+            s["stop"] = INCOMPLETE
             break
+        if not flags & 0x8000:
+            stop = PARTIAL if off + 12 + mlen > len(store) else ST_ENDED if typ == 4105 else \
+                NO_AMOUNT if typ == 256 and off + 12 + mlen + 22 > len(store) else None
+            if stop:
+                s["stop"] = stop
+                break
         if r % 3 == 1 and not store[off] & 0x80:
             why = 1 + (r // 3) % 8
             out[off] |= 0x80
@@ -67,7 +76,7 @@ def fake_prune(store):
             s["reverified"] += why == 6
         r += 1
         off += 12 + mlen
-    s["end_offset"], s["records"] = min(off, len(store)), r
+    s["end_offset"], s["records"] = off, r
     return bytes(out), s
 
 
@@ -138,7 +147,10 @@ CLIENT = r"""
 import ctypes, json, os, sys
 from lightning_b200.engine import SvGossipPruneSummary
 lib = ctypes.CDLL(sys.argv[1], use_errno=True)
-lib.gossip_store_prune.restype = ctypes.c_bool
+for fn in (lib.gossip_store_repair, lib.gossip_store_prune):
+    fn.restype = ctypes.c_bool
+lib.gossip_store_repair.argtypes = [ctypes.c_int, ctypes.c_uint64, ctypes.c_void_p, ctypes.POINTER(SvGossipPruneSummary),
+                                    ctypes.POINTER(ctypes.c_uint64)]
 lib.gossip_store_prune.argtypes = [ctypes.c_int, ctypes.c_uint64, ctypes.c_void_p, ctypes.POINTER(SvGossipPruneSummary)]
 lib.cln_sigverify_connect.argtypes = [ctypes.c_char_p]
 mode = sys.argv[2]
@@ -156,20 +168,25 @@ for c in json.load(open(sys.argv[3])):
         os.close(fd)
     else:
         fd = os.open(c["path"], os.O_RDWR if c["kind"] == "rw" else os.O_RDONLY)
-    s = SvGossipPruneSummary()
+    s, n = SvGossipPruneSummary(), ctypes.c_uint64(12345)
     chain = bytes.fromhex(c["chain"]) if c["chain"] else None
-    ok = lib.gossip_store_prune(fd, c["len"], chain, ctypes.byref(s))
+    if c["op"] == "prune":
+        ok = lib.gossip_store_prune(fd, c["len"], chain, ctypes.byref(s))
+    else:
+        ok = lib.gossip_store_repair(fd, c["len"], chain, ctypes.byref(s), ctypes.byref(n))
     e = ctypes.get_errno()
     if c["kind"] != "closed":
         os.close(fd)
     if c["kind"] == "pipe":
         os.close(w)
-    out.append([ok, 0 if ok else e, {f: getattr(s, f) for f, _ in SvGossipPruneSummary._fields_} if ok else None])
+    out.append([ok, 0 if ok else e, {f: getattr(s, f) for f, _ in SvGossipPruneSummary._fields_} if ok else None,
+                n.value if ok and c["op"] == "repair" else None])
 print(json.dumps(out))
 """
 
 
 def run_client(tmp_path, lib, mode, cases, pass_fds=(), check=True):
+    """each case's [ok, errno, summary, new_len (a repair's, else None)] from a process of its own"""
     path = tmp_path / ("cases%d.json" % time.monotonic_ns())
     path.write_text(json.dumps(cases))
     env = dict(os.environ, PYTHONPATH=ROOT + os.pathsep + os.environ.get("PYTHONPATH", ""))
@@ -181,9 +198,11 @@ def run_client(tmp_path, lib, mode, cases, pass_fds=(), check=True):
     return r
 
 
-def case(path, length=None, chain=TESTNET, kind="rw"):
+def case(path, length=None, chain=TESTNET, kind="rw", op="prune"):
+    """a gossip_store_prune (op "prune") or gossip_store_repair (op "repair") call on the file at path, or on a pipe or a
+    closed descriptor (kind "pipe", "closed")"""
     return dict(kind=kind, path=str(path), len=os.path.getsize(path) if length is None else length,
-                chain=chain.hex() if chain else None)
+                chain=chain.hex() if chain else None, op=op)
 
 
 def prune_frame(rid, length, chain=TESTNET):
@@ -228,7 +247,7 @@ def test_file_pruned_in_place_every_way(tmp_path, bins, seed, n, tail):
     again = dict(summary, pruned=0, reverified=0, **{r: 0 for r in REASONS})
     for how in files:
         assert files[how].read_bytes() == want, how
-        assert got[how] == [[True, 0, summary], [True, 0, again]], how
+        assert got[how] == [[True, 0, summary, None], [True, 0, again, None]], how
 
 
 def test_client_mode_never_creates_a_context(tmp_path, bins):
@@ -254,8 +273,8 @@ def test_refused_files(tmp_path, bins):
     big = tmp_path / "big"
     with open(big, "wb") as fh:  # sparse: no data blocks
         fh.truncate(MAX_PRUNE_STORE + 4096)
-    cases = [case(ro, kind="ro"), dict(kind="pipe", path="", len=64, chain=None), case(short, len(store) + 1),
-             case(v1), case(big), dict(kind="closed", path="", len=10, chain=None), case(short, 0), case(good)]
+    cases = [case(ro, kind="ro"), case("", 64, None, kind="pipe"), case(short, len(store) + 1), case(v1), case(big),
+             case("", 10, None, kind="closed"), case(short, 0), case(good)]
     want_err = [errno.EBADF, errno.EINVAL, errno.EINVAL, errno.EINVAL, errno.EFBIG, errno.EBADF, errno.EINVAL]
     before = {f: f.read_bytes() for f in (ro, short, v1)}
     with serve(tmp_path, bins["daemon"], _env(tmp_path)) as (proc, sock):
@@ -265,7 +284,7 @@ def test_refused_files(tmp_path, bins):
         assert proc.poll() is None
         assert back_to(proc, base) == base
     assert [g[:2] for g in got[:-1]] == [[False, e] for e in want_err]
-    assert got[-1] == [True, 0, fake_prune(store)[1]]
+    assert got[-1] == [True, 0, fake_prune(store)[1], None]
     for f, b in before.items():
         assert f.read_bytes() == b, f
     assert os.path.getsize(big) == MAX_PRUNE_STORE + 4096

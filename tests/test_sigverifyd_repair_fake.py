@@ -1,36 +1,30 @@
 """CPU: repairing a gossip_store FILE in place — sv_repair_gossip_store_fd and sv_gossip_prune_cut
 (lightning_b200/csrc/gossip_store_fd.c), the verifier subdaemon's sigverifyd_gossip_store_repair (the store's fd passed over
-the socket with SCM_RIGHTS) and the drop-in's gossip_store_repair in both modes — built with gcc against a fake prune
-(tests/host_emul/fake_engine_repair.c) whose walk stops where gossmap's does on a torn store.  Checked: the cut against a
-Python statement of the tail rule on every stop kind; the file ends as the fake's pruned store cut there, with the fake's
-summary and new_len, in-process, through a daemon on a socket and through `--fd N`; a client-mode process never creates a
-context; every refused file or frame is answered without the daemon exiting, leaves the file as it was and the daemon with
-no descriptor more than before; a repair runs on the gossip worker beside channel checks and never beside a prune; the codec
-of the new messages."""
+the socket with SCM_RIGHTS) and the drop-in's gossip_store_repair in both modes — built with gcc against the fake prune
+(tests/host_emul/fake_engine_prune.c) whose walk stops where gossmap's does on a torn store; the builds, the client process
+and the fake's Python statement are tests/test_sigverifyd_prune_fake.py's.  Checked: the cut against a Python statement of
+the tail rule on every stop kind; the file ends as the fake's pruned store cut there, with the fake's summary and new_len,
+in-process, through a daemon on a socket and through `--fd N`; a client-mode process never creates a context; every
+refused file or frame is answered without the daemon exiting, leaves the file as it was and the daemon with no descriptor
+more than before; a repair runs on the gossip worker beside channel checks and never beside a prune; the codec of the new
+messages."""
 import ctypes
 import errno
-import json
 import os
 import socket
 import struct
 import subprocess
-import sys
 import time
 
 import numpy as np
-import pytest
 
-from lightning_b200 import build
 from lightning_b200 import sigverifyd_wire as W
 from lightning_b200.engine import SvGossipPruneSummary
+from tests.gossip_store import BAD_CRC, EOF, INCOMPLETE, NO_AMOUNT, PARTIAL, ST_ENDED, TRUNCATED
 from tests.test_sigverifyd_fake_engine import verify_req
-from tests.test_sigverifyd_prune_fake import (FIELDS, MAX_PRUNE_STORE, PRUNE, REASONS, TESTNET, _begun, _env, _trace,
-                                              back_to, make_store, nfds, prune_frame, serve)
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HE = os.path.join(ROOT, "tests", "host_emul")
-STORE_FD = os.path.join(build.CSRC, "gossip_store_fd.c")
-EOF, INCOMPLETE, PARTIAL, TRUNCATED, BAD_CRC, ENDED, NO_AMOUNT = 0, 32, 33, 34, 35, 36, 37  # SV_GS_*
+from tests.test_sigverifyd_prune_fake import (FIELDS, MAX_PRUNE_STORE, PRUNE, TESTNET, _begun, _env, _trace, _wait,
+                                              back_to, bins, case, fake_prune, make_store, nfds, prune_frame, run_client,
+                                              serve)
 
 
 def tail_rule(stop, end_offset, length):
@@ -68,36 +62,7 @@ def cut_rule(pruned, s):
     return room_back_off(pruned, cut) if cut < len(pruned) else cut
 
 
-# ---- stores and what the fake makes of them (fake_engine_repair.c) ---------------------------------------------------
-def fake_prune(store):
-    """(the pruned store, the summary dict) the fake engine gives"""
-    out, s = bytearray(store), dict.fromkeys(FIELDS, 0)
-    off, r = 1, 0
-    s["version"], s["stop"] = store[0], EOF
-    while off + 12 < len(store):
-        flags, mlen = struct.unpack(">HH", store[off:off + 4])
-        typ = struct.unpack(">H", store[off + 12:off + 14])[0] if off + 14 <= len(store) else 0
-        if not flags & 0x2000:
-            s["stop"] = INCOMPLETE
-            break
-        if not flags & 0x8000:
-            stop = PARTIAL if off + 12 + mlen > len(store) else ENDED if typ == 4105 else \
-                NO_AMOUNT if typ == 256 and off + 12 + mlen + 22 > len(store) else None
-            if stop:
-                s["stop"] = stop
-                break
-        if r % 3 == 1 and not store[off] & 0x80:
-            why = 1 + (r // 3) % 8
-            out[off] |= 0x80
-            s["pruned"] += 1
-            s[REASONS[why - 1]] += 1
-            s["reverified"] += why == 6
-        r += 1
-        off += 12 + mlen
-    s["end_offset"], s["records"] = off, r
-    return bytes(out), s
-
-
+# ---- stores and what the fake makes of them (fake_engine_prune.c) ----------------------------------------------------
 def fake_repair(store):
     """(the repaired file, the summary, new_len)"""
     out, s = fake_prune(store)
@@ -134,86 +99,6 @@ def torn_stores():
     return out
 
 
-# ---- builds and client processes ------------------------------------------------------------------------------------
-def _gcc(args):
-    r = subprocess.run(["gcc"] + args, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-
-
-@pytest.fixture(scope="module")
-def bins(tmp_path_factory):
-    d = tmp_path_factory.mktemp("repair_fake")
-    out = dict(daemon=str(d / "cln_sigverifyd"), inproc=str(d / "libdropin_inproc.so"), client=str(d / "libdropin_client.so"),
-               shim=str(d / "libwire_shim_repair.so"))
-    fake = [os.path.join(HE, "fake_engine_repair.c"), STORE_FD]
-    _gcc(build.DAEMON_CFLAGS + [os.path.join(build.CSRC, "sigverifyd.c"), os.path.join(HE, "fake_engine_timed.c")] + fake +
-         ["-o", out["daemon"]])
-    dropin = build.DROPIN_CFLAGS + ["-shared", os.path.join(build.CSRC, "cln_dropin.c"), os.path.join(HE, "fake_engine.c")] + fake
-    _gcc(dropin + ["-o", out["inproc"]])
-    _gcc(dropin + ["-DFAKE_ENGINE_NO_CONTEXT", "-o", out["client"]])  # its sv_create aborts
-    _gcc(["-O2", "-shared", "-fPIC", "-Wall", os.path.join(HE, "wire_shim_repair.c"), "-o", out["shim"]])
-    return out
-
-
-CLIENT = r"""
-import ctypes, json, os, sys
-from lightning_b200.engine import SvGossipPruneSummary
-lib = ctypes.CDLL(sys.argv[1], use_errno=True)
-for fn in (lib.gossip_store_repair, lib.gossip_store_prune):
-    fn.restype = ctypes.c_bool
-lib.gossip_store_repair.argtypes = [ctypes.c_int, ctypes.c_uint64, ctypes.c_void_p, ctypes.POINTER(SvGossipPruneSummary),
-                                    ctypes.POINTER(ctypes.c_uint64)]
-lib.gossip_store_prune.argtypes = [ctypes.c_int, ctypes.c_uint64, ctypes.c_void_p, ctypes.POINTER(SvGossipPruneSummary)]
-lib.cln_sigverify_connect.argtypes = [ctypes.c_char_p]
-mode = sys.argv[2]
-if mode.startswith("sock:"):
-    assert lib.cln_sigverify_connect(mode[5:].encode()) == 0
-elif mode.startswith("fd:"):
-    assert lib.cln_sigverify_connect_fd(int(mode[3:])) == 0
-out = []
-for c in json.load(open(sys.argv[3])):
-    if c["kind"] == "pipe":
-        fd, w = os.pipe()
-        os.write(w, bytes(64))
-    elif c["kind"] == "closed":
-        fd = os.open(os.devnull, os.O_RDONLY)
-        os.close(fd)
-    else:
-        fd = os.open(c["path"], os.O_RDWR if c["kind"] == "rw" else os.O_RDONLY)
-    s, n = SvGossipPruneSummary(), ctypes.c_uint64(12345)
-    chain = bytes.fromhex(c["chain"]) if c["chain"] else None
-    if c.get("op") == "prune":
-        ok = lib.gossip_store_prune(fd, c["len"], chain, ctypes.byref(s))
-    else:
-        ok = lib.gossip_store_repair(fd, c["len"], chain, ctypes.byref(s), ctypes.byref(n))
-    e = ctypes.get_errno()
-    if c["kind"] != "closed":
-        os.close(fd)
-    if c["kind"] == "pipe":
-        os.close(w)
-    out.append([ok, 0 if ok else e, {f: getattr(s, f) for f, _ in SvGossipPruneSummary._fields_} if ok else None,
-                n.value if ok and c.get("op") != "prune" else None])
-print(json.dumps(out))
-"""
-
-
-def run_client(tmp_path, lib, mode, cases, pass_fds=(), check=True):
-    path = tmp_path / ("cases%d.json" % time.monotonic_ns())
-    path.write_text(json.dumps(cases))
-    env = dict(os.environ, PYTHONPATH=ROOT + os.pathsep + os.environ.get("PYTHONPATH", ""))
-    r = subprocess.run([sys.executable, "-c", CLIENT, lib, mode, str(path)], env=env, capture_output=True, text=True,
-                       timeout=120, pass_fds=pass_fds)
-    if check:
-        assert r.returncode == 0, r.stderr[-3000:]
-        return json.loads(r.stdout)
-    return r
-
-
-def case(path, length=None, chain=TESTNET, kind="rw", op="repair"):
-    return dict(kind=kind, path=str(path), len=os.path.getsize(path) if length is None else length,
-                chain=chain.hex() if chain else None, op=op)
-
-
 def repair_frame(rid, length, chain=TESTNET):
     return W.encode("sigverifyd_gossip_store_repair", req_id=rid, has_chain=1 if chain else 0, chain_hash=chain or bytes(32),
                     len=length)
@@ -226,7 +111,7 @@ def test_cut_rule(bins):
     lib = ctypes.CDLL(bins["inproc"])
     lib.sv_gossip_prune_cut.restype = ctypes.c_uint64
     lib.sv_gossip_prune_cut.argtypes = [ctypes.POINTER(SvGossipPruneSummary), ctypes.c_char_p, ctypes.c_uint64]
-    stops = (EOF, 16, 17, 18, 19, INCOMPLETE, PARTIAL, TRUNCATED, BAD_CRC, ENDED, NO_AMOUNT, 0, 1, -1, 99)
+    stops = (EOF, 16, 17, 18, 19, INCOMPLETE, PARTIAL, TRUNCATED, BAD_CRC, ST_ENDED, NO_AMOUNT, 0, 1, -1, 99)
     for stop in stops:
         for length in (1, 13, 977, 70001):
             zeros = bytes(length)  # records of type 0: no announcement to back off from
@@ -278,7 +163,8 @@ def test_file_repaired_every_way(tmp_path, bins):
         d[how].mkdir()
         for k in names:
             (d[how] / k).write_bytes(stores[k])
-    cases = lambda how: [c for k in names for c in (case(d[how] / k), case(d[how] / k, want[k][2]))]
+    cases = lambda how: [c for k in names for c in (case(d[how] / k, op="repair"),
+                                                    case(d[how] / k, want[k][2], op="repair"))]
     got = {"inproc": run_client(tmp_path, bins["inproc"], "inproc", cases("inproc"))}
     with serve(tmp_path, bins["daemon"], _env(tmp_path)) as (proc, sock):
         got["sock"] = run_client(tmp_path, bins["client"], "sock:" + sock, cases("sock"))
@@ -311,14 +197,14 @@ def test_clean_store_repair_is_the_prune(tmp_path, bins):
         a, b = tmp_path / (name + ".p"), tmp_path / (name + ".r")
         a.write_bytes(st)
         b.write_bytes(st)
-        p, r = run_client(tmp_path, bins["inproc"], "inproc", [case(a, op="prune"), case(b)])
+        p, r = run_client(tmp_path, bins["inproc"], "inproc", [case(a), case(b, op="repair")])
         assert a.read_bytes() == b.read_bytes() and p[2] == r[2] and r[3] == len(st), name
 
 
 def test_client_mode_never_creates_a_context(tmp_path, bins):
     f = tmp_path / "gossip_store"
     f.write_bytes(torn_stores()["partial_100"])
-    r = run_client(tmp_path, bins["client"], "inproc", [case(f)], check=False)
+    r = run_client(tmp_path, bins["client"], "inproc", [case(f, op="repair")], check=False)
     assert r.returncode != 0 and "sv_create called" in r.stderr
 
 
@@ -336,8 +222,9 @@ def test_refused_files(tmp_path, bins):
     big = tmp_path / "big"
     with open(big, "wb") as fh:
         fh.truncate(MAX_PRUNE_STORE + 4096)
-    cases = [case(ro, kind="ro"), dict(kind="pipe", path="", len=64, chain=None), case(short, len(store) + 1), case(v1),
-             case(big), dict(kind="closed", path="", len=10, chain=None), case(short, 0), case(good)]
+    cases = [case(ro, kind="ro", op="repair"), case("", 64, None, kind="pipe", op="repair"),
+             case(short, len(store) + 1, op="repair"), case(v1, op="repair"), case(big, op="repair"),
+             case("", 10, None, kind="closed", op="repair"), case(short, 0, op="repair"), case(good, op="repair")]
     want_err = [errno.EBADF, errno.EINVAL, errno.EINVAL, errno.EINVAL, errno.EFBIG, errno.EBADF, errno.EINVAL]
     before = {f: f.read_bytes() for f in (ro, short, v1)}
     with serve(tmp_path, bins["daemon"], _env(tmp_path)) as (proc, sock):
@@ -411,7 +298,7 @@ def test_repair_beside_channel_checks_never_beside_a_prune(tmp_path, bins):
                 c.settimeout(30)
                 c.connect(sock)
             socket.send_fds(a, [repair_frame(1, len(stores[0]))], [fds[0]])
-            _wait_for(_begun(tmp_path, PRUNE))
+            _wait(_begun(tmp_path, PRUNE))
             socket.send_fds(b, [prune_frame(2, len(stores[1]))], [fds[1]])
             for k in range(3):
                 f, want = verify_req(rng, 10 + k, 0, 3)
@@ -430,15 +317,6 @@ def test_repair_beside_channel_checks_never_beside_a_prune(tmp_path, bins):
     assert [e[0] for e in _trace(tmp_path) if e[1] == PRUNE] == ["begin", "end", "begin", "end"]
     assert files[0].read_bytes() == fake_repair(stores[0])[0]
     assert files[1].read_bytes() == fake_prune(stores[1])[0]
-
-
-def _wait_for(pred, timeout=30):
-    end = time.time() + timeout
-    while time.time() < end:
-        if pred():
-            return
-        time.sleep(0.01)
-    raise AssertionError("condition not reached")
 
 
 # ---- the codec -------------------------------------------------------------------------------------------------------
