@@ -136,6 +136,8 @@ void cln_sigverify_shutdown(void);
  *                                                                                        the fd travels, not the store)
  *   gossip_store_repair                                                                 (sigverifyd_gossip_store_repair:
  *                                                                                        likewise)
+ *   gossip_store_salvage                                                                (sigverifyd_gossip_store_salvage:
+ *                                                                                        likewise)
  * check_tx_sig gates the sighash type before it sends anything; the BIP143 sighash is built on the daemon's device.
  * check_tx_sigs_bip143_batch sends requests of at most 65536 transactions and 64 MiB of scripts each.  pubkey_from_der
  * returns false for a length other than 33 without sending anything.  The daemon serves the requests of all its clients
@@ -289,6 +291,15 @@ bool gossip_store_prune(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_
  * gossip_store_prune, or that of a failed ftruncate; the deletions already written stay.  Client mode as for
  * gossip_store_prune. */
 bool gossip_store_repair(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_prune_summary *summary, uint64_t *new_len);
+
+/* gossip_store_repair, after the store's damaged record headers in mid-store are mended (sv_salvage_gossip_store_fd in
+ * cln_sigverify.h): a header whose length or COMPLETED bit was damaged is restored where its checksum says its record
+ * ends, any other damaged span is covered by deleted filler records, so the records after the damage are kept instead of
+ * cut with a torn tail.  A store without such damage is repaired exactly as by gossip_store_repair.  true: *summary,
+ * *salvage and *new_len (each may be NULL) say what the repair deleted, what the salvage mended and where the file ends
+ * now.  false with errno as for gossip_store_repair.  Client mode as for gossip_store_prune. */
+bool gossip_store_salvage(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_prune_summary *summary,
+                          sv_gossip_salvage_summary *salvage, uint64_t *new_len);
 
 #ifdef __cplusplus
 }

@@ -398,6 +398,71 @@ int sv_repair_gossip_store_fd(sv_ctx *ctx, int fd, uint64_t len, const uint8_t *
                               uint64_t *new_len);
 uint64_t sv_gossip_prune_cut(const sv_gossip_prune_summary *summary, const uint8_t *pruned, uint64_t len);
 
+/* ---- SALVAGE a gossip_store past damaged record headers.  Every walk above follows the length in each record's header,
+ *      as map_catchup does, so one flipped bit in a record's flags or length sends it into the middle of a message, where
+ *      it soon stops (SV_GS_INCOMPLETE) and the repair cuts the file there: every record after the damage is lost though
+ *      it is intact.  The salvage finds where the records resume and mends the chain of lengths with a few header
+ *      writes, so the prune and the repair keep them.
+ *
+ *      A SOUND record at offset o: its 12-byte header and its message lie inside the store, COMPLETED is set, len >= 2,
+ *      the type is 256, 257, 258, 4101, 4103, 4105, 4106 or 4107, and crc32c(timestamp, msg[0, len)) is the header's
+ *      crc.  The deleted bit does not matter (gossipd's deletions keep a valid checksum).  The walk starts at offset 1 and
+ *      goes on while 12 bytes of header fit before the end.  A sound record is stepped over by its length; a sound,
+ *      non-deleted gossip_store_ended record stops the walk.  At a record t that is not sound:
+ *        1. If COMPLETED is set and t + 12 + len is sound, the length is right: t is left to the prune, which deletes it
+ *           (SV_GP_BAD_CRC, SV_GP_TRUNCATED or SV_GP_UNKNOWN), and the walk goes on at t + 12 + len.
+ *        2. Else let q be the smallest sound offset with q >= t + 14.  If there is none, t is the tail: the walk stops and
+ *           leaves it to sv_gossip_prune_cut.  The end of the store is never a q, so a torn tail is repaired exactly as
+ *           sv_repair_gossip_store_fd repairs it without the salvage.
+ *        3. RESTORE when q - t - 12 <= 65535 and crc32c(timestamp(t), store[t + 12, q)) == crc(t): len = q - t - 12 is
+ *           written and COMPLETED set, the other flag bits kept.  The record is whole again and the prune judges it.
+ *        4. Else BRIDGE [t, q) with filler records: flags DELETED | COMPLETED, a length in [2, 65535], as few as cover the
+ *           span, their sizes as even as possible (the first span % k one byte longer).  Only each filler's 4 bytes of
+ *           flags and length are written.  gossmap skips a deleted record by its length before it looks at anything else
+ *           (common/gossmap.c:842-847), and gossipd's compaction (gossipd/compactd.c copy_records) reads len - 2 bytes of
+ *           every record, deleted or not, hence the 14-byte minimum.
+ *        The walk goes on at q.  A span [t, q) that already holds exactly the fillers rule 4 would write is not a break
+ *      (fillers are never sound, so a salvaged store leads the walk there again).  For a message of 2 bytes or more, rule 1 is "COMPLETED and t + 12 + len == q"; for a
+ *      shorter one (SV_GS_TRUNCATED, which ends before any q can lie) it keeps the sound record right after it.
+ *      A store without a break (a torn tail included) is not changed; a salvaged store has no break left, so a second
+ *      salvage writes nothing.  Known limit: a sound record that an attacker embeds in the damaged record's own payload is
+ *      taken as q.  It still goes through the prune, where every signed message is verified; the store's own record
+ *      types carry no signature.
+ *
+ *      sv_salvage_gossip_store_host: out (len bytes; may equal store) is store with the header writes.  One action per
+ *      break, in store order: act_off = t, act_resume = q, act_kind = SV_SALVAGE_RESTORED or SV_SALVAGE_BRIDGED; at most
+ *      act_capacity are listed (the arrays may be NULL when it is 0), summary->breaks counts them all.  A major version
+ *      other than 0: SV_ERR_ARG, nothing written.  On the device: k_salvage_filter (one thread per byte offset: the
+ *      header tests, and an order-preserving compaction of the candidates through a per-block count and k_salvage_scan),
+ *      then k_salvage_crc (the slice-by-8 checksum, one thread per candidate, a warp per candidate over 1,024 bytes).  The
+ *      host walks the store with the sorted sound offsets (a galloping binary search, header bytes only), and
+ *      k_salvage_restore checks each break's restore CRC on the device, one warp per break.
+ *
+ *      sv_salvage_gossip_store_fd: the salvage on bytes [0, len) of fd, then fsync, then exactly sv_repair_gossip_store_fd
+ *      (*summary and *new_len are its).  Each action is written back (pwrite) as 4 bytes of flags and length per header;
+ *      a bridge's fillers are written from the last to the first and synced (fsync) before the first one overwrites the
+ *      damaged header at t.  Until that 4-byte write reaches the disk the walk still stops at the damaged header and never
+ *      reads the other fillers, so a crash or a power loss at any point leaves each break as it was or whole.  Arguments,
+ *      errors and errno are those of sv_repair_gossip_store_fd; *salvage is written on SV_OK.  The verifier subdaemon
+ *      serves this call for its clients (sigverifyd_gossip_store_salvage: the fd travels over its socket). ---- */
+#define SV_SALVAGE_RESTORED 1
+#define SV_SALVAGE_BRIDGED 2
+typedef struct {
+    uint64_t breaks;        /* records restored or bridged */
+    uint64_t restored, bridged;
+    uint64_t bridged_bytes; /* bytes the bridges cover */
+    uint64_t fillers;       /* filler records written */
+    uint64_t sound;         /* sound offsets found in the store */
+} sv_gossip_salvage_summary;
+int sv_salvage_gossip_store_host(sv_ctx *ctx, const uint8_t *store, size_t len, uint8_t *out, uint64_t *act_off,
+                                 uint64_t *act_resume, uint8_t *act_kind, size_t act_capacity,
+                                 sv_gossip_salvage_summary *summary);
+int sv_salvage_gossip_store_fd(sv_ctx *ctx, int fd, uint64_t len, const uint8_t *chain_hash32,
+                               sv_gossip_prune_summary *summary, sv_gossip_salvage_summary *salvage, uint64_t *new_len);
+/* profiling mode: ms3 = the two filter passes with the scan, the checksum kernel (device events around the kernels
+ * only), the host walk */
+int sv_get_last_gossip_salvage_timing(sv_ctx *ctx, float *ms3);
+
 /* L2 residency hint for the throughput kernels (default on): the G comb table and the per-thread multiples tables are
  * marked persisting through a stream access-policy window, the rest of the stream's traffic streaming.  0 switches it off
  * for streams not yet seen (measurement aid). */

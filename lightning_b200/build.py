@@ -70,6 +70,12 @@ def build_engine(force=False, verbose=False):
                        capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("gcc (gossip_store_fd.c) failed:\n" + r.stdout + r.stderr)
+    # salvaging a gossip_store file in place (sv_salvage_gossip_store_fd): plain C over the salvage and the repair
+    salvage_fd_o = os.path.join(CSRC, "gossip_salvage_fd.o")
+    r = subprocess.run(["gcc"] + DROPIN_CFLAGS + ["-c", os.path.join(CSRC, "gossip_salvage_fd.c"), "-o", salvage_fd_o],
+                       capture_output=True, text=True)
+    if r.returncode != 0:
+        raise RuntimeError("gcc (gossip_salvage_fd.c) failed:\n" + r.stdout + r.stderr)
     # the batch-verification kernels are a translation unit of their own, compiled with the field multiplier as real
     # functions (see batch.cu); everything else inlines it
     batch_flags = [f for f in NVCC_FLAGS if f not in ("-shared", "-DSV_FE_INLINE", "-DSV_MAIN_SYNC")] + ["-DSV_NO_SYNC_INLINE", "-c"]
@@ -81,7 +87,7 @@ def build_engine(force=False, verbose=False):
     if r.returncode != 0:
         raise RuntimeError("nvcc (batch.cu) failed:\n" + r.stdout + r.stderr)
     cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + [
-        "-o", LIB, os.path.join(CSRC, "engine.cu"), batch_o, dropin_o, store_fd_o]
+        "-o", LIB, os.path.join(CSRC, "engine.cu"), batch_o, dropin_o, store_fd_o, salvage_fd_o]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if verbose:
         sys.stderr.write(r.stderr)
@@ -103,7 +109,8 @@ def build_engine(force=False, verbose=False):
 
 def build_host_emul(force=False):
     src = [os.path.join(ROOT, "tests", "host_emul", f) for f in ("emul.cpp", "bolt12_emul.cpp", "gossip_store_emul.cpp",
-                                                             "gossip_funding_emul.cpp", "fee_grind_emul.cpp")]
+                                                             "gossip_funding_emul.cpp", "fee_grind_emul.cpp",
+                                                             "gossip_salvage_emul.cpp")]
     srcs = _sources(CSRC, (".cuh",)) + src
     if not force and _newer(EMUL, srcs):
         return EMUL

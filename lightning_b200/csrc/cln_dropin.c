@@ -20,6 +20,7 @@
 /* likewise for the in-place prune: gossip_store_prune then works through the daemon only */
 #pragma weak sv_prune_gossip_store_fd
 #pragma weak sv_repair_gossip_store_fd
+#pragma weak sv_salvage_gossip_store_fd
 
 #include <errno.h>
 #include <fcntl.h>
@@ -1128,17 +1129,20 @@ static void ticket_reply(const struct req *q, const u8 *r, size_t rl) {
     }
 }
 
-/* ---- gossip_store_prune / gossip_store_repair: gossipd's store pruned in place (sv_prune_gossip_store_fd), and its
- * torn tail cut (sv_repair_gossip_store_fd); in client mode the file's descriptor goes to the daemon with the request,
- * never its bytes ---- */
-static bool remote_prune(bool repair, int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_prune_summary *summary,
-                         uint64_t *new_len) {
+/* ---- gossip_store_prune / gossip_store_repair / gossip_store_salvage: gossipd's store pruned in place
+ * (sv_prune_gossip_store_fd), its torn tail cut (sv_repair_gossip_store_fd), its damaged headers mended first
+ * (sv_salvage_gossip_store_fd); in client mode the file's descriptor goes to the daemon with the request, never its
+ * bytes ---- */
+enum store_op { STORE_PRUNE, STORE_REPAIR, STORE_SALVAGE };
+static bool remote_prune(enum store_op op, int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_prune_summary *summary,
+                         uint64_t *new_len, sv_gossip_salvage_summary *salvage) {
     static const u8 zero[32];
     size_t mlen = 2 + 8 + 1 + 32 + 8, rl;
     u8 f[4 + 2 + 8 + 1 + 32 + 8];
     uint64_t id = ++g_req_id;
     const u8 *chain = chain_hash32 ? chain_hash32 : zero;
-    if (repair) towire_sigverifyd_gossip_store_repair(f + 4, mlen, id, chain_hash32 != NULL, chain, len);
+    if (op == STORE_SALVAGE) towire_sigverifyd_gossip_store_salvage(f + 4, mlen, id, chain_hash32 != NULL, chain, len);
+    else if (op == STORE_REPAIR) towire_sigverifyd_gossip_store_repair(f + 4, mlen, id, chain_hash32 != NULL, chain, len);
     else towire_sigverifyd_gossip_store_prune(f + 4, mlen, id, chain_hash32 != NULL, chain, len);
     /* every request before it is written out first (send_some writes in order), so the fd rides on this frame's first
      * byte: the daemon matches it to this request */
@@ -1151,10 +1155,18 @@ static bool remote_prune(bool repair, int fd, uint64_t len, const u8 *chain_hash
     u8 *r = g_q[at].reply;
     rl = g_q[at].reply_len;
     g_t = g_s = g_r = at;
-    /* the repair reply is the prune reply's fields, then new_len */
+    /* the repair reply is the prune reply's fields, then new_len; the salvage reply adds the salvage summary */
     struct sigverifyd_gossip_store_prune_reply p;
     struct sigverifyd_gossip_store_repair_reply q;
-    if (repair) {
+    struct sigverifyd_gossip_store_salvage_reply v;
+    if (op == STORE_SALVAGE) {
+        if (!fromwire_sigverifyd_gossip_store_salvage_reply(r, rl, &v)) die_daemon("malformed gossip_store salvage reply");
+        p = (struct sigverifyd_gossip_store_prune_reply){v.req_id, v.err, v.version, v.stop, v.end_offset, v.records,
+                                                         v.pruned, v.bad_crc, v.truncated, v.message, v.redundant,
+                                                         v.no_channel, v.signature, v.amount, v.unknown, v.reverified};
+        *new_len = v.new_len;
+        *salvage = (sv_gossip_salvage_summary){v.breaks, v.restored, v.bridged, v.bridged_bytes, v.fillers, v.sound};
+    } else if (op == STORE_REPAIR) {
         if (!fromwire_sigverifyd_gossip_store_repair_reply(r, rl, &q)) die_daemon("malformed gossip_store repair reply");
         p = (struct sigverifyd_gossip_store_prune_reply){q.req_id, q.err, q.version, q.stop, q.end_offset, q.records,
                                                          q.pruned, q.bad_crc, q.truncated, q.message, q.redundant,
@@ -1189,7 +1201,7 @@ bool gossip_store_prune(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_
     sv_gossip_prune_summary s;
     if (fcntl(fd, F_GETFD) < 0) return false; /* errno EBADF: nothing to send */
     if (client()) {
-        if (!remote_prune(false, fd, len, chain_hash32, &s, NULL)) return false;
+        if (!remote_prune(STORE_PRUNE, fd, len, chain_hash32, &s, NULL, NULL)) return false;
     } else {
         if (!sv_prune_gossip_store_fd) die("gossip_store_prune: this engine has no sv_prune_gossip_store_fd", SV_ERR_ARG);
         int rc = sv_prune_gossip_store_fd(ctx(), fd, len, chain_hash32, &s);
@@ -1205,7 +1217,7 @@ bool gossip_store_repair(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip
     uint64_t cut = 0;
     if (fcntl(fd, F_GETFD) < 0) return false; /* errno EBADF: nothing to send */
     if (client()) {
-        if (!remote_prune(true, fd, len, chain_hash32, &s, &cut)) return false;
+        if (!remote_prune(STORE_REPAIR, fd, len, chain_hash32, &s, &cut, NULL)) return false;
     } else {
         if (!sv_repair_gossip_store_fd) die("gossip_store_repair: this engine has no sv_repair_gossip_store_fd", SV_ERR_ARG);
         int rc = sv_repair_gossip_store_fd(ctx(), fd, len, chain_hash32, &s, &cut);
@@ -1213,6 +1225,26 @@ bool gossip_store_repair(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip
         if (rc != SV_OK) die("sv_repair_gossip_store_fd", rc);
     }
     if (summary) *summary = s;
+    if (new_len) *new_len = cut;
+    return true;
+}
+
+bool gossip_store_salvage(int fd, uint64_t len, const u8 *chain_hash32, sv_gossip_prune_summary *summary,
+                          sv_gossip_salvage_summary *salvage, uint64_t *new_len) {
+    sv_gossip_prune_summary s;
+    sv_gossip_salvage_summary v;
+    uint64_t cut = 0;
+    if (fcntl(fd, F_GETFD) < 0) return false; /* errno EBADF: nothing to send */
+    if (client()) {
+        if (!remote_prune(STORE_SALVAGE, fd, len, chain_hash32, &s, &cut, &v)) return false;
+    } else {
+        if (!sv_salvage_gossip_store_fd) die("gossip_store_salvage: this engine has no sv_salvage_gossip_store_fd", SV_ERR_ARG);
+        int rc = sv_salvage_gossip_store_fd(ctx(), fd, len, chain_hash32, &s, &v, &cut);
+        if (rc == SV_ERR_ARG || rc == SV_ERR_IO) return false; /* errno says why */
+        if (rc != SV_OK) die("sv_salvage_gossip_store_fd", rc);
+    }
+    if (summary) *summary = s;
+    if (salvage) *salvage = v;
     if (new_len) *new_len = cut;
     return true;
 }

@@ -1,6 +1,6 @@
 /* cln_verify_gossip_store — audit a Core Lightning gossip_store before lightningd loads it.
  *
- *   cln_verify_gossip_store [--chain HEX] [--device N] [--funding TABLE] [--prune OUT [--cut-tail]] FILE
+ *   cln_verify_gossip_store [--chain HEX] [--device N] [--funding TABLE] [--prune OUT [--cut-tail | --salvage]] FILE
  *
  * Walks the store as gossmap does, checks every record checksum and verifies every signature on the GPU
  * (sv_verify_gossip_store_host).  Prints a summary and one line per failing record (offset, type, status).
@@ -25,6 +25,11 @@
  * incomplete or partial record, an announcement without its amount record, or a torn header; an announcement the cut
  * would leave without its amount record goes too), as
  * sv_repair_gossip_store_fd cuts a file in place.  Prints where it cut, then audits OUT as --prune does.
+ *
+ * --salvage (with --prune; implies --cut-tail): before the prune, mends the chain of record lengths past damaged headers
+ * (sv_salvage_gossip_store_host), as sv_salvage_gossip_store_fd does in place.  Prints each break's offset, the offset
+ * where the records resume and what was done (header restored, or span bridged by deleted filler records), then prunes,
+ * cuts and audits OUT as --cut-tail does.
  *
  * --funding TABLE: also checks every announcement against lightningd's funding outputs (TABLE as written by
  * `python -m lightning_b200.funding export`; sv_verify_gossip_store_funding_host).  Prints the funding counts and one
@@ -65,8 +70,8 @@ static const char *status_name(int s) {
 }
 
 static int usage(void) {
-    fprintf(stderr, "usage: cln_verify_gossip_store [--chain HEX] [--device N] [--funding TABLE] [--prune OUT [--cut-tail]] "
-                    "FILE\n");
+    fprintf(stderr, "usage: cln_verify_gossip_store [--chain HEX] [--device N] [--funding TABLE] "
+                    "[--prune OUT [--cut-tail | --salvage]] FILE\n");
     return 3;
 }
 
@@ -166,6 +171,33 @@ static int audit(sv_ctx *ctx, const uint8_t *store, size_t len, const uint8_t *c
 
 static void audit_free(audit_result *a) { free(a->off); free(a->type); free(a->status); free(a->fund); }
 
+/* --salvage: out = store[0, len) salvaged; the breaks are printed.  Returns 0, or 3 after saying why it failed. */
+static int salvage(sv_ctx *ctx, const char *path, const uint8_t *store, size_t len, uint8_t *out) {
+    size_t cap = 1024;
+    sv_gossip_salvage_summary v;
+    uint64_t *off = NULL, *resume = NULL;
+    uint8_t *kind = NULL;
+    for (;;) { /* again with room for every break when the first guess was short */
+        free(off); free(resume); free(kind);
+        off = malloc(8 * cap);
+        resume = malloc(8 * cap);
+        kind = malloc(cap);
+        if (!off || !resume || !kind) { fprintf(stderr, "out of memory\n"); return 3; }
+        int rc = sv_salvage_gossip_store_host(ctx, store, len, out, off, resume, kind, cap, &v);
+        if (rc != SV_OK) { fprintf(stderr, "sv_salvage_gossip_store_host: %d %s\n", rc, sv_last_error(ctx)); return 3; }
+        if (v.breaks <= cap) break;
+        cap = (size_t)v.breaks;
+    }
+    for (uint64_t i = 0; i < v.breaks; i++)
+        printf("break @%" PRIu64 ": records resume at %" PRIu64 ", %s\n", off[i], resume[i],
+               kind[i] == SV_SALVAGE_RESTORED ? "header restored" : "span bridged with deleted fillers");
+    printf("salvage of %s: %" PRIu64 " sound records found, %" PRIu64 " breaks: %" PRIu64 " restored, %" PRIu64
+           " bridged (%" PRIu64 " bytes in %" PRIu64 " fillers)\n", path, v.sound, v.breaks, v.restored, v.bridged,
+           v.bridged_bytes, v.fillers);
+    free(off); free(resume); free(kind);
+    return 0;
+}
+
 /* --prune: write the pruned copy (cut_tail: without its torn tail), report it, audit it; returns the exit code */
 static int prune(sv_ctx *ctx, const char *path, const uint8_t *store, size_t len, const uint8_t *chain, const char *outp,
                  int cut_tail, const sv_funding_table *table) {
@@ -215,7 +247,7 @@ static int prune(sv_ctx *ctx, const char *path, const uint8_t *store, size_t len
 int main(int argc, char **argv) {
     const char *path = NULL, *prune_out = NULL, *funding_path = NULL;
     uint8_t chain[32];
-    int have_chain = 0, device = 0, cut_tail = 0;
+    int have_chain = 0, device = 0, cut_tail = 0, salv = 0;
     for (int i = 1; i < argc; i++) {
         if (!strcmp(argv[i], "--chain") && i + 1 < argc) {
             const char *h = argv[++i];
@@ -234,6 +266,8 @@ int main(int argc, char **argv) {
             funding_path = argv[++i];
         } else if (!strcmp(argv[i], "--cut-tail")) {
             cut_tail = 1;
+        } else if (!strcmp(argv[i], "--salvage")) {
+            salv = cut_tail = 1;
         } else if (argv[i][0] == '-' || path) {
             return usage();
         } else {
@@ -264,7 +298,14 @@ int main(int argc, char **argv) {
     sv_ctx *ctx = NULL;
     if (sv_create(&ctx, device) != SV_OK) { fprintf(stderr, "engine: %s\n", sv_last_error(NULL)); return 3; }
     if (prune_out) {
-        int code = prune(ctx, path, store, len, have_chain ? chain : NULL, prune_out, cut_tail, table);
+        uint8_t *src = store;
+        int code = 0;
+        if (salv) {
+            src = malloc(len);
+            code = src ? salvage(ctx, path, store, len, src) : (fprintf(stderr, "out of memory\n"), 3);
+        }
+        if (!code) code = prune(ctx, path, src, len, have_chain ? chain : NULL, prune_out, cut_tail, table);
+        if (src != store) free(src);
         sv_destroy(ctx);
         free(store);
         return code;

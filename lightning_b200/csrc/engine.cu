@@ -35,6 +35,7 @@
 #include "verify.cuh"
 #include "bolt12.cuh"
 #include "gossip_store.cuh"
+#include "gossip_salvage.cuh"
 #include "gossip_funding.cuh"
 #include "selftest.cuh"
 #include "batch.cuh"  // constants and the host-testable stages; the kernels themselves are in batch.cu
@@ -637,6 +638,113 @@ __global__ void __launch_bounds__(256) k_store_finish(const u8* store, const u64
     if (m >= n) return;
     const u8* p = store + msg_off[m];
     if (p[0] == 1 && p[1] == 2 && holder[m] == GS_NONE && (status[m] == 0 || status[m] == 1)) status[m] = -2;
+}
+
+// ---- gossip_store salvage (gossip_salvage.cuh): every byte offset that holds a sound record -------------------------
+// k_salvage_filter: one thread per byte offset o = 1 + global thread index, 256 per block.  Without out, count[b] = the
+// candidates (gs_salvage_candidate) of block b.  With out, count holds each block's exclusive prefix (k_salvage_scan) and
+// every candidate goes to out[count[b] + its rank in the block]: the list is in store order.
+__global__ void __launch_bounds__(256) k_salvage_filter(const u8* store, u64 len, u64* count, u64* out) {
+    __shared__ u32 warp_n[8];
+    const u64 o = 1 + (u64)blockIdx.x * 256 + threadIdx.x;
+    const bool c = gs_salvage_candidate(store, len, o);
+    const unsigned m = __ballot_sync(~0u, c);
+    const u32 w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (lane == 0) warp_n[w] = __popc(m);
+    __syncthreads();
+    if (!out) {
+        if (threadIdx.x == 0) {
+            u64 n = 0;
+            for (int k = 0; k < 8; k++) n += warp_n[k];
+            count[blockIdx.x] = n;
+        }
+        return;
+    }
+    if (!c) return;
+    u64 r = count[blockIdx.x] + __popc(m & ((1u << lane) - 1));
+    for (u32 k = 0; k < w; k++) r += warp_n[k];
+    out[r] = o;
+}
+// one block: count[0, nb) replaced by its exclusive prefix sums, count[nb] = the total
+__global__ void __launch_bounds__(1024) k_salvage_scan(u64* count, size_t nb) {
+    __shared__ u64 ws[32];
+    __shared__ u64 carry;
+    const u32 lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    if (threadIdx.x == 0) carry = 0;
+    __syncthreads();
+    for (size_t base = 0; base < nb; base += 1024) {
+        const size_t i = base + threadIdx.x;
+        const u64 v = i < nb ? count[i] : 0;
+        u64 x = v;
+        for (int d = 1; d < 32; d <<= 1) {
+            const u64 y = __shfl_up_sync(~0u, x, d);
+            if (lane >= (u32)d) x += y;
+        }
+        if (lane == 31) ws[w] = x;
+        __syncthreads();
+        if (w == 0) {
+            u64 y = ws[lane];
+            for (int d = 1; d < 32; d <<= 1) {
+                const u64 z = __shfl_up_sync(~0u, y, d);
+                if (lane >= (u32)d) y += z;
+            }
+            ws[lane] = y;
+        }
+        __syncthreads();
+        const u64 before = carry + (w ? ws[w - 1] : 0) + x - v;
+        if (i < nb) count[i] = before;
+        __syncthreads();
+        if (threadIdx.x == 1023) carry = before + v;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) count[nb] = carry;
+}
+// k_salvage_crc: sound[i] = 1 if candidate i's checksum matches.  One thread per candidate; a candidate whose message is
+// longer than GS_SV_LONG (up to 65,535 bytes, mostly random offsets) is checksummed by its whole warp, one slice per
+// lane (gs_crc_lane), so it costs the warp about what a short candidate costs one thread.
+__global__ void __launch_bounds__(256) k_salvage_crc(const u8* store, const u64* cand, size_t n, u8* sound) {
+    __shared__ u32 tab[2048];
+    __shared__ u32 x2n[32];
+    for (u32 i = threadIdx.x; i < 256; i += blockDim.x) gs_crc_fill(tab, i);
+    if (threadIdx.x == 0) gs_crc_x2n(x2n);
+    __syncthreads();
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const u32 lane = threadIdx.x & 31;
+    const u64 o = i < n ? cand[i] : 0;
+    const u32 ml = i < n ? gs_be16(store + o + 2) : 0;
+    const bool lng = ml > GS_SV_LONG;
+    if (i < n && !lng) sound[i] = gs_record_crc_ok(tab, store, o);
+    for (unsigned m = __ballot_sync(~0u, lng); m; m &= m - 1) {
+        const u32 src = __ffs(m) - 1;
+        const u64 oo = __shfl_sync(~0u, o, src);
+        const u32 L = __shfl_sync(~0u, ml, src);
+        const u8* h = store + oo;
+        u32 r = gs_crc_lane(tab, x2n, h + GS_HDR, L, lane);
+        for (int d = 16; d; d >>= 1) r ^= __shfl_xor_sync(~0u, r, d);
+        if (lane == src) sound[i] = (gs_crc_shift(x2n, gs_be32(h + 8), L) ^ r) == gs_be32(h + 4);
+    }
+}
+// k_salvage_restore: one warp per break [t, q) the host walk found: restore[b] = 1 if the damaged header's checksum, with
+// its timestamp, covers exactly store[t + 12, q) (at most 65,535 bytes)
+__global__ void __launch_bounds__(256) k_salvage_restore(const u8* store, const u64* brk, size_t n, u8* restore) {
+    __shared__ u32 tab[2048];
+    __shared__ u32 x2n[32];
+    for (u32 i = threadIdx.x; i < 256; i += blockDim.x) gs_crc_fill(tab, i);
+    if (threadIdx.x == 0) gs_crc_x2n(x2n);
+    __syncthreads();
+    const size_t b = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / 32;
+    const u32 lane = threadIdx.x & 31;
+    if (b >= n) return;  // whole warps
+    const u64 t = brk[2 * b], q = brk[2 * b + 1];
+    if (!gs_restore_fits(t, q)) {
+        if (lane == 0) restore[b] = 0;
+        return;
+    }
+    const u8* h = store + t;
+    const u32 L = (u32)(q - t - GS_HDR);
+    u32 r = gs_crc_lane(tab, x2n, h + GS_HDR, L, lane);
+    for (int d = 16; d; d >>= 1) r ^= __shfl_xor_sync(~0u, r, d);
+    if (lane == 0) restore[b] = (gs_crc_shift(x2n, gs_be32(h + 8), L) ^ r) == gs_be32(h + 4);
 }
 
 // ---- gossip_store prune (sv_prune_gossip_store_host): the deletions, a second channel table and the flag writes ------
@@ -1319,6 +1427,7 @@ struct sv_ctx {
     float gs_ms[4] = {};         // last sv_verify_gossip_store_host: header walk, H2D, checksums, verification (profiling mode)
     float gp_ms[4] = {};         // last sv_prune_gossip_store_host: header walk, first round, second round, flag write
     float gf_ms[2] = {};         // last funding call: table staging and sort, k_store_funding
+    float gv_ms[3] = {};         // last sv_salvage_gossip_store_host: filter, checksums, host walk
     unsigned long long launches = 0;
     std::vector<sv_queue_item> queue;
     std::string err;
@@ -2636,6 +2745,112 @@ extern "C" int sv_prune_gossip_store_funding_host(sv_ctx* ctx, const uint8_t* st
 extern "C" int sv_get_last_gossip_prune_timing(sv_ctx* ctx, float* ms4) {
     if (!ctx || !ctx->profiling || !ms4) return SV_ERR_ARG;
     for (int i = 0; i < 4; i++) ms4[i] = ctx->gp_ms[i];
+    return SV_OK;
+}
+
+// ---- salvaging a gossip_store past damaged record headers (see cln_sigverify.h) -----------------------------------
+// The store staged once: the sorted sound offsets (the filter twice around the scan, then the checksums), the host walk's
+// breaks, and the restore check of each.  gv_ms (profiling mode): the two filter passes and the scan (device events
+// around the kernels only: e[0]..e[1] and e[2]..e[3], without the count's copy back and the candidate buffer's
+// allocation between them), the checksums (e[3]..e[4]), the host walk.
+static int salvage_run(sv_ctx* ctx, const uint8_t* store, size_t len, std::vector<u64>& sound, std::vector<u64>& brk,
+                       std::vector<u8>& restore) {
+    for (float& ms : ctx->gv_ms) ms = 0;
+    if (len < 1 + GS_HDR + 2) return SV_OK;  // no record fits
+    cudaStream_t st = ctx->stream;
+    const u64 nb = (len - 1 + 255) / 256;
+    ev_set E;
+    if (ctx->profiling)
+        for (int i = 0; i < 5; i++) CK(cudaEventCreate(&E.e[i]));
+    dev_buf<> d_store, d_cnt, d_cand, d_brk;
+    int rc = d_store.reserve(ctx, len, len);
+    if (!rc) rc = d_cnt.reserve(ctx, 8 * (nb + 1), 8 * (nb + 1));
+    if (rc) return rc;
+    u64* cnt = d_cnt.at<u64>(0);
+    CK(cudaMemcpyAsync(d_store, store, len, cudaMemcpyHostToDevice, st));
+    if (E.e[0]) CK(cudaEventRecord(E.e[0], st));
+    k_salvage_filter<<<(unsigned)nb, 256, 0, st>>>(d_store, len, cnt, nullptr);
+    k_salvage_scan<<<1, 1024, 0, st>>>(cnt, nb);
+    ctx->launches += 2;
+    if (E.e[1]) CK(cudaEventRecord(E.e[1], st));
+    u64 n = 0;
+    CK(cudaMemcpyAsync(&n, cnt + nb, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (n) {
+        rc = d_cand.reserve(ctx, 9 * n, 9 * n);
+        if (rc) return rc;
+        u64* cand = d_cand.at<u64>(0);
+        u8* ok = d_cand.at<u8>(8 * n);
+        if (E.e[2]) CK(cudaEventRecord(E.e[2], st));
+        k_salvage_filter<<<(unsigned)nb, 256, 0, st>>>(d_store, len, cnt, cand);
+        if (E.e[3]) CK(cudaEventRecord(E.e[3], st));
+        k_salvage_crc<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_store, cand, n, ok);
+        ctx->launches += 2;
+        if (E.e[4]) CK(cudaEventRecord(E.e[4], st));
+        std::vector<u64> c(n);
+        std::vector<u8> good(n);
+        CK(cudaMemcpyAsync(c.data(), cand, 8 * n, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(good.data(), ok, n, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        for (u64 k = 0; k < n; k++)
+            if (good[k]) sound.push_back(c[k]);
+    } else if (E.e[0]) {
+        for (int i = 2; i < 5; i++) CK(cudaEventRecord(E.e[i], st));
+        CK(cudaStreamSynchronize(st));
+    }
+    if (E.e[0]) {
+        float a, b;
+        CK(cudaEventElapsedTime(&a, E.e[0], E.e[1]));
+        CK(cudaEventElapsedTime(&b, E.e[2], E.e[3]));
+        ctx->gv_ms[0] = a + b;
+        CK(cudaEventElapsedTime(&ctx->gv_ms[1], E.e[3], E.e[4]));
+    }
+    const auto t0 = std::chrono::steady_clock::now();
+    gs_salvage_breaks(store, len, sound.data(), sound.size(), [&brk](u64 t, u64 q) { brk.push_back(t); brk.push_back(q); });
+    ctx->gv_ms[2] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    const size_t nbrk = brk.size() / 2;
+    restore.assign(nbrk, 0);
+    if (!nbrk) return SV_OK;
+    rc = d_brk.reserve(ctx, 17 * nbrk, 17 * nbrk);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(d_brk, brk.data(), 16 * nbrk, cudaMemcpyHostToDevice, st));
+    k_salvage_restore<<<(unsigned)((nbrk + 7) / 8), 256, 0, st>>>(d_store, d_brk.at<u64>(0), nbrk, d_brk + 16 * nbrk);
+    ctx->launches += 1;
+    CK(cudaMemcpyAsync(restore.data(), d_brk + 16 * nbrk, nbrk, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return SV_OK;
+}
+extern "C" int sv_salvage_gossip_store_host(sv_ctx* ctx, const uint8_t* store, size_t len, uint8_t* out, uint64_t* act_off,
+                                            uint64_t* act_resume, uint8_t* act_kind, size_t act_capacity,
+                                            sv_gossip_salvage_summary* sum) {
+    if (!ctx || !store || !out || len < 1 || !sum || (act_capacity && (!act_off || !act_resume || !act_kind)))
+        return SV_ERR_ARG;
+    if (store[0] >> 5) return fail(ctx, SV_ERR_ARG, "gossip_store major version is not 0", cudaSuccess);
+    dev_guard dg;
+    CK(dg.enter(ctx->device));
+    std::vector<u64> sound, brk;
+    std::vector<u8> restore;
+    int rc = salvage_run(ctx, store, len, sound, brk, restore);
+    if (rc) return rc;
+    const size_t n = restore.size();
+    std::vector<u64> t(n), q(n);
+    for (size_t i = 0; i < n; i++) {
+        t[i] = brk[2 * i];
+        q[i] = brk[2 * i + 1];
+        if (i < act_capacity) {
+            act_off[i] = t[i];
+            act_resume[i] = q[i];
+            act_kind[i] = restore[i] ? SV_SALVAGE_RESTORED : SV_SALVAGE_BRIDGED;
+        }
+    }
+    if (out != store) memcpy(out, store, len);
+    const gs_salvage_count c = gs_salvage_apply(out, t.data(), q.data(), restore.data(), n);
+    *sum = sv_gossip_salvage_summary{c.breaks, c.restored, c.bridged, c.bridged_bytes, c.fillers, (uint64_t)sound.size()};
+    return SV_OK;
+}
+extern "C" int sv_get_last_gossip_salvage_timing(sv_ctx* ctx, float* ms3) {
+    if (!ctx || !ctx->profiling || !ms3) return SV_ERR_ARG;
+    for (int i = 0; i < 3; i++) ms3[i] = ctx->gv_ms[i];
     return SV_OK;
 }
 

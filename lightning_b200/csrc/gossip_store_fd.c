@@ -8,6 +8,7 @@
  */
 #define _GNU_SOURCE
 #include "../../include/cln_sigverify.h"
+#include "gossip_store_fd.h"
 
 #include <errno.h>
 #include <fcntl.h>
@@ -18,8 +19,7 @@
 
 #define IO_CHUNK ((size_t)1 << 30) /* bytes per pread / pwrite call */
 
-/* len bytes from offset 0; -1 with errno on failure (EIO: the file ended early) */
-static int read_all(int fd, uint8_t *p, size_t len) {
+int gsfd_read_all(int fd, uint8_t *p, size_t len) {
     size_t got = 0;
     while (got < len) {
         size_t want = len - got < IO_CHUNK ? len - got : IO_CHUNK;
@@ -32,7 +32,7 @@ static int read_all(int fd, uint8_t *p, size_t len) {
     return 0;
 }
 
-static int write_at(int fd, const uint8_t *p, size_t len, uint64_t off) {
+int gsfd_write_at(int fd, const uint8_t *p, size_t len, uint64_t off) {
     while (len) {
         ssize_t w = pwrite(fd, p, len, (off_t)off);
         if (w < 0 && errno == EINTR) continue;
@@ -44,7 +44,7 @@ static int write_at(int fd, const uint8_t *p, size_t len, uint64_t off) {
     return 0;
 }
 
-static int sync_fd(int fd) {
+int gsfd_sync(int fd) {
     while (fsync(fd) < 0)
         if (errno != EINTR) return -1;
     return 0;
@@ -90,16 +90,22 @@ uint64_t sv_gossip_prune_cut(const sv_gossip_prune_summary *s, const uint8_t *pr
     return cut;
 }
 
-/* sv_prune_gossip_store_fd; with cut, also where the repair ends the file (sv_gossip_prune_cut of the pruned store) */
-static int prune_file(sv_ctx *ctx, int fd, uint64_t len, const uint8_t *chain_hash32, sv_gossip_prune_summary *summary,
-                      uint64_t *cut) {
+int gsfd_check(int fd, uint64_t len) {
     struct stat st;
-    if (!ctx || !summary) { errno = EINVAL; return SV_ERR_ARG; }
     int fl = fcntl(fd, F_GETFL);
     if (fl < 0) return SV_ERR_IO; /* errno EBADF: not an open descriptor */
     if (fstat(fd, &st) < 0) return SV_ERR_IO;
     if (!S_ISREG(st.st_mode) || len < 1 || len > (uint64_t)st.st_size || len > SIZE_MAX) { errno = EINVAL; return SV_ERR_ARG; }
     if ((fl & O_ACCMODE) != O_RDWR) { errno = EBADF; return SV_ERR_IO; } /* the deletions could not be written */
+    return SV_OK;
+}
+
+/* sv_prune_gossip_store_fd; with cut, also where the repair ends the file (sv_gossip_prune_cut of the pruned store) */
+static int prune_file(sv_ctx *ctx, int fd, uint64_t len, const uint8_t *chain_hash32, sv_gossip_prune_summary *summary,
+                      uint64_t *cut) {
+    if (!ctx || !summary) { errno = EINVAL; return SV_ERR_ARG; }
+    int chk = gsfd_check(fd, len);
+    if (chk != SV_OK) return chk;
     uint8_t *store = (uint8_t *)malloc((size_t)len);
     if (!store) return SV_ERR_NOMEM;
     int rc = SV_ERR_IO, e = 0;
@@ -107,7 +113,7 @@ static int prune_file(sv_ctx *ctx, int fd, uint64_t len, const uint8_t *chain_ha
     uint16_t *rec_type = NULL;
     int *rec_status = NULL;
     uint8_t *rec_pruned = NULL;
-    if (read_all(fd, store, (size_t)len) < 0) { e = errno; goto out; }
+    if (gsfd_read_all(fd, store, (size_t)len) < 0) { e = errno; goto out; }
     size_t cap = sv_gossip_prune_count(store, (size_t)len);
     rec_off = (uint64_t *)malloc(8 * (cap + 1));
     rec_type = (uint16_t *)malloc(2 * (cap + 1));
@@ -118,8 +124,8 @@ static int prune_file(sv_ctx *ctx, int fd, uint64_t len, const uint8_t *chain_ha
                                     cap, summary);
     if (rc != SV_OK) { e = rc == SV_ERR_ARG ? EINVAL : 0; goto out; }
     for (uint64_t r = 0; r < summary->records; r++)
-        if (rec_pruned[r] && write_at(fd, store + rec_off[r], 2, rec_off[r]) < 0) { rc = SV_ERR_IO; e = errno; goto out; }
-    if (sync_fd(fd) < 0) { rc = SV_ERR_IO; e = errno; goto out; }
+        if (rec_pruned[r] && gsfd_write_at(fd, store + rec_off[r], 2, rec_off[r]) < 0) { rc = SV_ERR_IO; e = errno; goto out; }
+    if (gsfd_sync(fd) < 0) { rc = SV_ERR_IO; e = errno; goto out; }
     if (cut) *cut = sv_gossip_prune_cut(summary, store, len);
 out:
     free(store); free(rec_off); free(rec_type); free(rec_status); free(rec_pruned);
@@ -140,8 +146,9 @@ int sv_repair_gossip_store_fd(sv_ctx *ctx, int fd, uint64_t len, const uint8_t *
     if (cut < len) {
         int r;
         while ((r = ftruncate(fd, (off_t)cut)) < 0 && errno == EINTR) {}
-        if (r < 0 || sync_fd(fd) < 0) return SV_ERR_IO;
+        if (r < 0 || gsfd_sync(fd) < 0) return SV_ERR_IO;
     }
     if (new_len) *new_len = cut;
     return SV_OK;
 }
+

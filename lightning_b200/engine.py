@@ -64,6 +64,15 @@ GP_KEPT, GP_BAD_CRC, GP_TRUNCATED, GP_MESSAGE, GP_REDUNDANT, GP_NO_CHANNEL, GP_S
 GP_REASONS = ("kept", "bad_crc", "truncated", "message", "redundant", "no_channel", "signature", "amount", "unknown")
 
 
+class SvGossipSalvageSummary(ctypes.Structure):
+    """sv_gossip_salvage_summary (include/cln_sigverify.h)"""
+    _fields_ = [(f, ctypes.c_uint64) for f in ("breaks", "restored", "bridged", "bridged_bytes", "fillers", "sound")]
+
+
+# what salvage_gossip_store did at a break (include/cln_sigverify.h SV_SALVAGE_*)
+SALVAGE_RESTORED, SALVAGE_BRIDGED = 1, 2
+
+
 class SvFundingTable(ctypes.Structure):
     """sv_funding_table (include/cln_sigverify.h)"""
     _fields_ = [("scid", ctypes.c_void_p), ("satoshis", ctypes.c_void_p), ("script34", ctypes.c_void_p),
@@ -137,6 +146,10 @@ def load_library():
                                               ctypes.POINTER(ctypes.c_uint64)]
     lib.sv_gossip_prune_cut.restype = ctypes.c_uint64
     lib.sv_gossip_prune_cut.argtypes = [ctypes.POINTER(SvGossipPruneSummary), ctypes.c_char_p, ctypes.c_uint64]
+    lib.sv_salvage_gossip_store_host.argtypes = [vp, vp, sz, vp, vp, vp, vp, sz, ctypes.POINTER(SvGossipSalvageSummary)]
+    lib.sv_salvage_gossip_store_fd.argtypes = [vp, i, ctypes.c_uint64, vp, ctypes.POINTER(SvGossipPruneSummary),
+                                               ctypes.POINTER(SvGossipSalvageSummary), ctypes.POINTER(ctypes.c_uint64)]
+    lib.sv_get_last_gossip_salvage_timing.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
     lib.sv_verify_tx_host.argtypes = [vp, i, vp, vp, sz, vp, vp, sz, vp, vp]
     lib.sv_grind_tx_fee_host.argtypes = [vp, i, vp, vp, sz, vp, vp, ctypes.c_uint64, ctypes.c_uint32, ctypes.c_uint32,
                                          ctypes.POINTER(ctypes.c_int64), ctypes.POINTER(ctypes.c_uint64)]
@@ -405,6 +418,47 @@ class SigVerifier:
         pruned = bytes(pruned)
         return int(self.lib.sv_gossip_prune_cut(ctypes.byref(s), pruned, len(pruned)))
 
+    def salvage_gossip_store(self, store, capacity=1024):
+        """Mend the chain of record lengths of a gossip_store past damaged headers (sv_salvage_gossip_store_host; the rule
+        is in include/cln_sigverify.h): each break's header is restored, or the span up to where the records resume is
+        covered by deleted filler records.  Returns (salvaged bytes, actions, summary dict): the store with those header
+        writes (same length; the input is not changed), and one (offset, resume, SALVAGE_RESTORED or SALVAGE_BRIDGED)
+        per break in store order.  capacity: actions to make room for; with more breaks the call is made again with room
+        for all."""
+        buf = np.frombuffer(bytes(store), dtype=np.uint8)
+        while True:
+            out = np.empty(max(buf.size, 1), np.uint8)
+            off, resume, kind = np.zeros(max(capacity, 1), np.uint64), np.zeros(max(capacity, 1), np.uint64), \
+                np.zeros(max(capacity, 1), np.uint8)
+            s = SvGossipSalvageSummary()
+            self._check(self.lib.sv_salvage_gossip_store_host(
+                self._ctx, buf.ctypes.data, buf.size, out.ctypes.data, off.ctypes.data, resume.ctypes.data, kind.ctypes.data,
+                capacity, ctypes.byref(s)), "sv_salvage_gossip_store_host")
+            if s.breaks <= capacity:
+                break
+            capacity = s.breaks
+        acts = [(int(off[k]), int(resume[k]), int(kind[k])) for k in range(s.breaks)]
+        return out[:buf.size].tobytes(), acts, {f: getattr(s, f) for f, _ in SvGossipSalvageSummary._fields_}
+
+    def salvage_gossip_store_fd(self, fd, length, chain_hash=None):
+        """salvage_gossip_store on a FILE, in place, then repair_gossip_store_fd (sv_salvage_gossip_store_fd): only the
+        4 bytes of flags and length of each header the salvage changed are written, a bridge's fillers from the last to
+        the first.  Returns (the repair's summary dict, the salvage's summary dict, new_len).  Errors as
+        repair_gossip_store_fd."""
+        chain = None if chain_hash is None else _chain_hash(chain_hash)
+        s, v, new_len = SvGossipPruneSummary(), SvGossipSalvageSummary(), ctypes.c_uint64(0)
+        rc = self.lib.sv_salvage_gossip_store_fd(self._ctx, int(fd), int(length), chain.ctypes.data if chain is not None else None,
+                                                 ctypes.byref(s), ctypes.byref(v), ctypes.byref(new_len))
+        self._check_fd(rc, "sv_salvage_gossip_store_fd")
+        return ({f: getattr(s, f) for f, _ in SvGossipPruneSummary._fields_},
+                {f: getattr(v, f) for f, _ in SvGossipSalvageSummary._fields_}, int(new_len.value))
+
+    def last_gossip_salvage_timing(self):
+        """(filter kernels with the scan, checksum kernel, host walk) in ms of the last salvage (profiling mode)"""
+        ms = (ctypes.c_float * 3)()
+        self._check(self.lib.sv_get_last_gossip_salvage_timing(self._ctx, ms), "sv_get_last_gossip_salvage_timing")
+        return tuple(ms)
+
     def _store_fd(self, repair, fd, length, chain_hash):
         chain = None if chain_hash is None else _chain_hash(chain_hash)
         s, new_len = SvGossipPruneSummary(), ctypes.c_uint64(0)
@@ -415,11 +469,15 @@ class SigVerifier:
         else:
             name = "sv_prune_gossip_store_fd"
             rc = self.lib.sv_prune_gossip_store_fd(self._ctx, int(fd), int(length), cp, ctypes.byref(s))
+        self._check_fd(rc, name)
+        return {f: getattr(s, f) for f, _ in SvGossipPruneSummary._fields_}, int(new_len.value)
+
+    def _check_fd(self, rc, name):
+        """a file call's refusal (SV_ERR_ARG, SV_ERR_IO) as OSError with its errno; other failures as EngineError"""
         if rc in (SV_ERR_ARG, SV_ERR_IO):
             e = ctypes.get_errno() or errno.EINVAL
             raise OSError(e, f"{name}: {os.strerror(e)}")
         self._check(rc, name)
-        return {f: getattr(s, f) for f, _ in SvGossipPruneSummary._fields_}, int(new_len.value)
 
     def last_gossip_prune_timing(self):
         """(header walk, first round, second round, flag write) in ms of the last prune_gossip_store (profiling mode)"""
