@@ -24,6 +24,11 @@
  *                                           :1501-1507, lightningd/offer.c:88-89, devtools/bolt12-cli.c:319-321
  *   sv_verify_bolt12_tagged_host(...)       the same checks, many callers' tags in one batch (the verifier
  *                                           subdaemon serves the plugins' bolt12_check_signature calls with it)
+ *   sv_verify_bolt11_host(...)              bolt11_decode()'s signature step common/bolt11.c:980-1062 (bech32,
+ *                                           the field walk of bolt11_decode_nosig :887-936, hash_u5's signing hash,
+ *                                           then secp256k1_ecdsa_verify against `n` or secp256k1_ecdsa_recover);
+ *                                           run by every invoice string given to pay, xpay, renepay, decode,
+ *                                           listsendpays and listinvoices
  *   sv_verify_gossip_burst_host(...)        gossipd's signature gate over a burst: parse, node-id order and chain
  *                                           gates gossipd/gossmap_manage.c:659-670, :1048-1051, sigcheck_*, and the
  *                                           pending map that gives a channel_update its signer (:695-703,
@@ -573,6 +578,30 @@ int sv_verify_bolt12_tagged_host(sv_ctx *ctx, size_t ntags, const char *const *m
                                  const uint32_t *len, const uint8_t *xonly32, const uint8_t *sig64, size_t n,
                                  int *status, uint8_t *sighash32_out);
 
+/* ---- BOLT11 invoice signatures, everything on the device: bolt11_decode's signature step (common/bolt11.c:980-1062)
+ *      for n invoice strings.  Invoice i is blob[off[i] .. off[i]+len[i]), read up to its first NUL byte as strlen would
+ *      read it, exactly as bolt11_decode receives it (no "lightning:" prefix is stripped; callers lower-case and strip it
+ *      with to_canonical_invstr).  No bound on invoice length beyond the 32-bit span.
+ *      status[i] = -1  the structure that locates the signed bytes and the key is unsound: bech32_decode refuses the
+ *                      string (fewer than 8 characters, a character outside 33..126, mixed case, no '1', fewer than 6
+ *                      checksum characters, a bad checksum) or gives BECH32M; the 35-bit timestamp cannot be read; the
+ *                      tagged-field walk fails (a tag or length it cannot read, a field longer than what is left); the walk
+ *                      does not end with exactly 104 words for the signature; the first 53-word `n` field (a later one
+ *                      is an unknown field) has a non-zero trailing bit or is not a valid compressed key;
+ *                   0  the signature step refuses: recovery id above 3, r >= n or s >= n; with `n`,
+ *                      secp256k1_ecdsa_verify is false (high-S included); without `n`, secp256k1_ecdsa_recover fails
+ *                      (r = 0, s = 0, recid & 2 with r + n >= p, R.x off the curve, Q = infinity; high-S is accepted);
+ *                   1  the signature step accepts.
+ *      node_id33_out (n x 33): the receiver_id bolt11_decode would set (the `n` key, or the recovered key compressed)
+ *      where status is 1, zeros elsewhere.  hash32_out (optional, n x 32): hash_u5's signing hash, SHA-256 of the
+ *      lowercased hrp and every word before the signature packed to bytes and zero-padded; zeros where status is -1.
+ *      NOT checked on the device (field values the caller's own decode handles, so an invoice bolt11_decode refuses for
+ *      one of them can still get status 1): the hrp's "ln" prefix, chain and amount; whether p, s and one of d / h are
+ *      present; trailing bits of p / h / s; UTF-8 in d; x, c, f, r, m; 9 against our_features; h against a description.
+ *      Spans out of range or NULL required pointers: SV_ERR_ARG.  n == 0 is valid. ---- */
+int sv_verify_bolt11_host(sv_ctx *ctx, const uint8_t *blob, size_t blob_len, const uint64_t *off, const uint32_t *len,
+                          size_t n, int *status, uint8_t *node_id33_out, uint8_t *hash32_out);
+
 /* ---- DEVICE buffers (same SoA layout, device pointers); asynchronous on `stream`
  *      (a cudaStream_t passed as void*; NULL = the context's own stream).  d_verdicts[n] bytes;
  *      d_bitmap, if non-NULL, receives ceil(n/32) little-endian 32-bit words, bit i%32 of word i/32. ---- */
@@ -687,6 +716,8 @@ int sv_set_profiling(sv_ctx *ctx, int on);
 int sv_get_last_timing(sv_ctx *ctx, float *prep_ms, float *main_ms);
 /* the same for the last sv_verify_bolt12_host call: parse + Merkle + sighash kernels, then the verification kernels */
 int sv_get_last_bolt12_timing(sv_ctx *ctx, float *merkle_ms, float *verify_ms);
+/* the same for the last sv_verify_bolt11_host call: parse + hash kernels, then the verification and recovery kernels */
+int sv_get_last_bolt11_timing(sv_ctx *ctx, float *parse_ms, float *curve_ms);
 
 /* integer-pipe roofline probe: runs a dependent-chain IMAD.WIDE.U32 microbenchmark and returns the
  * achieved 32x32->64 multiply-accumulates per second on this device (the roofline denominator

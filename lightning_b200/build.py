@@ -9,6 +9,7 @@ Everything is built IN-TREE, so the package and the tests run from the source tr
   oracle/_ref/libcln_ref.so, libcln_bolt12.so, libcln_gossmap.so   CLN's own plumbing, BOLT12 Merkle code and
                                         gossip_store loader (common/gossmap.c) from the same tree [gcc]
   oracle/_ref/libcln_funding.so         CLN's funding script (bitcoin/script.c bitcoin_redeem_2of2) from the same tree [gcc]
+  oracle/_ref/libcln_bolt11.so          CLN's BOLT11 decoder (common/bolt11.c bolt11_decode) from the same tree [gcc]
 """
 import os
 import shutil
@@ -110,7 +111,7 @@ def build_engine(force=False, verbose=False):
 def build_host_emul(force=False):
     src = [os.path.join(ROOT, "tests", "host_emul", f) for f in ("emul.cpp", "bolt12_emul.cpp", "gossip_store_emul.cpp",
                                                              "gossip_funding_emul.cpp", "fee_grind_emul.cpp",
-                                                             "gossip_salvage_emul.cpp")]
+                                                             "gossip_salvage_emul.cpp", "bolt11_emul.cpp")]
     srcs = _sources(CSRC, (".cuh",)) + src
     if not force and _newer(EMUL, srcs):
         return EMUL
@@ -146,6 +147,11 @@ def build_oracle():
                        text=True, stdin=subprocess.DEVNULL, timeout=900)
     if r.returncode != 0:
         raise RuntimeError("oracle build (funding.mk) failed:\n" + r.stdout + r.stderr)
+    # the reference's BOLT11 decoder (common/bolt11.c), linked against the library of the `cln` target
+    r = subprocess.run(["make", "-C", os.path.join(ROOT, "oracle"), "-f", "bolt11.mk", "all"], capture_output=True,
+                       text=True, stdin=subprocess.DEVNULL, timeout=900)
+    if r.returncode != 0:
+        raise RuntimeError("oracle build (bolt11.mk) failed:\n" + r.stdout + r.stderr)
 
 
 def build_all(force=False, verbose=False):

@@ -14,6 +14,8 @@
 //       k_main_shared, k_dedup_*, k_sharedkey_build_many   one multiples table per distinct key (same-key / gossip batches)
 //       k_gossip_slice / _status, k_bip143, k_mixed_*       callers' data formats on the device (rows N1, N2, C3)
 //       k_b12_*                          BOLT12 streams: TLV parse, Merkle root (one warp per stream), tagged sighash
+//       k_b11_*                          BOLT11 invoices: bech32, field walk, signing hash; public-key recovery around
+//                                        k_main<SV_KIND_SCHNORR> (prep of u1, u2 and R.x, then affine Q compressed)
 //       k_sb_* (batch.cu)                BIP-340 batch verification by random linear combination
 //       k_pack_bitmap                    verdict bytes -> 1 bit per verification (ballot)
 //       k_pubkey_parse                   batched pubkey_from_der
@@ -34,6 +36,7 @@
 #include "../../include/cln_sigverify.h"
 #include "verify.cuh"
 #include "bolt12.cuh"
+#include "bolt11.cuh"
 #include "gossip_store.cuh"
 #include "gossip_salvage.cuh"
 #include "gossip_funding.cuh"
@@ -995,6 +998,75 @@ __global__ void __launch_bounds__(256) k_b12_status(const u32* cnt, const u8* ve
     if (i < n) status[i] = cnt[i] ? (int)verdict[i] : -1;
 }
 
+// ---- BOLT11 invoices (bolt11.cuh): bolt11_decode's signature step ----------------------------------------------------
+// k_b11_parse: one thread per invoice: bech32, the field walk, the `n` key, the signature bytes and the signing hash.
+// is_n / is_r flag the invoices verified against their `n` key and the ones whose key is recovered (0 / 0: status -1).
+__global__ void __launch_bounds__(128) k_b11_parse(const u8* blob, const u64* off, const u32* len, size_t n, u8* msg32,
+                                                   u8* key33, u8* sig64, u8* recid, u32* is_n, u32* is_r) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const u8* s = blob + off[i];
+    b11_str b;
+    b11_parsed p;
+    const bool ok = b11_parse(s, len[i], &b, &p);
+    if (ok) {
+        b11_sighash(msg32 + 32 * i, s, b);
+        for (int k = 0; k < 64; k++) sig64[64 * i + k] = p.sig[k];
+        for (int k = 0; k < 33; k++) key33[33 * i + k] = p.key33[k];
+        recid[i] = p.recid;
+    } else {
+        for (int k = 0; k < 32; k++) msg32[32 * i + k] = 0;
+    }
+    is_n[i] = ok && p.have_n;
+    is_r[i] = ok && !p.have_n;
+}
+// the `n` invoices, packed (base_n: exclusive prefix sum of is_n) for the ordinary compressed-key ECDSA path
+__global__ void __launch_bounds__(128) k_b11_gather_n(const u32* is_n, const u64* base_n, size_t n, const u8* msg32,
+                                                      const u8* key33, const u8* sig64, u8* cmsg, u8* ckey, u8* csig) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || !is_n[i]) return;
+    const size_t j = base_n[i];
+    for (int k = 0; k < 32; k++) cmsg[32 * j + k] = msg32[32 * i + k];
+    for (int k = 0; k < 33; k++) ckey[33 * j + k] = key33[33 * i + k];
+    for (int k = 0; k < 64; k++) csig[64 * j + k] = sig64[64 * i + k];
+}
+// the recovered invoices, packed: R's x (the ladder's x-only key) and the work record of u1 = -e / r, u2 = +-s / r
+__global__ void __launch_bounds__(128) k_b11_rec_prep(const u32* is_r, const u64* base_r, size_t n, const u8* msg32,
+                                                      const u8* sig64, const u8* recid, u8* x32, sv_work* work) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || !is_r[i]) return;
+    const size_t j = base_r[i];
+    sv_work w;
+    b11_recover_prep(w, x32 + 32 * j, sig64 + 64 * i, recid[i], msg32 + 32 * i);
+    work[j] = w;
+}
+// Q = u1 G + u2 E as k_main<SV_KIND_SCHNORR> parked it: affine, checked, compressed (SV_FINAL_BATCH per thread)
+__global__ void __launch_bounds__(64) k_b11_rec_final(const sv_work* work, size_t n, int* rstat, u8* rkey33) {
+    size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    size_t base = t * SV_FINAL_BATCH;
+    if (base >= n) return;
+    int cnt = (int)((n - base < SV_FINAL_BATCH) ? (n - base) : SV_FINAL_BATCH);
+    b11_recover_final_batch(rstat + base, rkey33 + 33 * base, reinterpret_cast<const sv_jac*>(work) + base, cnt);
+}
+// status and receiver_id of every invoice, from whichever path it took
+__global__ void __launch_bounds__(256) k_b11_status(const u32* is_n, const u64* base_n, const u32* is_r, const u64* base_r,
+                                                    size_t n, const u8* recid, const u8* key33, const u8* verdict_n,
+                                                    const int* rstat, const u8* rkey33, int* status, u8* node33) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    int st = -1;
+    const u8* key = nullptr;
+    if (is_n[i]) {
+        st = (recid[i] <= 3 && verdict_n[base_n[i]]) ? 1 : 0;  // recid > 3 is refused before secp256k1_ecdsa_verify
+        key = key33 + 33 * i;
+    } else if (is_r[i]) {
+        st = rstat[base_r[i]];
+        key = rkey33 + 33 * base_r[i];
+    }
+    status[i] = st;
+    for (int k = 0; k < 33; k++) node33[33 * i + k] = st == 1 ? key[k] : 0;
+}
+
 static_assert(sizeof(sv_jac) == sizeof(sv_work), "R is parked in place of the work record");
 __global__ void __launch_bounds__(64) k_final_schnorr(const sv_work* work, const u8* sig, size_t n, u8* verdict) {
     size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1424,6 +1496,7 @@ struct sv_ctx {
     int profiling = 0;
     cudaEvent_t ev[3] = {};      // before prep, between prep and main, after main (profiling mode only)
     cudaEvent_t b12_ev[2] = {};  // around the BOLT12 parse / Merkle / sighash kernels (profiling mode only)
+    cudaEvent_t b11_ev[4] = {};  // around the BOLT11 parse stage, and around its curve stage (profiling mode only)
     float gs_ms[4] = {};         // last sv_verify_gossip_store_host: header walk, H2D, checksums, verification (profiling mode)
     float gp_ms[4] = {};         // last sv_prune_gossip_store_host: header walk, first round, second round, flag write
     float gf_ms[2] = {};         // last funding call: table staging and sort, k_store_funding
@@ -1609,6 +1682,7 @@ extern "C" void sv_destroy(sv_ctx* ctx) {
         if (sl.done) cudaEventDestroy(sl.done);
     for (cudaEvent_t e : ctx->ev) if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : ctx->b12_ev) if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : ctx->b11_ev) if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : ctx->h2d_ev) if (e) cudaEventDestroy(e);
     for (cudaStream_t s : {ctx->copy_stream, ctx->stream2, ctx->stream}) if (s) cudaStreamDestroy(s);
     delete ctx;  // the device buffers free themselves
@@ -1840,6 +1914,8 @@ extern "C" int sv_set_profiling(sv_ctx* ctx, int on) {
         for (int i = 0; i < 3; i++) CK(cudaEventCreate(&ctx->ev[i]));
     if (on && !ctx->b12_ev[0])
         for (int i = 0; i < 2; i++) CK(cudaEventCreate(&ctx->b12_ev[i]));
+    if (on && !ctx->b11_ev[0])
+        for (cudaEvent_t& e : ctx->b11_ev) CK(cudaEventCreate(&e));
     ctx->profiling = on ? 1 : 0;
     return SV_OK;
 }
@@ -1848,6 +1924,13 @@ extern "C" int sv_get_last_bolt12_timing(sv_ctx* ctx, float* merkle_ms, float* v
     if (!ctx || !ctx->profiling || !merkle_ms || !verify_ms) return SV_ERR_ARG;
     CK(cudaEventElapsedTime(merkle_ms, ctx->b12_ev[0], ctx->b12_ev[1]));
     CK(cudaEventElapsedTime(verify_ms, ctx->ev[0], ctx->ev[2]));
+    return SV_OK;
+}
+// device time of the last sv_verify_bolt11_host call: parse and hash stage, then the verification and recovery stage
+extern "C" int sv_get_last_bolt11_timing(sv_ctx* ctx, float* parse_ms, float* curve_ms) {
+    if (!ctx || !ctx->profiling || !parse_ms || !curve_ms) return SV_ERR_ARG;
+    CK(cudaEventElapsedTime(parse_ms, ctx->b11_ev[0], ctx->b11_ev[1]));
+    CK(cudaEventElapsedTime(curve_ms, ctx->b11_ev[2], ctx->b11_ev[3]));
     return SV_OK;
 }
 // device time of the last sv_verify_* launch pair (call after the stream has been synchronised)
@@ -3187,6 +3270,91 @@ extern "C" int sv_verify_bolt12_tagged_host(sv_ctx* ctx, size_t ntags, const cha
     if (n == 0) return SV_OK;
     return bolt12_pass(ctx, ntags, messagenames, fieldnames, tag_of, blob, blob_len, off, len, xonly32, sig64, n, status,
                        sighash32_out);
+}
+
+// ---- BOLT11: bolt11_decode's signature step (common/bolt11.c:980-1062) for n invoice strings ---------------------------
+// The host copies bytes only.  k_b11_parse gives every invoice its structure, signature and signing hash; two prefix sums
+// (the BOLT12 scan kernels) pack the invoices with an `n` key and the ones to recover.  One host synchronisation reads the
+// two counts.  `n` invoices then take the ordinary compressed-key ECDSA path (small-batch kernel or throughput kernels,
+// launch_verify).  Recovered invoices take k_b11_rec_prep, the plain-flow ladder k_main<SV_KIND_SCHNORR> (which parks the
+// Jacobian result) and k_b11_rec_final.  k_b11_status folds both into one int and one key per invoice.
+extern "C" int sv_verify_bolt11_host(sv_ctx* ctx, const uint8_t* blob, size_t blob_len, const uint64_t* off,
+                                     const uint32_t* len, size_t n, int* status, uint8_t* node_id33_out,
+                                     uint8_t* hash32_out) {
+    if (!ctx || (n && (!blob || !off || !len || !status || !node_id33_out))) return SV_ERR_ARG;
+    if (n == 0) return SV_OK;
+    dev_guard dg__;
+    CK(dg__.enter(ctx->device));
+    int rc = ensure_staging(ctx, n);
+    if (rc) return rc;
+    rc = stage_spans(ctx, blob, blob_len, off, len, n);
+    if (rc) return rc;
+    const size_t nb = (n + SV_B12_SCAN - 1) / SV_B12_SCAN;
+    // per-call scratch in the auxiliary slab.  Per invoice: flags, prefix sums, recovery id, `n` key, status and key out.
+    // Packed: the `n` invoices' message / key / signature, the recovered invoices' R.x, status and key.
+    slab_layout L;
+    const size_t o_isn = L.take(4 * n), o_bn = L.take(8 * n), o_sn = L.take(8 * (nb + 1)), o_isr = L.take(4 * n),
+                 o_br = L.take(8 * n), o_sr = L.take(8 * (nb + 1)), o_recid = L.take(n), o_key = L.take(33 * n),
+                 o_status = L.take(4 * n), o_node = L.take(33 * n), o_cmsg = L.take(32 * n), o_ckey = L.take(33 * n),
+                 o_csig = L.take(64 * n), o_x = L.take(32 * n), o_rstat = L.take(4 * n), o_rkey = L.take(33 * n);
+    rc = ensure_gbuf(ctx, L.size);
+    if (rc) return rc;
+    const dev_buf<>& G = ctx->g_buf;
+    u32 *is_n = G.at<u32>(o_isn), *is_r = G.at<u32>(o_isr);
+    u64 *base_n = G.at<u64>(o_bn), *sums_n = G.at<u64>(o_sn), *base_r = G.at<u64>(o_br), *sums_r = G.at<u64>(o_sr);
+    int *d_status = G.at<int>(o_status), *rstat = G.at<int>(o_rstat);
+    u8 *recid = G + o_recid, *key33 = G + o_key, *node = G + o_node, *cmsg = G + o_cmsg, *ckey = G + o_ckey,
+       *csig = G + o_csig, *x32 = G + o_x, *rkey = G + o_rkey;
+    cudaStream_t st = ctx->stream;
+    const unsigned g128 = (unsigned)((n + 127) / 128);
+    if (ctx->profiling) cudaEventRecord(ctx->b11_ev[0], st);
+    k_b11_parse<<<g128, 128, 0, st>>>(ctx->d_data, ctx->d_off, ctx->d_len, n, ctx->d_msg, key33, ctx->d_sig, recid, is_n, is_r);
+    for (int pass = 0; pass < 2; pass++) {
+        const u32* flag = pass ? is_r : is_n;
+        u64 *base = pass ? base_r : base_n, *sums = pass ? sums_r : sums_n;
+        k_b12_scan_local<<<(unsigned)nb, SV_B12_SCAN, 0, st>>>(flag, n, base, sums);
+        k_b12_scan_sums<<<1, SV_B12_SCAN, 0, st>>>(sums, nb);
+        k_b12_scan_add<<<(unsigned)nb, SV_B12_SCAN, 0, st>>>(base, n, sums);
+    }
+    k_b11_gather_n<<<g128, 128, 0, st>>>(is_n, base_n, n, ctx->d_msg, key33, ctx->d_sig, cmsg, ckey, csig);
+    ctx->launches += 8;
+    if (ctx->profiling) cudaEventRecord(ctx->b11_ev[1], st);
+    CK(cudaGetLastError());
+    u64 cnt[2] = {0, 0};
+    CK(cudaMemcpyAsync(&cnt[0], sums_n + nb, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&cnt[1], sums_r + nb, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (ctx->profiling) cudaEventRecord(ctx->b11_ev[2], st);
+    rc = launch_verify(ctx, SV_KIND_ECDSA33, cmsg, ckey, csig, (size_t)cnt[0], ctx->d_verdict, nullptr, st);
+    if (rc) return rc;
+    const size_t cr = (size_t)cnt[1];
+    if (cr) {
+        sv_ctx::slot_t* sl = nullptr;
+        rc = acquire_slot(ctx, cr, st, &sl);
+        if (rc) return rc;
+        apply_l2_policy(ctx, st, sl->d_scratch);
+        k_b11_rec_prep<<<g128, 128, 0, st>>>(is_r, base_r, n, ctx->d_msg, ctx->d_sig, recid, x32, sl->d_work);
+        // the plain BIP-340 curve kernel computes u1 G + u2 E for the x-only key E and parks it; it reads no signature
+        // and writes no verdict for this kind
+        k_main<SV_KIND_SCHNORR><<<main_grid_for(ctx, cr), SV_MAIN_BLOCK, 0, st>>>(sl->d_work, x32, csig, cr, ctx->d_gtab,
+                                                                                   sl->d_scratch, nullptr, nullptr);
+        const size_t threads = (cr + SV_FINAL_BATCH - 1) / SV_FINAL_BATCH;
+        k_b11_rec_final<<<(unsigned)((threads + 63) / 64), 64, 0, st>>>(sl->d_work, cr, rstat, rkey);
+        ctx->launches += 3;
+        CK(cudaGetLastError());
+        rc = release_slot(ctx, sl, st);
+        if (rc) return rc;
+    }
+    k_b11_status<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(is_n, base_n, is_r, base_r, n, recid, key33, ctx->d_verdict,
+                                                             rstat, rkey, d_status, node);
+    ctx->launches += 1;
+    if (ctx->profiling) cudaEventRecord(ctx->b11_ev[3], st);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(status, d_status, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(node_id33_out, node, 33 * n, cudaMemcpyDeviceToHost, st));
+    if (hash32_out) CK(cudaMemcpyAsync(hash32_out, ctx->d_msg, 32 * n, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return SV_OK;
 }
 
 // ---- BIP-340 batch verification, host entry (batch.cuh) --------------------------------------------------------------

@@ -157,6 +157,8 @@ def load_library():
     lib.sv_verify_bolt12_host.argtypes = [vp, ctypes.c_char_p, ctypes.c_char_p, vp, sz, vp, vp, vp, vp, sz, vp, vp]
     lib.sv_verify_bolt12_tagged_host.argtypes = [vp, sz, vp, vp, vp, vp, sz, vp, vp, vp, vp, sz, vp, vp]
     lib.sv_get_last_bolt12_timing.argtypes = [vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float)]
+    lib.sv_verify_bolt11_host.argtypes = [vp, vp, sz, vp, vp, sz, vp, vp, vp]
+    lib.sv_get_last_bolt11_timing.argtypes = [vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float)]
     lib.sv_sync.argtypes = [vp, vp]
     lib.sv_get_stream.argtypes = [vp]
     lib.sv_set_profiling.argtypes = [vp, i]
@@ -590,6 +592,45 @@ class SigVerifier:
         """(merkle_ms, verify_ms) device time of the last verify_bolt12 call; needs set_profiling(True)."""
         a, b = ctypes.c_float(), ctypes.c_float()
         self._check(self.lib.sv_get_last_bolt12_timing(self._ctx, ctypes.byref(a), ctypes.byref(b)), "sv_get_last_bolt12_timing")
+        return a.value, b.value
+
+    def verify_bolt11(self, invoices):
+        """bolt11_decode's signature step (common/bolt11.c:980-1062) for a list of invoice strings (str or bytes-like, as
+        bolt11_decode receives them: no "lightning:" prefix).  Returns (status (n,) int32, node_id33 (n, 33), hash32 (n, 32)):
+        status 1 the signature step accepts, 0 it refuses, -1 the structure that locates the signed bytes and the key is
+        unsound; node_id33 the receiver_id (the `n` key or the recovered one) where status is 1; hash32 hash_u5's signing
+        hash where status is not -1.  Field values (prefix, amount, p / s / d / h presence ...) are not checked: see
+        cln_sigverify.h."""
+        enc = [s.encode() if isinstance(s, str) else bytes(s) for s in invoices]
+        lens = np.array([len(s) for s in enc], dtype=np.uint32)
+        offs = np.zeros(len(enc), dtype=np.uint64)
+        if len(enc) > 1:
+            offs[1:] = np.cumsum(lens[:-1], dtype=np.uint64)
+        blob = np.frombuffer(b"".join(enc), dtype=np.uint8)
+        return self.verify_bolt11_spans(blob, offs, lens)
+
+    def verify_bolt11_spans(self, blob, off, length):
+        """verify_bolt11 with the invoices already laid out: invoice i = blob[off[i]:off[i]+length[i]], read up to its
+        first NUL byte."""
+        blob = np.ascontiguousarray(blob, dtype=np.uint8).reshape(-1)
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        length = np.ascontiguousarray(length, dtype=np.uint32)
+        n = off.shape[0]
+        if length.shape[0] != n:
+            raise ValueError("length mismatch")
+        status = np.zeros(max(n, 1), dtype=np.int32)
+        node = np.zeros((max(n, 1), 33), dtype=np.uint8)
+        h = np.zeros((max(n, 1), 32), dtype=np.uint8)
+        self._check(self.lib.sv_verify_bolt11_host(self._ctx, blob.ctypes.data, blob.size, off.ctypes.data,
+                                                   length.ctypes.data, n, status.ctypes.data, node.ctypes.data,
+                                                   h.ctypes.data), "sv_verify_bolt11_host")
+        return status[:n], node[:n], h[:n]
+
+    def last_bolt11_timing(self):
+        """(parse_ms, curve_ms) device time of the last verify_bolt11 call: bech32, field walk and signing hash, then
+        verification and recovery; needs set_profiling(True)."""
+        a, b = ctypes.c_float(), ctypes.c_float()
+        self._check(self.lib.sv_get_last_bolt11_timing(self._ctx, ctypes.byref(a), ctypes.byref(b)), "sv_get_last_bolt11_timing")
         return a.value, b.value
 
     def sha256_double(self, data, off, length):
