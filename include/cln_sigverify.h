@@ -438,10 +438,10 @@ uint64_t sv_gossip_prune_cut(const sv_gossip_prune_summary *summary, const uint8
  *      break, in store order: act_off = t, act_resume = q, act_kind = SV_SALVAGE_RESTORED or SV_SALVAGE_BRIDGED; at most
  *      act_capacity are listed (the arrays may be NULL when it is 0), summary->breaks counts them all.  A major version
  *      other than 0: SV_ERR_ARG, nothing written.  On the device: k_salvage_filter (one thread per byte offset: the
- *      header tests, and an order-preserving compaction of the candidates through a per-block count and k_salvage_scan),
- *      then k_salvage_crc (the slice-by-8 checksum, one thread per candidate, a warp per candidate over 1,024 bytes).  The
- *      host walks the store with the sorted sound offsets (a galloping binary search, header bytes only), and
- *      k_salvage_restore checks each break's restore CRC on the device, one warp per break.
+ *      header tests, and an order-preserving compaction of the candidates through a per-block count and cub's scan of
+ *      the counts), then k_salvage_crc (the slice-by-8 checksum, one thread per candidate, a warp per candidate over
+ *      1,024 bytes).  The host walks the store with the sorted sound offsets (a galloping binary search, header bytes
+ *      only), and k_salvage_restore checks each break's restore CRC on the device, one warp per break.
  *
  *      sv_salvage_gossip_store_fd: the salvage on bytes [0, len) of fd, then fsync, then exactly sv_repair_gossip_store_fd
  *      (*summary and *new_len are its).  Each action is written back (pwrite) as 4 bytes of flags and length per header;
@@ -704,7 +704,7 @@ typedef struct {
     int main_regs;        /* registers per thread (cudaFuncGetAttributes) */
     size_t gtable_bytes;
     size_t scratch_bytes;
-    unsigned long long launches; /* kernels launched by this context so far */
+    unsigned long long launches; /* kernels launched by this context so far, not counting cub's sorts and scans */
     size_t l2_persist_bytes;     /* persisting L2 carve-out behind the table-slab access-policy window (0: hint off) */
     size_t l2_max_persist_bytes; /* what the device would allow */
 } sv_info;
@@ -714,7 +714,10 @@ int sv_get_info(const sv_ctx *ctx, sv_info *info);
  * around the scalar-side and curve-side kernels; read them back after synchronising. */
 int sv_set_profiling(sv_ctx *ctx, int on);
 int sv_get_last_timing(sv_ctx *ctx, float *prep_ms, float *main_ms);
-/* the same for the last sv_verify_bolt12_host call: parse + Merkle + sighash kernels, then the verification kernels */
+/* the same for the last sv_verify_bolt12_host call: parse + Merkle + sighash kernels, then the verification kernels.
+ * It and sv_get_last_bolt11_timing report what the last profiled call of their own entry point measured before it
+ * returned, as the gossip_store getters do: a later call of any other entry point leaves them as they are, and before
+ * the first such call they are 0. */
 int sv_get_last_bolt12_timing(sv_ctx *ctx, float *merkle_ms, float *verify_ms);
 /* the same for the last sv_verify_bolt11_host call: parse + hash kernels, then the verification and recovery kernels */
 int sv_get_last_bolt11_timing(sv_ctx *ctx, float *parse_ms, float *curve_ms);

@@ -112,7 +112,7 @@ extern "C" int sv_batch_launch(const u8* d_msg, const u8* d_key, const u8* d_sig
                                cudaStream_t st, cudaEvent_t ev_mid) {
     const u32 groups = (u32)((n + SV_SB_GROUP - 1) / SV_SB_GROUP);
     k_sb_prep<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(d_msg, d_key, d_sig, n, d_seed, (qtab_entry*)d_pts, d_dig, (sc*)d_t, d_ok);
-    if (ev_mid) cudaEventRecord(ev_mid, st);
+    if (ev_mid && cudaEventRecord(ev_mid, st) != cudaSuccess) return -1;
     u32 jobs = groups * SV_SB_WINDOWS;
     k_sb_window<<<(jobs + SV_SB_WARPS - 1) / SV_SB_WARPS, 32 * SV_SB_WARPS, 0, st>>>((const qtab_entry*)d_pts, d_dig, n, groups, (sv_jac*)d_S);
     k_sb_final<<<(groups + 63) / 64, 64, 0, st>>>((const sv_jac*)d_S, (const sc*)d_t, n, groups, (const ge_mem*)d_gtab, d_gok);

@@ -26,8 +26,10 @@
 // runs the kernels or fails with an error code.
 #include <cuda_runtime.h>
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 #include <stdio.h>
 #include <chrono>
+#include <memory>
 #include <stdlib.h>
 #include <string.h>
 #include <string>
@@ -645,7 +647,7 @@ __global__ void __launch_bounds__(256) k_store_finish(const u8* store, const u64
 
 // ---- gossip_store salvage (gossip_salvage.cuh): every byte offset that holds a sound record -------------------------
 // k_salvage_filter: one thread per byte offset o = 1 + global thread index, 256 per block.  Without out, count[b] = the
-// candidates (gs_salvage_candidate) of block b.  With out, count holds each block's exclusive prefix (k_salvage_scan) and
+// candidates (gs_salvage_candidate) of block b.  With out, count holds each block's exclusive prefix (cub's scan) and
 // every candidate goes to out[count[b] + its rank in the block]: the list is in store order.
 __global__ void __launch_bounds__(256) k_salvage_filter(const u8* store, u64 len, u64* count, u64* out) {
     __shared__ u32 warp_n[8];
@@ -667,40 +669,6 @@ __global__ void __launch_bounds__(256) k_salvage_filter(const u8* store, u64 len
     u64 r = count[blockIdx.x] + __popc(m & ((1u << lane) - 1));
     for (u32 k = 0; k < w; k++) r += warp_n[k];
     out[r] = o;
-}
-// one block: count[0, nb) replaced by its exclusive prefix sums, count[nb] = the total
-__global__ void __launch_bounds__(1024) k_salvage_scan(u64* count, size_t nb) {
-    __shared__ u64 ws[32];
-    __shared__ u64 carry;
-    const u32 lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (size_t base = 0; base < nb; base += 1024) {
-        const size_t i = base + threadIdx.x;
-        const u64 v = i < nb ? count[i] : 0;
-        u64 x = v;
-        for (int d = 1; d < 32; d <<= 1) {
-            const u64 y = __shfl_up_sync(~0u, x, d);
-            if (lane >= (u32)d) x += y;
-        }
-        if (lane == 31) ws[w] = x;
-        __syncthreads();
-        if (w == 0) {
-            u64 y = ws[lane];
-            for (int d = 1; d < 32; d <<= 1) {
-                const u64 z = __shfl_up_sync(~0u, y, d);
-                if (lane >= (u32)d) y += z;
-            }
-            ws[lane] = y;
-        }
-        __syncthreads();
-        const u64 before = carry + (w ? ws[w - 1] : 0) + x - v;
-        if (i < nb) count[i] = before;
-        __syncthreads();
-        if (threadIdx.x == 1023) carry = before + v;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) count[nb] = carry;
 }
 // k_salvage_crc: sound[i] = 1 if candidate i's checksum matches.  One thread per candidate; a candidate whose message is
 // longer than GS_SV_LONG (up to 65,535 bytes, mostly random offsets) is checksummed by its whole warp, one slice per
@@ -847,56 +815,6 @@ __global__ void __launch_bounds__(128) k_b12_count(const u8* blob, const u64* of
     if (i >= n) return;
     long long c = b12_count(blob + off[i], len[i]);
     cnt[i] = c < 0 ? 0u : (u32)c;
-}
-// exclusive prefix sum of the field counts (u64): block-local scan, scan of the block totals, add-back.  sums[nb] = total.
-#define SV_B12_SCAN 1024
-__device__ __forceinline__ u64 b12_block_scan(u64 v, u64* total) {
-    __shared__ u64 warp_sums[SV_B12_SCAN / 32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    u64 x = v;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-        u64 y = __shfl_up_sync(0xFFFFFFFFu, x, d);
-        if (lane >= d) x += y;
-    }
-    if (lane == 31) warp_sums[warp] = x;
-    __syncthreads();
-    if (warp == 0) {
-        u64 s = lane < (int)(blockDim.x >> 5) ? warp_sums[lane] : 0;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            u64 y = __shfl_up_sync(0xFFFFFFFFu, s, d);
-            if (lane >= d) s += y;
-        }
-        warp_sums[lane] = s;
-    }
-    __syncthreads();
-    u64 excl = x - v + (warp ? warp_sums[warp - 1] : 0);
-    *total = warp_sums[(blockDim.x >> 5) - 1];
-    __syncthreads();
-    return excl;
-}
-__global__ void __launch_bounds__(SV_B12_SCAN) k_b12_scan_local(const u32* cnt, size_t n, u64* base, u64* sums) {
-    size_t i = (size_t)blockIdx.x * SV_B12_SCAN + threadIdx.x;
-    u64 total;
-    u64 e = b12_block_scan(i < n ? cnt[i] : 0, &total);
-    if (i < n) base[i] = e;
-    if (threadIdx.x == 0) sums[blockIdx.x] = total;
-}
-__global__ void __launch_bounds__(SV_B12_SCAN) k_b12_scan_sums(u64* sums, size_t nb) {
-    u64 carry = 0;
-    for (size_t c = 0; c < nb; c += SV_B12_SCAN) {
-        size_t i = c + threadIdx.x;
-        u64 total;
-        u64 e = b12_block_scan(i < nb ? sums[i] : 0, &total);
-        if (i < nb) sums[i] = carry + e;
-        carry += total;
-    }
-    if (threadIdx.x == 0) sums[nb] = carry;
-}
-__global__ void __launch_bounds__(SV_B12_SCAN) k_b12_scan_add(u64* base, size_t n, const u64* sums) {
-    size_t i = (size_t)blockIdx.x * SV_B12_SCAN + threadIdx.x;
-    if (i < n) base[i] += sums[blockIdx.x];
 }
 // k_b12_tags: thread t < ntags computes the sighash midstate of tag t (tag bytes tagbytes[tagoff[t] .. +taglen[t])), thread
 // ntags the leaf and branch midstates every tag shares
@@ -1441,6 +1359,22 @@ struct slab_layout {
     }
 };
 
+// The marks of the profiling mode, one timing event each.  Every verification launch records MK_PREP, MK_MAIN and MK_END
+// (sv_get_last_timing reads them).  A synchronous entry point records its stage marks as well and turns its marks into
+// its splits before it returns.  Calls on one context are issued one at a time, so the entry points share stage slots.
+enum sv_mark {
+    MK_PREP, MK_MAIN, MK_END,
+    // BOLT12, BOLT11
+    MK_B12_PARSE = 3, MK_B12_SIGHASH,
+    MK_B11_PARSE = 3, MK_B11_PACKED, MK_B11_CURVE, MK_B11_DONE,
+    // the gossip_store audit and prune, and their funding step
+    MK_STORE_COPY = 3, MK_STORE_COPIED, MK_STORE_CRC, MK_STORE_PASS, MK_PRUNE_ROUND2, MK_PRUNE_FLAGS,
+    MK_FUND_STAGE, MK_FUND_STAGED, MK_FUND_KERNEL, MK_FUND_DONE,
+    // the salvage
+    MK_SALVAGE_COUNT = 3, MK_SALVAGE_SCANNED, MK_SALVAGE_EMIT, MK_SALVAGE_CRC, MK_SALVAGE_DONE,
+    MK_COUNT = MK_FUND_DONE + 1
+};
+
 struct sv_ctx {
     int device = 0;
     int sm_count = 0;
@@ -1494,9 +1428,9 @@ struct sv_ctx {
     // BOLT12 field records and tree nodes, sized by the counting pass
     dev_buf<> b12_buf;
     int profiling = 0;
-    cudaEvent_t ev[3] = {};      // before prep, between prep and main, after main (profiling mode only)
-    cudaEvent_t b12_ev[2] = {};  // around the BOLT12 parse / Merkle / sighash kernels (profiling mode only)
-    cudaEvent_t b11_ev[4] = {};  // around the BOLT11 parse stage, and around its curve stage (profiling mode only)
+    cudaEvent_t mark_ev[MK_COUNT] = {};  // one timing event per mark (sv_set_profiling)
+    float b12_ms[2] = {};        // last sv_verify_bolt12_host: parse / Merkle / sighash kernels, verification kernels
+    float b11_ms[2] = {};        // last sv_verify_bolt11_host: parse stage, curve stage
     float gs_ms[4] = {};         // last sv_verify_gossip_store_host: header walk, H2D, checksums, verification (profiling mode)
     float gp_ms[4] = {};         // last sv_prune_gossip_store_host: header walk, first round, second round, flag write
     float gf_ms[2] = {};         // last funding call: table staging and sort, k_store_funding
@@ -1531,6 +1465,14 @@ static int fail(sv_ctx* ctx, int code, const char* what, cudaError_t e) {
         cudaError_t e__ = (call);                                                  \
         if (e__ != cudaSuccess) return fail(ctx, e__ == cudaErrorMemoryAllocation ? SV_ERR_NOMEM : SV_ERR_CUDA, #call, e__); \
     } while (0)
+
+// profiling mode: mark k recorded on st (nothing otherwise), and the milliseconds from mark a to mark b
+static cudaError_t mark(const sv_ctx* ctx, sv_mark k, cudaStream_t st) {
+    return ctx->profiling ? cudaEventRecord(ctx->mark_ev[k], st) : cudaSuccess;
+}
+static cudaError_t mark_ms(const sv_ctx* ctx, sv_mark a, sv_mark b, float* ms) {
+    return cudaEventElapsedTime(ms, ctx->mark_ev[a], ctx->mark_ev[b]);
+}
 
 // Grow-only: nothing happens while the buffer holds `bytes`.  Otherwise it waits until no launch can still read the old
 // allocation (the whole device, or only the event `wait` when the caller knows the last user), frees it and allocates the
@@ -1680,9 +1622,7 @@ extern "C" void sv_destroy(sv_ctx* ctx) {
     if (ctx->h_small) cudaFreeHost(ctx->h_small);
     for (sv_ctx::slot_t& sl : ctx->slot)
         if (sl.done) cudaEventDestroy(sl.done);
-    for (cudaEvent_t e : ctx->ev) if (e) cudaEventDestroy(e);
-    for (cudaEvent_t e : ctx->b12_ev) if (e) cudaEventDestroy(e);
-    for (cudaEvent_t e : ctx->b11_ev) if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : ctx->mark_ev) if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : ctx->h2d_ev) if (e) cudaEventDestroy(e);
     for (cudaStream_t s : {ctx->copy_stream, ctx->stream2, ctx->stream}) if (s) cudaStreamDestroy(s);
     delete ctx;  // the device buffers free themselves
@@ -1753,12 +1693,12 @@ static int launch_verify_dedup(sv_ctx* ctx, int kind, const u8* d_msg, const u8*
     sv_ctx::slot_t* sl = nullptr;
     rc = acquire_slot(ctx, n, st, &sl);
     if (rc) return rc;
-    if (ctx->profiling) cudaEventRecord(ctx->ev[0], st);
+    CK(mark(ctx, MK_PREP, st));
     launch_ecdsa_prep(ctx, d_msg, d_sig, n, sl->d_work, st);
-    if (ctx->profiling) cudaEventRecord(ctx->ev[1], st);
+    CK(mark(ctx, MK_MAIN, st));
     k_sharedkey_build_many<<<(distinct + 127) / 128, 128, 0, st>>>(kind, d_key, keylen, replist, distinct, sk);
     k_main_shared<<<main_grid_for(ctx, n), SV_MAIN_BLOCK, 0, st>>>(sl->d_work, d_sig, n, ctx->d_gtab, sk, tid, d_verdict, d_aux);
-    if (ctx->profiling) cudaEventRecord(ctx->ev[2], st);
+    CK(mark(ctx, MK_END, st));
     ctx->launches += 2;
     CK(cudaGetLastError());
     rc = release_slot(ctx, sl, st);
@@ -1798,8 +1738,8 @@ static void apply_l2_policy(sv_ctx* ctx, cudaStream_t st, const void* slab) {
 static int launch_small(sv_ctx* ctx, int kind, const u8* d_msg, const u8* d_key, const u8* d_sig, size_t n,
                         u8* d_verdict, u8* d_aux, cudaStream_t st) {
     unsigned grid = (unsigned)((n + SV_SMALL_ITEMS - 1) / SV_SMALL_ITEMS);
-    if (ctx->profiling) cudaEventRecord(ctx->ev[0], st);
-    if (ctx->profiling) cudaEventRecord(ctx->ev[1], st);
+    CK(mark(ctx, MK_PREP, st));
+    CK(mark(ctx, MK_MAIN, st));
     // x-only keys: without the square root unless switched off (verify.cuh).  BIP-340 needs a field inversion at the end
     // either way, so dropping the square root is pure gain.  For compressed-key ECDSA the division
     // D/B would be an inversion the plain flow does not have, as long as the square root it replaces and divergent across
@@ -1808,7 +1748,7 @@ static int launch_small(sv_ctx* ctx, int kind, const u8* d_msg, const u8* d_key,
     else if (kind == SV_KIND_ECDSA_XY) k_small<SV_KIND_ECDSA_XY, false><<<grid, 160, 0, st>>>(d_msg, d_key, d_sig, n, ctx->d_gtab, d_verdict, d_aux);
     else if (ctx->nosqrt) k_small<SV_KIND_SCHNORR, true><<<grid, 160, 0, st>>>(d_msg, d_key, d_sig, n, ctx->d_gtab, d_verdict, d_aux);
     else k_small<SV_KIND_SCHNORR, false><<<grid, 160, 0, st>>>(d_msg, d_key, d_sig, n, ctx->d_gtab, d_verdict, d_aux);
-    if (ctx->profiling) cudaEventRecord(ctx->ev[2], st);
+    CK(mark(ctx, MK_END, st));
     ctx->launches += 1;
     CK(cudaGetLastError());
     return SV_OK;
@@ -1832,14 +1772,14 @@ static int launch_verify(sv_ctx* ctx, int kind, const u8* d_msg, const u8* d_key
     if (rc) return rc;
     apply_l2_policy(ctx, st, sl->d_scratch);
     sv_work* work = sl->d_work;
-    if (ctx->profiling) cudaEventRecord(ctx->ev[0], st);
+    CK(mark(ctx, MK_PREP, st));
     if (kind == SV_KIND_SCHNORR) {
         k_prep_schnorr<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(d_msg, d_key, d_sig, n, work);
         ctx->launches += 1;
     } else {
         launch_ecdsa_prep(ctx, d_msg, d_sig, n, work, st);
     }
-    if (ctx->profiling) cudaEventRecord(ctx->ev[1], st);
+    CK(mark(ctx, MK_MAIN, st));
     const unsigned grid = main_grid_for(ctx, n);
     if (kind == SV_KIND_ECDSA33 && ctx->nosqrt) {
         // compressed keys: the flow that skips the square root (verify.cuh "without the square root")
@@ -1862,7 +1802,7 @@ static int launch_verify(sv_ctx* ctx, int kind, const u8* d_msg, const u8* d_key
         k_final_schnorr<<<(unsigned)((threads + 63) / 64), 64, 0, st>>>(work, d_sig, n, d_verdict);
         ctx->launches += 1;
     }
-    if (ctx->profiling) cudaEventRecord(ctx->ev[2], st);
+    CK(mark(ctx, MK_END, st));
     ctx->launches += 1;
     if (d_bitmap) {
         size_t nb = (n + 255) / 256;
@@ -1910,34 +1850,30 @@ extern "C" int sv_set_profiling(sv_ctx* ctx, int on) {
     if (!ctx) return SV_ERR_ARG;
     dev_guard dg__;
     CK(dg__.enter(ctx->device));
-    if (on && !ctx->ev[0])
-        for (int i = 0; i < 3; i++) CK(cudaEventCreate(&ctx->ev[i]));
-    if (on && !ctx->b12_ev[0])
-        for (int i = 0; i < 2; i++) CK(cudaEventCreate(&ctx->b12_ev[i]));
-    if (on && !ctx->b11_ev[0])
-        for (cudaEvent_t& e : ctx->b11_ev) CK(cudaEventCreate(&e));
+    if (on && !ctx->mark_ev[0])
+        for (cudaEvent_t& e : ctx->mark_ev) CK(cudaEventCreate(&e));
     ctx->profiling = on ? 1 : 0;
     return SV_OK;
 }
 // device time of the last sv_verify_bolt12_host call: parse + Merkle + sighash kernels, then the verification kernels
 extern "C" int sv_get_last_bolt12_timing(sv_ctx* ctx, float* merkle_ms, float* verify_ms) {
     if (!ctx || !ctx->profiling || !merkle_ms || !verify_ms) return SV_ERR_ARG;
-    CK(cudaEventElapsedTime(merkle_ms, ctx->b12_ev[0], ctx->b12_ev[1]));
-    CK(cudaEventElapsedTime(verify_ms, ctx->ev[0], ctx->ev[2]));
+    *merkle_ms = ctx->b12_ms[0];
+    *verify_ms = ctx->b12_ms[1];
     return SV_OK;
 }
 // device time of the last sv_verify_bolt11_host call: parse and hash stage, then the verification and recovery stage
 extern "C" int sv_get_last_bolt11_timing(sv_ctx* ctx, float* parse_ms, float* curve_ms) {
     if (!ctx || !ctx->profiling || !parse_ms || !curve_ms) return SV_ERR_ARG;
-    CK(cudaEventElapsedTime(parse_ms, ctx->b11_ev[0], ctx->b11_ev[1]));
-    CK(cudaEventElapsedTime(curve_ms, ctx->b11_ev[2], ctx->b11_ev[3]));
+    *parse_ms = ctx->b11_ms[0];
+    *curve_ms = ctx->b11_ms[1];
     return SV_OK;
 }
 // device time of the last sv_verify_* launch pair (call after the stream has been synchronised)
 extern "C" int sv_get_last_timing(sv_ctx* ctx, float* prep_ms, float* main_ms) {
     if (!ctx || !ctx->profiling || !prep_ms || !main_ms) return SV_ERR_ARG;
-    CK(cudaEventElapsedTime(prep_ms, ctx->ev[0], ctx->ev[1]));
-    CK(cudaEventElapsedTime(main_ms, ctx->ev[1], ctx->ev[2]));
+    CK(mark_ms(ctx, MK_PREP, MK_MAIN, prep_ms));
+    CK(mark_ms(ctx, MK_MAIN, MK_END, main_ms));
     return SV_OK;
 }
 
@@ -2251,15 +2187,11 @@ static_assert(GS_ST_DELETED == SV_GS_DELETED && GS_ST_STORE_RECORD == SV_GS_STOR
                   GS_ST_ENDED == SV_GS_ENDED && GS_ST_NO_AMOUNT == SV_GS_NO_AMOUNT,
               "gossip_store.cuh and cln_sigverify.h must agree on the record statuses");
 
-struct ev_set {  // CUDA events of one call, destroyed on every exit path
-    cudaEvent_t e[6] = {};
-    ~ev_set() { for (cudaEvent_t x : e) if (x) cudaEventDestroy(x); }
-};
-
 // One pass over a staged store: the messages (item slots laid out from the 2-byte type) and channel events of the live
 // records before `cut` (skip[r] != 0 leaves record r out as well), sliced, resolved, hashed and verified on the device.
 // The slab stays allocated with the pass, so the prune's second round reuses the sorted events, the first holders and
-// the digests (item slots of ctx->d_msg / d_sig; ctx's staging holds extra_items more slots after them).
+// the digests (item slots of ctx->d_msg / d_sig; ctx's staging holds extra_items more slots after them).  MK_STORE_PASS
+// (profiling mode) follows the last status.
 struct store_pass {
     std::vector<u64> moff, eoff;
     std::vector<u32> mlen, base, mrec, emsg, msg_of;
@@ -2274,8 +2206,7 @@ struct store_pass {
     u8 *d_ekind = nullptr, *d_ok = nullptr;
 };
 static int store_pass_run(sv_ctx* ctx, const u8* d_store, size_t len, const uint8_t* chain_hash32,
-                          const std::vector<gs_rec>& rec, size_t cut, const u8* skip, size_t extra_items, store_pass& P,
-                          cudaEvent_t done) {
+                          const std::vector<gs_rec>& rec, size_t cut, const u8* skip, size_t extra_items, store_pass& P) {
     cudaStream_t st = ctx->stream;
     P.msg_of.assign(rec.size(), GS_NONE);
     size_t& items = P.items;
@@ -2300,10 +2231,8 @@ static int store_pass_run(sv_ctx* ctx, const u8* d_store, size_t len, const uint
     P.mstatus.assign(n_msgs, 0);
     P.holder.assign(n_msgs, GS_NONE);
     if (!n_msgs) {
-        if (done) {
-            CK(cudaEventRecord(done, st));
-            CK(cudaStreamSynchronize(st));
-        }
+        CK(mark(ctx, MK_STORE_PASS, st));
+        CK(cudaStreamSynchronize(st));
         return SV_OK;
     }
     int rc = ensure_staging(ctx, items + extra_items);
@@ -2362,7 +2291,7 @@ static int store_pass_run(sv_ctx* ctx, const u8* d_store, size_t len, const uint
                                         d_kinds, nullptr, nullptr);
     k_store_finish<<<(unsigned)((n_msgs + 255) / 256), 256, 0, st>>>(d_store, d_moff, d_holder, n_msgs, d_status);
     ctx->launches += 2;
-    if (done) CK(cudaEventRecord(done, st));
+    CK(mark(ctx, MK_STORE_PASS, st));
     CK(cudaMemcpyAsync(P.mstatus.data(), d_status, 4 * n_msgs, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(P.holder.data(), d_holder, 4 * n_msgs, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -2370,12 +2299,12 @@ static int store_pass_run(sv_ctx* ctx, const u8* d_store, size_t len, const uint
 }
 
 // The funding table staged on the device for one call and sorted there: the outputs by scid (their entries carried as
-// values), the heights ascending.  A duplicate scid is SV_ERR_ARG.  ev (profiling mode): e[0], e[1] around the staging.
+// values), the heights ascending.  A duplicate scid is SV_ERR_ARG.  MK_FUND_STAGE, MK_FUND_STAGED around the staging.
 struct funding_stage {
     dev_buf<> s;
     gf_table t{};
 };
-static int funding_stage_run(sv_ctx* ctx, const sv_funding_table* tb, funding_stage& F, const ev_set& ev) {
+static int funding_stage_run(sv_ctx* ctx, const sv_funding_table* tb, funding_stage& F) {
     cudaStream_t st = ctx->stream;
     const size_t n = tb->n_outputs, nb = tb->n_blocks;
     if (n >= 0x7FFFFFFFu || nb >= 0x7FFFFFFFu) return fail(ctx, SV_ERR_ARG, "funding table too large", cudaSuccess);
@@ -2393,7 +2322,7 @@ static int funding_stage_run(sv_ctx* ctx, const sv_funding_table* tb, funding_st
     if (rc) return rc;
     dev_buf<>& s = F.s;
     u32* d_dup = s.at<u32>(o_dup);
-    if (ev.e[0]) CK(cudaEventRecord(ev.e[0], st));
+    CK(mark(ctx, MK_FUND_STAGE, st));
     CK(cudaMemsetAsync(d_dup, 0, 4, st));
     if (n) {
         CK(cudaMemcpyAsync(s.at<u64>(o_key), tb->scid, 8 * n, cudaMemcpyHostToDevice, st));
@@ -2409,7 +2338,7 @@ static int funding_stage_run(sv_ctx* ctx, const sv_funding_table* tb, funding_st
         CK(cudaMemcpyAsync(s.at<u32>(o_blk), tb->blocks, 4 * nb, cudaMemcpyHostToDevice, st));
         CK(cub::DeviceRadixSort::SortKeys(s + o_cub, cub_keys, s.at<u32>(o_blk), s.at<u32>(o_blk2), (int)nb, 0, 32, st));
     }
-    if (ev.e[1]) CK(cudaEventRecord(ev.e[1], st));
+    CK(mark(ctx, MK_FUND_STAGED, st));
     u32 dup = 0;
     CK(cudaMemcpyAsync(&dup, d_dup, 4, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -2426,13 +2355,6 @@ static void funding_count(sv_gossip_funding_summary& F, u8 v) {
     F.checked++;
     (*per[v])++;
 }
-static int funding_timing(sv_ctx* ctx, const ev_set& fev) {
-    if (fev.e[0]) {
-        CK(cudaEventElapsedTime(&ctx->gf_ms[0], fev.e[0], fev.e[1]));
-        CK(cudaEventElapsedTime(&ctx->gf_ms[1], fev.e[2], fev.e[3]));
-    }
-    return SV_OK;
-}
 
 static_assert(GF_NONE == SV_GF_NONE && GF_FUNDED == SV_GF_FUNDED && GF_UNCHECKED == SV_GF_UNCHECKED &&
                   GF_DYING == SV_GF_DYING && GF_NO_TXOUT == SV_GF_NO_TXOUT && GF_SCRIPT == SV_GF_SCRIPT &&
@@ -2441,14 +2363,13 @@ static_assert(GF_NONE == SV_GF_NONE && GF_FUNDED == SV_GF_FUNDED && GF_UNCHECKED
 
 // What the audit and the prune share: gossmap's header walk (past_truncated: the prune's), the funding table staged
 // (with a table), the store staged in a buffer of its own (a store can be hundreds of MB) and the checksum of every live
-// record and of the ENDED record tested on the device.  ev (profiling mode): e[0] before the store's copy, e[1] after
-// it, e[2] after the checksums; e[3..5] are the caller's.  fev: the funding step's (funding_stage_run, store_funding_run).
+// record and of the ENDED record tested on the device.  Marks: MK_STORE_COPY before the store's copy, MK_STORE_COPIED
+// after it, MK_STORE_CRC after the checksums.
 struct store_front {
     dev_guard dg;  // the first member: the buffers below are freed on the context's device
     std::vector<gs_rec> rec;
     gs_walk_end we;
     float walk_ms = 0;
-    ev_set ev, fev;
     funding_stage F;
     dev_buf<> d_store, d_crc;
     std::vector<u8> bad;  // per record: 1 if its checksum was tested and failed
@@ -2470,13 +2391,8 @@ static int store_front_run(sv_ctx* ctx, const uint8_t* store, size_t len, const 
     G.walk_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
     CK(G.dg.enter(ctx->device));
     cudaStream_t st = ctx->stream;
-    if (ctx->profiling)
-        for (int i = 0; i < 6; i++) {
-            CK(cudaEventCreate(&G.ev.e[i]));
-            if (table && i < 4) CK(cudaEventCreate(&G.fev.e[i]));
-        }
     if (table) {
-        int rc = funding_stage_run(ctx, table, G.F, G.fev);
+        int rc = funding_stage_run(ctx, table, G.F);
         if (rc) return rc;
     }
     const size_t n = crc_off.size(), crc_bytes = n * 9 + 16;
@@ -2485,16 +2401,15 @@ static int store_front_run(sv_ctx* ctx, const uint8_t* store, size_t len, const 
     if (rc) return rc;
     u64* d_off = G.d_crc.at<u64>(0);
     u8* d_bad = G.d_crc.at<u8>(n * 8);
-    const cudaEvent_t* ev = G.ev.e;
-    if (ev[0]) CK(cudaEventRecord(ev[0], st));
+    CK(mark(ctx, MK_STORE_COPY, st));
     CK(cudaMemcpyAsync(G.d_store, store, len, cudaMemcpyHostToDevice, st));
     if (n) CK(cudaMemcpyAsync(d_off, crc_off.data(), n * 8, cudaMemcpyHostToDevice, st));
-    if (ev[1]) CK(cudaEventRecord(ev[1], st));
+    CK(mark(ctx, MK_STORE_COPIED, st));
     if (n) {
         k_store_crc_flags<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(G.d_store, d_off, n, d_bad);
         ctx->launches += 1;
     }
-    if (ev[2]) CK(cudaEventRecord(ev[2], st));
+    CK(mark(ctx, MK_STORE_CRC, st));
     std::vector<u8> bad(n);
     if (n) CK(cudaMemcpyAsync(bad.data(), d_bad, n, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -2505,7 +2420,7 @@ static int store_front_run(sv_ctx* ctx, const uint8_t* store, size_t len, const 
 
 // The funding verdicts of P's announcements whose status is 0 and whose record lies before cut, GF_NONE for every other
 // message: in d_fund on the device (n_msgs bytes at its start, which k_prune_mark reads) and in fund on the host once the
-// stream is synchronised.  fev: e[2], e[3] around the kernel.
+// stream is synchronised.  MK_FUND_KERNEL, MK_FUND_DONE around the kernel.
 static int store_funding_run(sv_ctx* ctx, const store_front& G, size_t len, const store_pass& P, size_t cut,
                              dev_buf<>& d_fund, std::vector<u8>& fund) {
     cudaStream_t st = ctx->stream;
@@ -2519,16 +2434,15 @@ static int store_funding_run(sv_ctx* ctx, const store_front& G, size_t len, cons
     int rc = d_fund.reserve(ctx, L.size, L.size);
     if (rc) return rc;
     u32* d_cand = d_fund.at<u32>(o_cand);
-    const cudaEvent_t* fev = G.fev.e;
     CK(cudaMemsetAsync(d_fund, GF_NONE, n, st));
-    if (fev[2]) CK(cudaEventRecord(fev[2], st));
+    CK(mark(ctx, MK_FUND_KERNEL, st));
     if (!cand.empty()) {
         CK(cudaMemcpyAsync(d_cand, cand.data(), 4 * cand.size(), cudaMemcpyHostToDevice, st));
         k_store_funding<<<(unsigned)((cand.size() + 127) / 128), 128, 0, st>>>(G.d_store, len, P.d_moff, d_cand, cand.size(),
                                                                                G.F.t, d_fund);
         ctx->launches += 1;
     }
-    if (fev[3]) CK(cudaEventRecord(fev[3], st));
+    CK(mark(ctx, MK_FUND_DONE, st));
     fund.resize(n);
     if (n) CK(cudaMemcpyAsync(fund.data(), d_fund, n, cudaMemcpyDeviceToHost, st));
     return SV_OK;
@@ -2563,7 +2477,7 @@ static int store_audit(sv_ctx* ctx, const uint8_t* store, size_t len, const uint
     while (cut < nrec && !G.bad[cut]) cut++;
     int cut_status = cut < nrec ? GS_ST_BAD_CRC : 0;
     store_pass P;
-    rc = store_pass_run(ctx, G.d_store, len, chain_hash32, rec, cut, nullptr, 0, P, G.ev.e[3]);
+    rc = store_pass_run(ctx, G.d_store, len, chain_hash32, rec, cut, nullptr, 0, P);
     if (rc) return rc;
     const std::vector<u32>&msg_of = P.msg_of, &mrec = P.mrec, &holder = P.holder;
     // an announcement without room for its amount record stops the walk unless it is redundant (add_channel returns the
@@ -2617,9 +2531,16 @@ static int store_audit(sv_ctx* ctx, const uint8_t* store, size_t len, const uint
     *sum = S;
     if (table) *fsum = FS;
     ctx->gs_ms[0] = G.walk_ms;
-    if (G.ev.e[0])
-        for (int i = 0; i < 3; i++) CK(cudaEventElapsedTime(&ctx->gs_ms[1 + i], G.ev.e[i], G.ev.e[i + 1]));
-    return funding_timing(ctx, G.fev);
+    if (ctx->profiling) {
+        CK(mark_ms(ctx, MK_STORE_COPY, MK_STORE_COPIED, &ctx->gs_ms[1]));
+        CK(mark_ms(ctx, MK_STORE_COPIED, MK_STORE_CRC, &ctx->gs_ms[2]));
+        CK(mark_ms(ctx, MK_STORE_CRC, MK_STORE_PASS, &ctx->gs_ms[3]));
+        if (table) {
+            CK(mark_ms(ctx, MK_FUND_STAGE, MK_FUND_STAGED, &ctx->gf_ms[0]));
+            CK(mark_ms(ctx, MK_FUND_KERNEL, MK_FUND_DONE, &ctx->gf_ms[1]));
+        }
+    }
+    return SV_OK;
 }
 extern "C" int sv_verify_gossip_store_host(sv_ctx* ctx, const uint8_t* store, size_t len, const uint8_t* chain_hash32,
                                            uint64_t* rec_off, uint16_t* rec_type, int* rec_status, uint64_t* rec_holder,
@@ -2671,14 +2592,13 @@ static int store_prune(sv_ctx* ctx, const uint8_t* store, size_t len, const uint
     const std::vector<u8>& skip = G.bad;  // a live record whose checksum fails is deleted and left out of both rounds
     const size_t nrec = rec.size();
     const gs_walk_end& we = G.we;
-    const cudaEvent_t* ev = G.ev.e;
     u8* d_store = G.d_store;
     cudaStream_t st = ctx->stream;
     size_t n_upd = 0;
     for (const gs_rec& r : rec) n_upd += r.status == GS_LIVE && r.type == 258;
     // first round: the audit's statuses and channel table over the records with good checksums
     store_pass P;
-    rc = store_pass_run(ctx, d_store, len, chain_hash32, rec, nrec, skip.data(), n_upd, P, ev[3]);
+    rc = store_pass_run(ctx, d_store, len, chain_hash32, rec, nrec, skip.data(), n_upd, P);
     if (rc) return rc;
     const size_t n_msgs = P.n_msgs, nev = P.nev, items = P.items;
     // the funding verdicts of the announcements whose first-round status is 0: the refused ones join rule 2.  Without a
@@ -2727,11 +2647,11 @@ static int store_prune(sv_ctx* ctx, const uint8_t* store, size_t len, const uint
             k_prune_settle<<<(n_moved + 255) / 256, 256, 0, st>>>(d_list, ctx->d_verdict + items, d_reason);
             ctx->launches += 1;
         }
-        if (ev[4]) CK(cudaEventRecord(ev[4], st));
+        CK(mark(ctx, MK_PRUNE_ROUND2, st));
         CK(cudaMemcpyAsync(reason.data(), d_reason, n_msgs, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
-    } else if (ev[4]) {
-        CK(cudaEventRecord(ev[4], st));
+    } else {
+        CK(mark(ctx, MK_PRUNE_ROUND2, st));
     }
     // every record's reason, in store order
     std::vector<u8> pr(nrec, SV_GP_KEPT);
@@ -2766,7 +2686,7 @@ static int store_prune(sv_ctx* ctx, const uint8_t* store, size_t len, const uint
         ctx->launches += 1;
         CK(cudaMemcpyAsync(flag_hi.data(), d_hi, nd, cudaMemcpyDeviceToHost, st));
     }
-    if (ev[5]) CK(cudaEventRecord(ev[5], st));
+    CK(mark(ctx, MK_PRUNE_FLAGS, st));
     CK(cudaStreamSynchronize(st));
     if (out != store) memcpy(out, store, len);
     for (size_t i = 0; i < nd; i++) out[doff[i]] = flag_hi[i];
@@ -2799,12 +2719,16 @@ static int store_prune(sv_ctx* ctx, const uint8_t* store, size_t len, const uint
     *sum = S;
     if (table) *fsum = FS;
     ctx->gp_ms[0] = G.walk_ms;
-    if (ev[0]) {
-        CK(cudaEventElapsedTime(&ctx->gp_ms[1], ev[0], ev[3]));
-        CK(cudaEventElapsedTime(&ctx->gp_ms[2], ev[3], ev[4]));
-        CK(cudaEventElapsedTime(&ctx->gp_ms[3], ev[4], ev[5]));
+    if (ctx->profiling) {
+        CK(mark_ms(ctx, MK_STORE_COPY, MK_STORE_PASS, &ctx->gp_ms[1]));
+        CK(mark_ms(ctx, MK_STORE_PASS, MK_PRUNE_ROUND2, &ctx->gp_ms[2]));
+        CK(mark_ms(ctx, MK_PRUNE_ROUND2, MK_PRUNE_FLAGS, &ctx->gp_ms[3]));
+        if (table) {
+            CK(mark_ms(ctx, MK_FUND_STAGE, MK_FUND_STAGED, &ctx->gf_ms[0]));
+            CK(mark_ms(ctx, MK_FUND_KERNEL, MK_FUND_DONE, &ctx->gf_ms[1]));
+        }
     }
-    return funding_timing(ctx, G.fev);
+    return SV_OK;
 }
 extern "C" int sv_prune_gossip_store_host(sv_ctx* ctx, const uint8_t* store, size_t len, const uint8_t* chain_hash32,
                                           uint8_t* out, uint64_t* rec_off, uint16_t* rec_type, int* rec_status,
@@ -2832,30 +2756,34 @@ extern "C" int sv_get_last_gossip_prune_timing(sv_ctx* ctx, float* ms4) {
 }
 
 // ---- salvaging a gossip_store past damaged record headers (see cln_sigverify.h) -----------------------------------
-// The store staged once: the sorted sound offsets (the filter twice around the scan, then the checksums), the host walk's
-// breaks, and the restore check of each.  gv_ms (profiling mode): the two filter passes and the scan (device events
-// around the kernels only: e[0]..e[1] and e[2]..e[3], without the count's copy back and the candidate buffer's
-// allocation between them), the checksums (e[3]..e[4]), the host walk.
+// The store staged once: the sorted sound offsets (the filter twice around the scan of its per-block counts, then the
+// checksums), the host walk's breaks, and the restore check of each.  gv_ms (profiling mode): the two filter passes and
+// the scan (device marks around the kernels only, without the count's copy back and the candidate buffer's allocation
+// between them), the checksums, the host walk.
 static int salvage_run(sv_ctx* ctx, const uint8_t* store, size_t len, std::vector<u64>& sound, std::vector<u64>& brk,
                        std::vector<u8>& restore) {
     for (float& ms : ctx->gv_ms) ms = 0;
     if (len < 1 + GS_HDR + 2) return SV_OK;  // no record fits
     cudaStream_t st = ctx->stream;
     const u64 nb = (len - 1 + 255) / 256;
-    ev_set E;
-    if (ctx->profiling)
-        for (int i = 0; i < 5; i++) CK(cudaEventCreate(&E.e[i]));
+    size_t scan_bytes = 0;
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (u64*)nullptr, nb + 1, st));
+    // [per-block counts u64 nb + 1][scan scratch]
+    slab_layout L;
+    L.take(8 * (nb + 1));
+    const size_t o_scan = L.take(scan_bytes);
     dev_buf<> d_store, d_cnt, d_cand, d_brk;
     int rc = d_store.reserve(ctx, len, len);
-    if (!rc) rc = d_cnt.reserve(ctx, 8 * (nb + 1), 8 * (nb + 1));
+    if (!rc) rc = d_cnt.reserve(ctx, L.size, L.size);
     if (rc) return rc;
     u64* cnt = d_cnt.at<u64>(0);
     CK(cudaMemcpyAsync(d_store, store, len, cudaMemcpyHostToDevice, st));
-    if (E.e[0]) CK(cudaEventRecord(E.e[0], st));
+    CK(cudaMemsetAsync(cnt + nb, 0, 8, st));  // count[0, nb) exclusive, count[nb] the total
+    CK(mark(ctx, MK_SALVAGE_COUNT, st));
     k_salvage_filter<<<(unsigned)nb, 256, 0, st>>>(d_store, len, cnt, nullptr);
-    k_salvage_scan<<<1, 1024, 0, st>>>(cnt, nb);
-    ctx->launches += 2;
-    if (E.e[1]) CK(cudaEventRecord(E.e[1], st));
+    CK(cub::DeviceScan::ExclusiveSum(d_cnt + o_scan, scan_bytes, cnt, nb + 1, st));
+    ctx->launches += 1;
+    CK(mark(ctx, MK_SALVAGE_SCANNED, st));
     u64 n = 0;
     CK(cudaMemcpyAsync(&n, cnt + nb, 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -2864,12 +2792,12 @@ static int salvage_run(sv_ctx* ctx, const uint8_t* store, size_t len, std::vecto
         if (rc) return rc;
         u64* cand = d_cand.at<u64>(0);
         u8* ok = d_cand.at<u8>(8 * n);
-        if (E.e[2]) CK(cudaEventRecord(E.e[2], st));
+        CK(mark(ctx, MK_SALVAGE_EMIT, st));
         k_salvage_filter<<<(unsigned)nb, 256, 0, st>>>(d_store, len, cnt, cand);
-        if (E.e[3]) CK(cudaEventRecord(E.e[3], st));
+        CK(mark(ctx, MK_SALVAGE_CRC, st));
         k_salvage_crc<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_store, cand, n, ok);
         ctx->launches += 2;
-        if (E.e[4]) CK(cudaEventRecord(E.e[4], st));
+        CK(mark(ctx, MK_SALVAGE_DONE, st));
         std::vector<u64> c(n);
         std::vector<u8> good(n);
         CK(cudaMemcpyAsync(c.data(), cand, 8 * n, cudaMemcpyDeviceToHost, st));
@@ -2877,16 +2805,18 @@ static int salvage_run(sv_ctx* ctx, const uint8_t* store, size_t len, std::vecto
         CK(cudaStreamSynchronize(st));
         for (u64 k = 0; k < n; k++)
             if (good[k]) sound.push_back(c[k]);
-    } else if (E.e[0]) {
-        for (int i = 2; i < 5; i++) CK(cudaEventRecord(E.e[i], st));
+    } else if (ctx->profiling) {
+        CK(mark(ctx, MK_SALVAGE_EMIT, st));
+        CK(mark(ctx, MK_SALVAGE_CRC, st));
+        CK(mark(ctx, MK_SALVAGE_DONE, st));
         CK(cudaStreamSynchronize(st));
     }
-    if (E.e[0]) {
+    if (ctx->profiling) {
         float a, b;
-        CK(cudaEventElapsedTime(&a, E.e[0], E.e[1]));
-        CK(cudaEventElapsedTime(&b, E.e[2], E.e[3]));
+        CK(mark_ms(ctx, MK_SALVAGE_COUNT, MK_SALVAGE_SCANNED, &a));
+        CK(mark_ms(ctx, MK_SALVAGE_EMIT, MK_SALVAGE_CRC, &b));
         ctx->gv_ms[0] = a + b;
-        CK(cudaEventElapsedTime(&ctx->gv_ms[1], E.e[3], E.e[4]));
+        CK(mark_ms(ctx, MK_SALVAGE_CRC, MK_SALVAGE_DONE, &ctx->gv_ms[1]));
     }
     const auto t0 = std::chrono::steady_clock::now();
     gs_salvage_breaks(store, len, sound.data(), sound.size(), [&brk](u64 t, u64 q) { brk.push_back(t); brk.push_back(q); });
@@ -3194,36 +3124,39 @@ static int bolt12_pass(sv_ctx* ctx, size_t ntags, const char* const* messagename
         tab.insert(tab.end(), fieldnames[t], fieldnames[t] + b);
     }
     if (tag_of) memcpy(tab.data() + t_of, tag_of, 4 * n);
-    const size_t nb = (n + SV_B12_SCAN - 1) / SV_B12_SCAN;
-    // per-call scratch in the auxiliary slab: [cnt u32 n][base u64 n][block sums u64 nb+1][status int n][tree tags]
-    // [sighash midstates 32 x ntags][tag table]
+    cudaStream_t st = ctx->stream;
+    size_t scan_bytes = 0;
+    CK(cub::DeviceScan::ExclusiveScan(nullptr, scan_bytes, (const u32*)nullptr, (u64*)nullptr, cuda::std::plus<>{}, (u64)0,
+                                      n + 1, st));
+    // per-call scratch in the auxiliary slab: [cnt u32 n+1][base u64 n+1][status int n][tree tags]
+    // [sighash midstates 32 x ntags][tag table][scan scratch].  base: the exclusive prefix sums of the field counts,
+    // accumulated in 64 bits (ExclusiveSum would add u32 counts in u32); with cnt[n] = 0, base[n] is the total.
     slab_layout L;
-    const size_t o_cnt = L.take(4 * n), o_base = L.take(8 * n), o_sums = L.take(8 * (nb + 1)), o_status = L.take(4 * n),
-                 o_tags = L.take(sizeof(b12_tags)), o_mid = L.take(32 * ntags), o_tab = L.take(tab.size());
+    const size_t o_cnt = L.take(4 * (n + 1)), o_base = L.take(8 * (n + 1)), o_status = L.take(4 * n),
+                 o_tags = L.take(sizeof(b12_tags)), o_mid = L.take(32 * ntags), o_tab = L.take(tab.size()),
+                 o_scan = L.take(scan_bytes);
     rc = ensure_gbuf(ctx, L.size + 64);
     if (rc) return rc;
     const dev_buf<>& G = ctx->g_buf;
     u32* d_cnt = G.at<u32>(o_cnt);
-    u64 *d_base = G.at<u64>(o_base), *d_sums = G.at<u64>(o_sums);
+    u64* d_base = G.at<u64>(o_base);
     int* d_status = G.at<int>(o_status);
     b12_tags* d_tags = G.at<b12_tags>(o_tags);
     u32* d_mid = G.at<u32>(o_mid);
     u8* d_tab = G + o_tab;
-    cudaStream_t st = ctx->stream;
     CK(cudaMemcpyAsync(ctx->d_key, xonly32, 32 * n, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->d_sig, sig64, 64 * n, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_tab, tab.data(), tab.size(), cudaMemcpyHostToDevice, st));
-    if (ctx->profiling) cudaEventRecord(ctx->b12_ev[0], st);
+    CK(cudaMemsetAsync(d_cnt + n, 0, 4, st));
+    CK(mark(ctx, MK_B12_PARSE, st));
     k_b12_tags<<<(unsigned)((ntags + 1 + 63) / 64), 64, 0, st>>>(d_tab + t_bytes, reinterpret_cast<const u64*>(d_tab + t_off),
                                                               reinterpret_cast<const u32*>(d_tab + t_len), ntags, d_tags, d_mid);
     k_b12_count<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(ctx->d_data, ctx->d_off, ctx->d_len, n, d_cnt);
-    k_b12_scan_local<<<(unsigned)nb, SV_B12_SCAN, 0, st>>>(d_cnt, n, d_base, d_sums);
-    k_b12_scan_sums<<<1, SV_B12_SCAN, 0, st>>>(d_sums, nb);
-    k_b12_scan_add<<<(unsigned)nb, SV_B12_SCAN, 0, st>>>(d_base, n, d_sums);
-    ctx->launches += 5;
+    ctx->launches += 2;
     CK(cudaGetLastError());
+    CK(cub::DeviceScan::ExclusiveScan(G + o_scan, scan_bytes, d_cnt, d_base, cuda::std::plus<>{}, (u64)0, n + 1, st));
     u64 total = 0;
-    CK(cudaMemcpyAsync(&total, d_sums + nb, sizeof total, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&total, d_base + n, sizeof total, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     const size_t per_field = sizeof(b12_field) + 32;
     if (total > ((size_t)-1) / per_field) return fail(ctx, SV_ERR_NOMEM, "BOLT12 field scratch", cudaSuccess);
@@ -3235,7 +3168,7 @@ static int bolt12_pass(sv_ctx* ctx, size_t ntags, const char* const* messagename
         ctx->d_data, ctx->d_off, ctx->d_len, n, d_cnt, d_base, d_tags, d_mid,
         tag_of ? reinterpret_cast<const u32*>(d_tab + t_of) : nullptr, d_recs, d_nodes, ctx->d_msg);
     ctx->launches += 1;
-    if (ctx->profiling) cudaEventRecord(ctx->b12_ev[1], st);
+    CK(mark(ctx, MK_B12_SIGHASH, st));
     CK(cudaGetLastError());
     // the sighashes are ordinary BIP-340 messages from here on: small-batch kernel or the throughput kernels
     rc = launch_verify(ctx, SV_KIND_SCHNORR, ctx->d_msg, ctx->d_key, ctx->d_sig, n, ctx->d_verdict, nullptr, st);
@@ -3246,6 +3179,10 @@ static int bolt12_pass(sv_ctx* ctx, size_t ntags, const char* const* messagename
     CK(cudaMemcpyAsync(status, d_status, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
     if (sighash32_out) CK(cudaMemcpyAsync(sighash32_out, ctx->d_msg, 32 * n, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
+    if (ctx->profiling) {
+        CK(mark_ms(ctx, MK_B12_PARSE, MK_B12_SIGHASH, &ctx->b12_ms[0]));
+        CK(mark_ms(ctx, MK_PREP, MK_END, &ctx->b12_ms[1]));
+    }
     return SV_OK;
 }
 extern "C" int sv_verify_bolt12_host(sv_ctx* ctx, const char* messagename, const char* fieldname, const uint8_t* blob,
@@ -3274,7 +3211,7 @@ extern "C" int sv_verify_bolt12_tagged_host(sv_ctx* ctx, size_t ntags, const cha
 
 // ---- BOLT11: bolt11_decode's signature step (common/bolt11.c:980-1062) for n invoice strings ---------------------------
 // The host copies bytes only.  k_b11_parse gives every invoice its structure, signature and signing hash; two prefix sums
-// (the BOLT12 scan kernels) pack the invoices with an `n` key and the ones to recover.  One host synchronisation reads the
+// (cub's device scan) pack the invoices with an `n` key and the ones to recover.  One host synchronisation reads the
 // two counts.  `n` invoices then take the ordinary compressed-key ECDSA path (small-batch kernel or throughput kernels,
 // launch_verify).  Recovered invoices take k_b11_rec_prep, the plain-flow ladder k_main<SV_KIND_SCHNORR> (which parks the
 // Jacobian result) and k_b11_rec_final.  k_b11_status folds both into one int and one key per invoice.
@@ -3289,42 +3226,42 @@ extern "C" int sv_verify_bolt11_host(sv_ctx* ctx, const uint8_t* blob, size_t bl
     if (rc) return rc;
     rc = stage_spans(ctx, blob, blob_len, off, len, n);
     if (rc) return rc;
-    const size_t nb = (n + SV_B12_SCAN - 1) / SV_B12_SCAN;
-    // per-call scratch in the auxiliary slab.  Per invoice: flags, prefix sums, recovery id, `n` key, status and key out.
-    // Packed: the `n` invoices' message / key / signature, the recovered invoices' R.x, status and key.
+    cudaStream_t st = ctx->stream;
+    size_t scan_bytes = 0;
+    CK(cub::DeviceScan::ExclusiveScan(nullptr, scan_bytes, (const u32*)nullptr, (u64*)nullptr, cuda::std::plus<>{}, (u64)0,
+                                      n + 1, st));
+    // per-call scratch in the auxiliary slab.  Per invoice: flags (one more, 0), their exclusive prefix sums in 64 bits
+    // (one more, the total), recovery id, `n` key, status and key out.  Packed: the `n` invoices' message / key /
+    // signature, the recovered invoices' R.x, status and key.  The scan's scratch.
     slab_layout L;
-    const size_t o_isn = L.take(4 * n), o_bn = L.take(8 * n), o_sn = L.take(8 * (nb + 1)), o_isr = L.take(4 * n),
-                 o_br = L.take(8 * n), o_sr = L.take(8 * (nb + 1)), o_recid = L.take(n), o_key = L.take(33 * n),
-                 o_status = L.take(4 * n), o_node = L.take(33 * n), o_cmsg = L.take(32 * n), o_ckey = L.take(33 * n),
-                 o_csig = L.take(64 * n), o_x = L.take(32 * n), o_rstat = L.take(4 * n), o_rkey = L.take(33 * n);
+    const size_t o_isn = L.take(4 * (n + 1)), o_bn = L.take(8 * (n + 1)), o_isr = L.take(4 * (n + 1)),
+                 o_br = L.take(8 * (n + 1)), o_recid = L.take(n), o_key = L.take(33 * n), o_status = L.take(4 * n),
+                 o_node = L.take(33 * n), o_cmsg = L.take(32 * n), o_ckey = L.take(33 * n), o_csig = L.take(64 * n),
+                 o_x = L.take(32 * n), o_rstat = L.take(4 * n), o_rkey = L.take(33 * n), o_scan = L.take(scan_bytes);
     rc = ensure_gbuf(ctx, L.size);
     if (rc) return rc;
     const dev_buf<>& G = ctx->g_buf;
     u32 *is_n = G.at<u32>(o_isn), *is_r = G.at<u32>(o_isr);
-    u64 *base_n = G.at<u64>(o_bn), *sums_n = G.at<u64>(o_sn), *base_r = G.at<u64>(o_br), *sums_r = G.at<u64>(o_sr);
+    u64 *base_n = G.at<u64>(o_bn), *base_r = G.at<u64>(o_br);
     int *d_status = G.at<int>(o_status), *rstat = G.at<int>(o_rstat);
     u8 *recid = G + o_recid, *key33 = G + o_key, *node = G + o_node, *cmsg = G + o_cmsg, *ckey = G + o_ckey,
        *csig = G + o_csig, *x32 = G + o_x, *rkey = G + o_rkey;
-    cudaStream_t st = ctx->stream;
     const unsigned g128 = (unsigned)((n + 127) / 128);
-    if (ctx->profiling) cudaEventRecord(ctx->b11_ev[0], st);
+    CK(cudaMemsetAsync(is_n + n, 0, 4, st));
+    CK(cudaMemsetAsync(is_r + n, 0, 4, st));
+    CK(mark(ctx, MK_B11_PARSE, st));
     k_b11_parse<<<g128, 128, 0, st>>>(ctx->d_data, ctx->d_off, ctx->d_len, n, ctx->d_msg, key33, ctx->d_sig, recid, is_n, is_r);
-    for (int pass = 0; pass < 2; pass++) {
-        const u32* flag = pass ? is_r : is_n;
-        u64 *base = pass ? base_r : base_n, *sums = pass ? sums_r : sums_n;
-        k_b12_scan_local<<<(unsigned)nb, SV_B12_SCAN, 0, st>>>(flag, n, base, sums);
-        k_b12_scan_sums<<<1, SV_B12_SCAN, 0, st>>>(sums, nb);
-        k_b12_scan_add<<<(unsigned)nb, SV_B12_SCAN, 0, st>>>(base, n, sums);
-    }
+    CK(cub::DeviceScan::ExclusiveScan(G + o_scan, scan_bytes, is_n, base_n, cuda::std::plus<>{}, (u64)0, n + 1, st));
+    CK(cub::DeviceScan::ExclusiveScan(G + o_scan, scan_bytes, is_r, base_r, cuda::std::plus<>{}, (u64)0, n + 1, st));
     k_b11_gather_n<<<g128, 128, 0, st>>>(is_n, base_n, n, ctx->d_msg, key33, ctx->d_sig, cmsg, ckey, csig);
-    ctx->launches += 8;
-    if (ctx->profiling) cudaEventRecord(ctx->b11_ev[1], st);
+    ctx->launches += 2;
+    CK(mark(ctx, MK_B11_PACKED, st));
     CK(cudaGetLastError());
     u64 cnt[2] = {0, 0};
-    CK(cudaMemcpyAsync(&cnt[0], sums_n + nb, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&cnt[1], sums_r + nb, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&cnt[0], base_n + n, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&cnt[1], base_r + n, 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    if (ctx->profiling) cudaEventRecord(ctx->b11_ev[2], st);
+    CK(mark(ctx, MK_B11_CURVE, st));
     rc = launch_verify(ctx, SV_KIND_ECDSA33, cmsg, ckey, csig, (size_t)cnt[0], ctx->d_verdict, nullptr, st);
     if (rc) return rc;
     const size_t cr = (size_t)cnt[1];
@@ -3348,12 +3285,16 @@ extern "C" int sv_verify_bolt11_host(sv_ctx* ctx, const uint8_t* blob, size_t bl
     k_b11_status<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(is_n, base_n, is_r, base_r, n, recid, key33, ctx->d_verdict,
                                                              rstat, rkey, d_status, node);
     ctx->launches += 1;
-    if (ctx->profiling) cudaEventRecord(ctx->b11_ev[3], st);
+    CK(mark(ctx, MK_B11_DONE, st));
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(status, d_status, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(node_id33_out, node, 33 * n, cudaMemcpyDeviceToHost, st));
     if (hash32_out) CK(cudaMemcpyAsync(hash32_out, ctx->d_msg, 32 * n, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
+    if (ctx->profiling) {
+        CK(mark_ms(ctx, MK_B11_PARSE, MK_B11_PACKED, &ctx->b11_ms[0]));
+        CK(mark_ms(ctx, MK_B11_CURVE, MK_B11_DONE, &ctx->b11_ms[1]));
+    }
     return SV_OK;
 }
 
@@ -3395,11 +3336,11 @@ extern "C" int sv_verify_schnorr_batch_host(sv_ctx* ctx, const uint8_t* msg32, c
     CK(cudaMemcpyAsync(ctx->d_msg, msg32, 32 * n, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->d_key, xonly32, 32 * n, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->d_sig, sig64, 64 * n, cudaMemcpyHostToDevice, st));
-    if (ctx->profiling) cudaEventRecord(ctx->ev[0], st);
+    CK(mark(ctx, MK_PREP, st));
     if (sv_batch_launch(ctx->d_msg, ctx->d_key, ctx->d_sig, n, d_seed, d_pts, d_dig, d_t, d_ok, d_S, d_gok, d_out, ctx->d_gtab, st,
-                        ctx->profiling ? ctx->ev[1] : nullptr) != 0)
+                        ctx->profiling ? ctx->mark_ev[MK_MAIN] : nullptr) != 0)
         return fail(ctx, SV_ERR_CUDA, "batch kernels", cudaGetLastError());
-    if (ctx->profiling) cudaEventRecord(ctx->ev[2], st);
+    CK(mark(ctx, MK_END, st));
     ctx->launches += 4;
     std::vector<u8> gok(groups), ok(n);
     CK(cudaMemcpyAsync(gok.data(), d_gok, groups, cudaMemcpyDeviceToHost, st));
@@ -3548,10 +3489,13 @@ extern "C" int sv_probe(sv_ctx* ctx, int mode, double* ops_per_sec) {
     const int iters = (mode == 2 || mode == 3 || mode >= 9) ? 2000 : 4000;
     // modes 9/10: ONE warp on the whole device — the dependent-chain latency of fe_mul / fe_sqr (small-batch path)
     const int blocks = mode >= 9 ? 1 : ctx->sm_count * 8, threads = mode >= 9 ? 32 : 256;
-    ev_set ev;
-    cudaEvent_t &e0 = ev.e[0], &e1 = ev.e[1];
+    // the probe's own events, destroyed on every exit path
+    using event_ptr = std::unique_ptr<CUevent_st, cudaError_t (*)(cudaEvent_t)>;
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
     CK(cudaEventCreate(&e0));
+    event_ptr own0(e0, cudaEventDestroy);
     CK(cudaEventCreate(&e1));
+    event_ptr own1(e1, cudaEventDestroy);
     float best = 1e30f;
     for (int rep = 0; rep < 4; rep++) {
         CK(cudaEventRecord(e0, ctx->stream));

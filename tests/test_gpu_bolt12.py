@@ -5,6 +5,7 @@ keeps it honest); here the whole path runs on the GPU: parse, Merkle root and si
 small-batch kernel or the throughput kernels, with and without the square-root-free flow.
 """
 import ctypes
+import time
 
 import numpy as np
 import pytest
@@ -119,6 +120,25 @@ def test_large_tiled_batch(engine, fx):
     assert len(idx) >= 200_000
     np.testing.assert_array_equal(status, want)
     np.testing.assert_array_equal(sh, fx["sighash"][idx])
+
+
+def test_timing_belongs_to_its_call(engine, fx):
+    """the splits of a BOLT12 call fit inside it, and a later verification of ~100,000 signatures leaves them as they
+    were"""
+    idx = np.nonzero(fx["names"] == 0)[0]
+    big = np.tile(idx, -(-100_000 // len(idx)))
+    engine.set_profiling(True)
+    try:
+        _run(engine, fx, idx, 0)  # warm-up
+        t = time.perf_counter()
+        _run(engine, fx, idx, 0)
+        wall = (time.perf_counter() - t) * 1e3
+        first = engine.last_bolt12_timing()
+        engine.verify(2, fx["sighash"][big], fx["xonly"][big], fx["sig"][big])
+        assert engine.last_bolt12_timing() == first
+        assert min(first) > 0 and sum(first) <= wall, (first, wall)
+    finally:
+        engine.set_profiling(False)
 
 
 def test_arguments(engine):

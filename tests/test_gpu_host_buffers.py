@@ -3,10 +3,10 @@
 A fresh context runs the entry points at sizes that rise, fall, then rise past the earlier maximum, interleaving entry
 points whose scratch layouts differ, so that every buffer is reallocated after other entry points laid their pieces out
 in it: the item staging and the launch slots' work records (sv_verify_host, samekey), the span arrays and data blob
-(raw spans, SHA256d, gossip, gossip_store, transactions), the per-call scratch slab (gossip, transactions, mixed, BOLT12,
-fee grind), the BOLT12 field records, the key de-duplication scratch (gossip, then BIP-340 batch) and the distinct keys'
-tables.  Every output must equal the same call on a second context that first ran every entry point at its largest
-size, so that none of its buffers grows during the sequence."""
+(raw spans, SHA256d, gossip, gossip_store, transactions, BOLT11), the per-call scratch slab (gossip, transactions, mixed,
+BOLT12, BOLT11, fee grind), the BOLT12 field records, the key de-duplication scratch (gossip, then BIP-340 batch) and the
+distinct keys' tables.  Every output must equal the same call on a second context that first ran every entry point at
+its largest size, so that none of its buffers grows during the sequence."""
 import json
 import os
 
@@ -14,7 +14,7 @@ import numpy as np
 import pytest
 
 from lightning_b200 import SvTx
-from tests import bolt12, feegrind, gossip, txsig
+from tests import bolt11, bolt12, feegrind, gossip, txsig
 from tests import gossip_store as gs
 
 pytestmark = pytest.mark.gpu
@@ -47,6 +47,7 @@ def _inputs(engine):
     store = open(os.path.join(ROOT, "tests", "golden", "gossip_store_subset.bin"), "rb").read()
     recs = gs.walk(store)[0]
     fx = bolt12.load_fixture()
+    fx11 = bolt11.load_fixture()
     vec = json.load(open(os.path.join(ROOT, "tests", "golden", "bolt3_htlc_txs.json")))[0]
     weight = feegrind.HTLC_SUCCESS_WEIGHT if "success" in vec["name"] else feegrind.HTLC_TIMEOUT_WEIGHT
     gtx, gblob = feegrind.htlc_tx(vec, 1, 5_000_000)
@@ -102,6 +103,10 @@ def _inputs(engine):
         return lambda e: (e.verify_bolt12_spans(*bolt12.NAMES[0], *a, want_sighash=True),
                           e.verify_bolt12_tagged(bolt12.NAMES, fx["names"][idx], *a, want_sighash=True))
 
+    def b11(s):
+        idx = np.arange(4000 * s) % len(fx11["off"])
+        return lambda e: e.verify_bolt11_spans(fx11["blob"], fx11["off"][idx], fx11["len"][idx])
+
     def grind(s):
         return lambda e: e.grind_tx_fee(0, gtx, gblob, gkey, bytes(gsig[0]), weight, 253, 20000 * s)
 
@@ -111,7 +116,8 @@ def _inputs(engine):
 
     # neighbours differ in how they carve the scratch slab; the BIP-340 batch follows the gossip de-duplication
     return [("verify", verify), ("burst", burst), ("tx", tx), ("bolt12", b12), ("grind", grind), ("store", store_prefix),
-            ("mixed", mixed), ("spans", spans), ("plain", plain), ("grind", grind), ("batch", batch), ("samekey", samekey)]
+            ("mixed", mixed), ("bolt11", b11), ("spans", spans), ("plain", plain), ("grind", grind), ("batch", batch),
+            ("samekey", samekey)]
 
 
 def _canon(x):
