@@ -15,6 +15,8 @@
  *
  *   bolt12_check_signature     common/bolt12.h           (common/bolt12.c:80-92) — same signature; the TLV Merkle root
  *                              and sighash are computed on the device
+ *   bolt11_check_signature     bolt11_decode's signature step (common/bolt11.c:1041-1059) for one invoice string;
+ *                              bech32, the signing hash and the key recovery run on the device
  *   check_tx_sig               bitcoin/signature.h:120   (bitcoin/signature.c:194-221) — same signature; the BIP143
  *                              sighash (bitcoin_tx_hash_for_sig :120-151 -> libwally tx_io.c:660-765) is computed
  *                              on the device from the wally_tx fields
@@ -126,6 +128,7 @@ void cln_sigverify_shutdown(void);
  * they never create a context:
  *   check_signed_hash, check_signed_hash_nodeid, check_schnorr_sig, check_tx_sigs_batch   (sigverifyd_verify)
  *   bolt12_check_signature                                                              (sigverifyd_bolt12)
+ *   bolt11_check_signature                                                              (sigverifyd_bolt11)
  *   check_tx_sig, check_tx_sigs_bip143_batch                                            (sigverifyd_tx)
  *   check_tx_sig_grind_fee                                                              (sigverifyd_fee_grind)
  *   sigcheck_channel_announcement_batch / _node_announcement_batch / _channel_update_batch (sigverifyd_gossip)
@@ -156,9 +159,10 @@ int cln_sigverify_connect_fd(int fd);
  *   0    the answer is already in *ok / status and no callback follows: always in in-process mode (the _start calls the
  *        blocking function), and for the local gates, which send nothing: check_tx_sig's sighash-type gate,
  *        bolt12_check_signature's empty or not strictly ascending field array (false, as the device answers the blocking
- *        call), sigcheck_gossip_batch with n == 0.
- *   > 0  a ticket.  The answer is written to *ok / status[0..n), then done(arg) runs (done may be NULL).  The caller keeps
- *        that output memory alive until the callback; every input is copied before the _start returns.
+ *        call), sigcheck_gossip_batch with n == 0.  bolt11_check_signature has no local gate: every call is sent.
+ *   > 0  a ticket.  The answer is written to *ok / status[0..n) (bolt11_check_signature_start: *status and
+ *        *receiver_id), then done(arg) runs (done may be NULL).  The caller keeps that output memory alive until the
+ *        callback; every input is copied before the _start returns.
  *
  * Verdicts, statuses and aborts are exactly the blocking function's: the request is built by the same code and the reply
  * passes the same checks.
@@ -188,6 +192,8 @@ uint64_t check_tx_sig_start(const struct bitcoin_tx *tx, size_t input_num, const
                             void *arg);
 uint64_t bolt12_check_signature_start(const struct tlv_field *fields, const char *messagename, const char *fieldname,
                                       const struct pubkey *key, const struct bip340sig *sig, bool *ok,
+                                      cln_sigverify_done done, void *arg);
+uint64_t bolt11_check_signature_start(const char *invstring, int *status, struct node_id *receiver_id,
                                       cln_sigverify_done done, void *arg);
 uint64_t sigcheck_gossip_batch_start(const u8 *chain_hash32, const u8 *const *msgs, const size_t *lens, size_t n,
                                      const u8 *signer_kind, const struct node_id *signers, int *status,
@@ -236,6 +242,13 @@ bool check_tx_sig_grind_fee(const struct bitcoin_tx *tx, const u8 *witness_scrip
  * asserts on that), is not a stream CLN's parser produces: the function returns false for it. */
 bool bolt12_check_signature(const struct tlv_field *fields, const char *messagename, const char *fieldname,
                             const struct pubkey *key, const struct bip340sig *sig);
+
+/* common/bolt11.c:1041-1059, bolt11_decode's signature step, for one invoice string as bolt11_decode receives it (read
+ * up to its NUL).  Returns sv_verify_bolt11_host's status: 1 accepted (*receiver_id = the `n` key or the recovered key),
+ * 0 refused, -1 the structure does not locate a signature; *receiver_id is zeroed unless 1.  Field values (amount,
+ * chain, p / s / d / h, features) stay with the caller's bolt11_decode_nosig.  In client mode the string travels as one
+ * sigverifyd_bolt11 request; a reply whose status is not 0, 1 or 255 aborts. */
+int bolt11_check_signature(const char *invstring, struct node_id *receiver_id);
 
 /* channeld HTLC loop: ok[i] = check_signed_hash(&hashes[i], &sigs[i].s, key) for one shared key. */
 void check_tx_sigs_batch(const struct sha256_double *hashes, const struct bitcoin_signature *sigs,

@@ -21,6 +21,8 @@
 #pragma weak sv_prune_gossip_store_fd
 #pragma weak sv_repair_gossip_store_fd
 #pragma weak sv_salvage_gossip_store_fd
+/* likewise for the BOLT11 check: bolt11_check_signature then works through the daemon only */
+#pragma weak sv_verify_bolt11_host
 
 #include <errno.h>
 #include <fcntl.h>
@@ -62,6 +64,7 @@ struct req {
     uint32_t n;
     bool *ok;
     int *status;
+    struct node_id *node;     /* a BOLT11 ticket's receiver id */
     cln_sigverify_done done;
     void *arg;
     u8 *reply;                /* a blocking call's reply message (malloc'ed) */
@@ -266,10 +269,10 @@ static u8 *roundtrip(u8 *frame, size_t len, uint64_t req_id, size_t *reply_len) 
     return r;
 }
 
-/* queues frame[4..4+len), a request whose reply ticket_reply() decodes into ok or status (n items), and returns its
- * ticket.  Above MAX_TICKETS tickets awaiting replies or MAX_UNSENT unsent bytes it first waits for the oldest. */
+/* queues frame[4..4+len), a request whose reply ticket_reply() decodes into ok or status (n items) and node, and returns
+ * its ticket.  Above MAX_TICKETS tickets awaiting replies or MAX_UNSENT unsent bytes it first waits for the oldest. */
 static uint64_t submit(u8 *frame, size_t len, uint64_t id, uint16_t type, uint32_t n, bool *ok, int *status,
-                       const struct later *lt) {
+                       struct node_id *node, const struct later *lt) {
     while (g_t - g_r >= MAX_TICKETS || g_unsent >= MAX_UNSENT) io_wait();
     wire_put(frame, len, 4);
     size_t at = push_req(id, frame, 4 + len, true); /* may move g_q */
@@ -278,6 +281,7 @@ static uint64_t submit(u8 *frame, size_t len, uint64_t id, uint16_t type, uint32
     q->n = n;
     q->ok = ok;
     q->status = status;
+    q->node = node;
     q->done = lt->done;
     q->arg = lt->arg;
     send_some();
@@ -389,7 +393,7 @@ static uint64_t verify_one(int kind, const u8 *msg32, const u8 *key, const u8 *s
             size_t len;
             uint64_t id;
             u8 *f = verify_request(kind, msg32, key, sig64, 1, &len, &id);
-            return submit(f, len, id, WIRE_SIGVERIFYD_VERIFY, 1, ok, NULL, lt);
+            return submit(f, len, id, WIRE_SIGVERIFYD_VERIFY, 1, ok, NULL, NULL, lt);
         }
         remote_verify(kind, msg32, key, sig64, 1, &v);
     } else {
@@ -736,7 +740,7 @@ static uint64_t tx_sig(const struct bitcoin_tx *tx, size_t input_num, const u8 *
         if (lt) {
             size_t len;
             u8 *f = tx_request(SV_KIND_ECDSA_XY, xy, &t, blob, s64, 1, tx_span_bytes(&t, n), &len, &ticket);
-            ticket = submit(f, len, ticket, WIRE_SIGVERIFYD_TX, 1, ok, NULL, lt);
+            ticket = submit(f, len, ticket, WIRE_SIGVERIFYD_TX, 1, ok, NULL, NULL, lt);
         } else {
             remote_tx(SV_KIND_ECDSA_XY, xy, &t, blob, n, s64, 1, &v);
             *ok = v == 1;
@@ -895,7 +899,7 @@ static uint64_t bolt12_sig(const struct tlv_field *fields, const char *messagena
         if (lt) {
             size_t mlen;
             u8 *f = bolt12_request(messagename, fieldname, blob, n, xy, sig->u8, &mlen, &ticket);
-            ticket = submit(f, mlen, ticket, WIRE_SIGVERIFYD_BOLT12, 1, ok, NULL, lt);
+            ticket = submit(f, mlen, ticket, WIRE_SIGVERIFYD_BOLT12, 1, ok, NULL, NULL, lt);
         } else {
             *ok = remote_bolt12(messagename, fieldname, blob, n, xy, sig->u8) == 1;
         }
@@ -919,6 +923,64 @@ uint64_t bolt12_check_signature_start(const struct tlv_field *fields, const char
                                       cln_sigverify_done done, void *arg) {
     const struct later lt = {done, arg};
     return bolt12_sig(fields, messagename, fieldname, key, sig, ok, &lt);
+}
+
+/* ---- bolt11_check_signature (common/bolt11.c:1041-1059): the invoice string goes to the device as it is; bech32, the
+ * field walk, hash_u5's signing hash and the verification against `n` or the recovery of the payee's key run there ---- */
+
+/* the sigverifyd_bolt11 request for one invoice string (its frame: 4 bytes for the length, then the message) */
+static u8 *bolt11_request(const char *invstring, size_t len, size_t *mlen, uint64_t *id) {
+    if (len > MAX_FRAME - (2 + 8 + 4 + 4 + 4)) die_daemon("invoice too large for one request");
+    *mlen = 2 + 8 + 4 + 4 + 4 + len;
+    u8 *f = (u8 *)malloc(4 + *mlen);
+    if (!f) die("malloc", -3);
+    u8 len_be[4];
+    wire_put(len_be, len, 4);
+    *id = ++g_req_id;
+    towire_sigverifyd_bolt11(f + 4, *mlen, *id, 1, len_be, (uint32_t)len, (const u8 *)invstring);
+    return f;
+}
+/* the invoice's status (1, 0 or -1); *receiver_id the reply's node where the status is 1, else zeros */
+static int bolt11_reply(const u8 *r, size_t rl, struct node_id *receiver_id) {
+    struct sigverifyd_bolt11_reply b;
+    if (!fromwire_sigverifyd_bolt11_reply(r, rl, &b) || b.n != 1 || (b.status[0] > 1 && b.status[0] != 255))
+        die_daemon("malformed bolt11 reply");
+    const int st = status_from_wire(b.status[0]);
+    if (st == 1) memcpy(receiver_id->k, b.node_ids, 33);
+    else memset(receiver_id->k, 0, 33);
+    return st;
+}
+
+static uint64_t bolt11_sig(const char *invstring, int *status, struct node_id *receiver_id, const struct later *lt) {
+    const size_t len = strlen(invstring); /* bolt11_decode reads the string up to its NUL */
+    if (client()) {
+        size_t mlen, rl;
+        uint64_t id;
+        u8 *f = bolt11_request(invstring, len, &mlen, &id);
+        if (lt) return submit(f, mlen, id, WIRE_SIGVERIFYD_BOLT11, 1, NULL, status, receiver_id, lt);
+        u8 *r = roundtrip(f, mlen, id, &rl);
+        *status = bolt11_reply(r, rl, receiver_id);
+        free(r);
+        free(f);
+        return 0;
+    }
+    if (!sv_verify_bolt11_host) die("bolt11_check_signature: this engine has no sv_verify_bolt11_host", SV_ERR_ARG);
+    if (len > 0xffffffffu) die("bolt11_check_signature: invoice longer than 4 GiB", -4);
+    uint64_t off = 0;
+    uint32_t l = (uint32_t)len;
+    int rc = sv_verify_bolt11_host(ctx(), (const u8 *)invstring, len, &off, &l, 1, status, receiver_id->k, NULL);
+    if (rc != SV_OK) die("sv_verify_bolt11_host", rc);
+    return 0;
+}
+int bolt11_check_signature(const char *invstring, struct node_id *receiver_id) {
+    int status;
+    bolt11_sig(invstring, &status, receiver_id, NULL);
+    return status;
+}
+uint64_t bolt11_check_signature_start(const char *invstring, int *status, struct node_id *receiver_id,
+                                      cln_sigverify_done done, void *arg) {
+    const struct later lt = {done, arg};
+    return bolt11_sig(invstring, status, receiver_id, &lt);
 }
 
 void check_tx_sigs_batch(const struct sha256_double *hashes, const struct bitcoin_signature *sigs,
@@ -1095,7 +1157,7 @@ static uint64_t gossip_burst(const u8 *chain_hash32, const u8 *const *msgs, cons
         if (lt) {
             size_t mlen;
             u8 *f = burst_request(chain_hash32, blob, total, lens, n, signer_kind, signers ? signers[0].k : NULL, &mlen, &ticket);
-            ticket = submit(f, mlen, ticket, WIRE_SIGVERIFYD_GOSSIP_BURST, (uint32_t)n, NULL, status, lt);
+            ticket = submit(f, mlen, ticket, WIRE_SIGVERIFYD_GOSSIP_BURST, (uint32_t)n, NULL, status, NULL, lt);
         } else {
             remote_gossip_burst(chain_hash32, blob, total, lens, n, signer_kind, signers ? signers[0].k : NULL, status);
         }
@@ -1125,6 +1187,7 @@ static void ticket_reply(const struct req *q, const u8 *r, size_t rl) {
     case WIRE_SIGVERIFYD_VERIFY: verify_reply(r, rl, 1, &v); *q->ok = v == 1; break;
     case WIRE_SIGVERIFYD_TX: tx_reply(r, rl, 1, &v); *q->ok = v == 1; break;
     case WIRE_SIGVERIFYD_BOLT12: *q->ok = bolt12_reply(r, rl) == 1; break;
+    case WIRE_SIGVERIFYD_BOLT11: *q->status = bolt11_reply(r, rl, q->node); break;
     case WIRE_SIGVERIFYD_GOSSIP_BURST: burst_reply(r, rl, q->n, q->status); break;
     }
 }
