@@ -2,6 +2,7 @@
 checksums (:815-937), and the channel table that decides which announcement signs each channel_update (add_channel
 :440-500, remove_channel_by_deletemsg :612-626).  sv_verify_gossip_store_host must agree with it record for record, and
 tests/test_gossmap.py checks both against gossmap.c itself."""
+import os
 import struct
 
 HDR = 12
@@ -12,6 +13,11 @@ EOF, ST_DELETED, STORE_RECORD, UNKNOWN, NOT_REACHED = 0, 16, 17, 18, 19
 INCOMPLETE, PARTIAL, TRUNCATED, BAD_CRC, ST_ENDED, NO_AMOUNT = 32, 33, 34, 35, 36, 37
 STORE_TYPES = (CHANNEL_AMOUNT, DELETE_CHAN, CHAN_DYING, UUID)  # the store's own records: status STORE_RECORD
 NONE = None
+
+
+def load_fixture():
+    """the committed store fixture (tests/golden/gossip_store_subset.bin)"""
+    return open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "gossip_store_subset.bin"), "rb").read()
 
 
 def _table():

@@ -9,7 +9,7 @@ import struct
 
 import numpy as np
 
-from tests.gossip_store import COMPLETED, DELETED, ENDED, HDR, crc32c
+from tests.gossip_store import COMPLETED, DELETED, ENDED, HDR, ST_DELETED, UUID, crc32c, record, walk
 
 KNOWN = (256, 257, 258, 4101, 4103, 4105, 4106, 4107)
 GAP, PIECE = 14, HDR + 65535
@@ -115,3 +115,53 @@ def salvage(store, sound=None):
             acts.append((t, q, BRIDGED))
         t = q
     return bytes(s), acts, sm
+
+
+# ---- damaged stores -------------------------------------------------------------------------------------------------
+def with_uuid(store):
+    """store with a gossip_store_uuid record first, as gossipd starts a store, and one channel_update deleted the way
+    gossipd deletes (its checksum kept)"""
+    uuid = record(struct.pack(">H", UUID) + bytes(range(32)))
+    out = bytearray(store[:1] + uuid + store[1:])
+    recs = walk(bytes(out))[0]
+    upd = [r for r in recs if r[1] == 258][len(recs) // 5]
+    out[upd[0]] |= DELETED >> 8
+    return bytes(out)
+
+
+def damage_classes(store):
+    """name -> (damaged store, (first, end) of the damaged bytes) of a with_uuid() store"""
+    recs = walk(store)[0]
+    n = len(recs)
+    off = [r[0] for r in recs]
+
+    def flip(d, o, mask):
+        d[o] ^= mask
+        return o, o + 1
+
+    out = {}
+    for name, at, mask in (("len_hi", 2, 0x01), ("len_lo", 3, 0x10), ("completed", 0, 0x20)):
+        d = bytearray(store)
+        out[name] = (d, flip(d, off[n // 3] + at, mask))
+    d = bytearray(store)
+    d[off[n // 3]:off[n // 3] + 12] = bytes(12)
+    out["header_zeroed"] = (d, (off[n // 3], off[n // 3] + 12))
+    d = bytearray(store)
+    z = off[n // 4] + 40
+    d[z:z + 100000] = bytes(100000)
+    out["zeroed_100k"] = (d, (z, z + 100000))
+    d = bytearray(store)
+    d[off[n // 5] + 2] ^= 0x01
+    d[off[3 * n // 5]:off[3 * n // 5] + 12] = bytes(12)
+    out["two_breaks"] = (d, (off[n // 5] + 2, off[3 * n // 5] + 12))
+    assert recs[0][1] == UUID
+    d = bytearray(store)
+    out["first_record"] = (d, flip(d, off[0] + 3, 0x04))
+    dl = next(i for i, r in enumerate(recs) if r[3] == ST_DELETED)
+    d = bytearray(store)
+    out["deleted_length"] = (d, flip(d, off[dl] + 2, 0x01))
+    d = bytearray(store)
+    out["last_payload"] = (d, flip(d, off[-1] + 12 + 50, 0x08))
+    d = bytearray(store)
+    out["last_length"] = (d, flip(d, off[-1] + 3, 0x04))
+    return {k: (bytes(v), s) for k, (v, s) in out.items()}

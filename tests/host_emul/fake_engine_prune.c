@@ -1,7 +1,7 @@
 /*
  * fake_engine_prune.c — a stand-in for the engine's gossip_store prune (sv_gossip_prune_count, sv_prune_gossip_store_host
- * of cln_sigverify.h) whose walk stops where gossmap's does on a torn store, linked beside fake_engine.c or
- * fake_engine_timed.c so that sv_prune_gossip_store_fd and sv_repair_gossip_store_fd
+ * of cln_sigverify.h) whose walk stops where gossmap's does on a torn store, linked beside fake_engine.c so that
+ * sv_prune_gossip_store_fd and sv_repair_gossip_store_fd
  * (lightning_b200/csrc/gossip_store_fd.c), the verifier subdaemon's prune and repair requests and the drop-in's
  * gossip_store_prune and gossip_store_repair can be tested without a GPU (tests/test_sigverifyd_prune_fake.py,
  * tests/test_sigverifyd_repair_fake.py).  It deletes a fixed set of records for fixed reasons, which the tests recompute:
@@ -15,37 +15,14 @@
  *   delete  entry r (0-based, in walk order) when r % 3 == 1 and it is not deleted yet, for reason 1 + (r / 3) % 8
  *           (SV_GP_BAD_CRC .. SV_GP_UNKNOWN); reverified counts the SV_GP_SIGNATURE deletions
  * A major version other than 0, len 0 or rec_capacity below the entry count: SV_ERR_ARG, nothing written.  Each call
- * appends "sv_prune_gossip_store_host 0 <entries> <len>" to $FAKE_ENGINE_LOG.  Like fake_engine_timed.c, a
- * "sv_prune_gossip_store_host=<ms>" entry in $FAKE_ENGINE_DELAY holds each call that long, between a
- * "begin sv_prune_gossip_store_host 0" and an "end sv_prune_gossip_store_host 0" line in $FAKE_ENGINE_TRACE.
+ * can be delayed and traced (fake_engine.h) before it checks its arguments, and logs
+ * "sv_prune_gossip_store_host 0 <entries> <len>" once they pass.
  */
-#define _POSIX_C_SOURCE 200809L /* nanosleep */
-#include "../../include/cln_sigverify.h"
+#include "fake_engine.h"
 
-#include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
-#include <time.h>
 
 #define FN "sv_prune_gossip_store_host"
-
-static void append(const char *var, const char *line) {
-    const char *path = getenv(var);
-    FILE *f = path ? fopen(path, "a") : NULL;
-    if (!f) return;
-    fputs(line, f);
-    fclose(f);
-}
-static long prune_delay_ms(void) {
-    const char *d = getenv("FAKE_ENGINE_DELAY");
-    size_t fl = strlen(FN);
-    while (d && *d) {
-        if (!strncmp(d, FN, fl) && d[fl] == '=') return strtol(d + fl + 1, NULL, 10);
-        d = strchr(d, ',');
-        if (d) d++;
-    }
-    return 0;
-}
 
 /* the walk: each entry's offset into offs (if given); returns the entry count, *end and *stop where it ended */
 static size_t walk(const uint8_t *s, size_t len, uint64_t *end, int32_t *stop, uint64_t *offs) {
@@ -80,20 +57,12 @@ int sv_prune_gossip_store_host(sv_ctx *ctx, const uint8_t *store, size_t len, co
                                uint64_t *rec_off, uint16_t *rec_type, int *rec_status, uint8_t *rec_pruned,
                                size_t rec_capacity, sv_gossip_prune_summary *sum) {
     (void)chain_hash32;
-    char line[128];
-    long ms = prune_delay_ms();
-    append("FAKE_ENGINE_TRACE", "begin " FN " 0\n");
-    if (ms > 0) {
-        struct timespec t = {ms / 1000, (ms % 1000) * 1000000L};
-        while (nanosleep(&t, &t) != 0) {}
-    }
-    append("FAKE_ENGINE_TRACE", "end " FN " 0\n");
+    fake_enter(FN, ctx);
     if (!ctx || !store || !out || !len || !sum || (store[0] >> 5)) return SV_ERR_ARG;
     uint64_t end;
     int32_t stop;
     size_t n = walk(store, len, &end, &stop, NULL);
-    snprintf(line, sizeof line, FN " 0 %zu %zu\n", n, len);
-    append("FAKE_ENGINE_LOG", line);
+    fake_log(FN, 0, n, len);
     if (n > rec_capacity || (n && (!rec_off || !rec_type || !rec_status || !rec_pruned))) return SV_ERR_ARG;
     if (out != store) memcpy(out, store, len);
     walk(store, len, &end, &stop, rec_off);

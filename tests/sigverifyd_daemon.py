@@ -14,23 +14,29 @@ from lightning_b200 import build
 from lightning_b200 import sigverifyd_wire as W
 
 
+class Socket(str):
+    """a running daemon's socket path; .proc is the daemon's process"""
+
+
 @contextlib.contextmanager
 def running(tmp_path, binary=build.DAEMON, env=None):
-    """runs `binary <dir>/sv.sock 0` and yields the socket path once it is up; the daemon is stopped (killed if need be)
-    however the block ends.  The socket goes under tmp_path when its path fits a unix socket address (108 bytes with the
-    NUL), else into a short directory of its own under /tmp, removed afterwards."""
+    """runs `binary <dir>/sv.sock 0` and yields the socket path, a Socket, once it is up; the daemon is stopped (killed if
+    need be) however the block ends.  The socket goes under tmp_path when its path fits a unix socket address (108 bytes
+    with the NUL), else into a short directory of its own under /tmp, removed afterwards."""
     short = None
     if len(os.fsencode(tmp_path / "sv.sock")) >= 100:
         short = tempfile.mkdtemp(prefix="sv", dir="/tmp")
     sock_path = os.path.join(short or str(tmp_path), "sv.sock")
     proc = subprocess.Popen([binary, sock_path, "0"], stderr=subprocess.PIPE, env=env)
     try:
-        for _ in range(600):
+        for _ in range(1200):
             if os.path.exists(sock_path) or proc.poll() is not None:
                 break
-            time.sleep(0.1)
+            time.sleep(0.05)
         assert os.path.exists(sock_path), "daemon did not come up"
-        yield sock_path
+        sock = Socket(sock_path)
+        sock.proc = proc
+        yield sock
     finally:
         proc.terminate()
         try:

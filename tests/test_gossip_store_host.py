@@ -10,14 +10,11 @@ import numpy as np
 import pytest
 
 from tests import gossip_store as gs
+from tests.gossip_store import load_fixture
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 P8 = ctypes.POINTER(ctypes.c_uint8)
 CHAIN = bytes.fromhex("43497fd7f826957108f4a30fd9cec3aeba79972084e90ead01ea330900000000")
-
-
-def load_fixture():
-    return open(os.path.join(GOLD, "gossip_store_subset.bin"), "rb").read()
 
 
 def _p(a):

@@ -3,13 +3,12 @@ the checksum of a long candidate in the warp's 32 slices, the walk) against the 
 on the fixture and on every damage class; what the model makes of each class pruned by the prune's model, cut by the
 repair's rule and loaded by Core Lightning's gossmap.c strictly, as gossipd loads its store at start-up; and
 sv_salvage_gossip_store_fd (lightning_b200/csrc/gossip_salvage_fd.c) built with gcc against a CPU salvage and the fake
-prune of tests/host_emul/fake_engine_prune.c, with every pwrite it makes logged.  CLN's answers are recorded under
+prune of tests/host_emul/fake_engine_prune.c (with the fake engine it is part of), with every pwrite it makes logged.  CLN's answers are recorded under
 tests/golden/oracle/ (tests/oracle_replay.py)."""
 import ctypes
 import errno
 import os
 import struct
-import subprocess
 
 import numpy as np
 import pytest
@@ -19,10 +18,11 @@ from lightning_b200.engine import SvGossipPruneSummary, SvGossipSalvageSummary
 from tests import gossip_store as gs
 from tests import gossip_store_prune as gp
 from tests import gossip_store_salvage as sv
-from tests.test_gossip_store_host import load_fixture
+from tests import sigverifyd_fake as sf
+from tests.gossip_store import load_fixture
+from tests.gossip_store_salvage import damage_classes, with_uuid
+from tests.sigverifyd_fake import cut_rule, fake_prune
 from tests.test_gossip_store_prune_host import oracle, strict_load
-from tests.test_sigverifyd_prune_fake import fake_prune
-from tests.test_sigverifyd_repair_fake import cut_rule
 
 HE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "host_emul")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -33,18 +33,7 @@ def _p(a):
     return a.ctypes.data_as(ctypes.c_void_p)
 
 
-# ---- the stores and the damage classes (tests/test_gpu_gossip_store_salvage.py uses them too) -------------------------
-def with_uuid(store):
-    """store with a gossip_store_uuid record first, as gossipd starts a store, and one channel_update deleted the way
-    gossipd deletes (its checksum kept)"""
-    uuid = gs.record(struct.pack(">H", gs.UUID) + bytes(range(32)))
-    out = bytearray(store[:1] + uuid + store[1:])
-    recs = gs.walk(bytes(out))[0]
-    upd = [r for r in recs if r[1] == 258][len(recs) // 5]
-    out[upd[0]] |= gs.DELETED >> 8
-    return bytes(out)
-
-
+# ---- the stores (tests/test_gpu_gossip_store_salvage.py uses them too) ------------------------------------------------
 def x53():
     fx = load_fixture()
     return fx[:1] + fx[1:] * 53
@@ -62,44 +51,6 @@ def header_flips(store):
             d[o + at] ^= mask
             out["%s_%d" % (name, i)] = (bytes(d), i)
     return out
-
-
-def damage_classes(store):
-    """name -> (damaged store, (first, end) of the damaged bytes) of a with_uuid() store"""
-    recs = gs.walk(store)[0]
-    n = len(recs)
-    off = [r[0] for r in recs]
-
-    def flip(d, o, mask):
-        d[o] ^= mask
-        return o, o + 1
-
-    out = {}
-    for name, at, mask in (("len_hi", 2, 0x01), ("len_lo", 3, 0x10), ("completed", 0, 0x20)):
-        d = bytearray(store)
-        out[name] = (d, flip(d, off[n // 3] + at, mask))
-    d = bytearray(store)
-    d[off[n // 3]:off[n // 3] + 12] = bytes(12)
-    out["header_zeroed"] = (d, (off[n // 3], off[n // 3] + 12))
-    d = bytearray(store)
-    z = off[n // 4] + 40
-    d[z:z + 100000] = bytes(100000)
-    out["zeroed_100k"] = (d, (z, z + 100000))
-    d = bytearray(store)
-    d[off[n // 5] + 2] ^= 0x01
-    d[off[3 * n // 5]:off[3 * n // 5] + 12] = bytes(12)
-    out["two_breaks"] = (d, (off[n // 5] + 2, off[3 * n // 5] + 12))
-    assert recs[0][1] == gs.UUID
-    d = bytearray(store)
-    out["first_record"] = (d, flip(d, off[0] + 3, 0x04))
-    dl = next(i for i, r in enumerate(recs) if r[3] == gs.ST_DELETED)
-    d = bytearray(store)
-    out["deleted_length"] = (d, flip(d, off[dl] + 2, 0x01))
-    d = bytearray(store)
-    out["last_payload"] = (d, flip(d, off[-1] + 12 + 50, 0x08))
-    d = bytearray(store)
-    out["last_length"] = (d, flip(d, off[-1] + 3, 0x04))
-    return {k: (bytes(v), s) for k, (v, s) in out.items()}
 
 
 # ---- the host build against the model --------------------------------------------------------------------------------
@@ -285,19 +236,12 @@ def test_strict_load_accepts_every_class():
 def fdlib(tmp_path_factory):
     d = tmp_path_factory.mktemp("salvage_fd")
     objs = []
-    for src in (os.path.join(build.CSRC, "gossip_store_fd.c"), os.path.join(build.CSRC, "gossip_salvage_fd.c"),
-                os.path.join(HE, "fake_engine_prune.c"), os.path.join(HE, "pwrite_log.c")):
+    for src in (sf.STORE_FD, sf.SALVAGE_FD, sf.FAKE_PRUNE, sf.FAKE, os.path.join(HE, "pwrite_log.c")):
         o = str(d / (os.path.basename(src) + ".o"))
-        r = subprocess.run(["gcc"] + build.DROPIN_CFLAGS + ["-c", src, "-o", o], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr
+        sf.gcc(build.DROPIN_CFLAGS + ["-c", src, "-o", o])
         objs.append(o)
-    o = str(d / "fake_engine_salvage.o")
-    r = subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-Wall", "-Wno-unused-function", "-c",
-                        os.path.join(HE, "fake_engine_salvage.cpp"), "-o", o], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
     lib = str(d / "libsalvage_fd.so")
-    r = subprocess.run(["g++", "-shared", "-Wl,--wrap=pwrite,--wrap=fsync"] + objs + [o, "-o", lib], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
+    sf.gcc(["-shared", "-Wl,--wrap=pwrite,--wrap=fsync"] + objs + [sf.fake_salvage_o(d), "-o", lib], cc="g++")
     L = ctypes.CDLL(lib, use_errno=True)
     L.sv_salvage_gossip_store_fd.argtypes = [ctypes.c_void_p, ctypes.c_int, U64, ctypes.c_void_p,
                                              ctypes.POINTER(SvGossipPruneSummary), ctypes.POINTER(SvGossipSalvageSummary),

@@ -8,7 +8,7 @@ x53 with 1 % of its records corrupted (tests/test_gpu_gossip_store_prune.py), at
 x53 store is 51 MB, so not at every byte).  For each torn store T with cut = sv_gossip_prune_cut of its prune:
   - the repaired file is byte for byte prune(T)[:cut] (prune = SigVerifier.prune_gossip_store on the same bytes), and
     also prune(untorn store[:cut]): the torn tail changes nothing before the cut;
-  - cut is where the rule puts it (tests/test_sigverifyd_repair_fake.py cut_rule), and the record boundary the tear
+  - cut is where the rule puts it (tests/sigverifyd_fake.py cut_rule), and the record boundary the tear
     lies behind;
   - CLN's strict load (oracle/gossmap_strict_harness.c, expected_len = the new length) accepts the repaired file, and its
     channel table equals that of CLN's lenient load (oracle/gossmap_harness.c) of prune(T) uncut, which stops at the cut:
@@ -39,8 +39,7 @@ from tests.test_gossmap import gossmap_load
 from tests.test_gpu_gossip_burst import PUB, SK, TESTNET, _ordered, _sha256d, make_ca, make_cu
 from tests.test_gpu_gossip_store import TOOL
 from tests.test_gpu_gossip_store_prune import corrupted_x53
-from tests.test_sigverifyd_prune_fake import case, run_client
-from tests.test_sigverifyd_repair_fake import cut_rule
+from tests.sigverifyd_fake import case, cut_rule, run_client
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -25,12 +25,14 @@ from lightning_b200 import build
 from tests import gossip_store as gs
 from tests import gossip_store_salvage as sv
 from tests import sigverifyd_daemon
+from tests.gossip_store_salvage import damage_classes, with_uuid
+from tests.sigverifyd_fake import run_client
+from tests.sigverifyd_fake import salvage_case as case
 from tests.test_gossip_store_host import load_fixture
 from tests.test_gossip_store_prune_host import oracle, strict_load
-from tests.test_gossip_store_salvage_host import damage_classes, header_flips, kept_changes, with_uuid, x53
+from tests.test_gossip_store_salvage_host import header_flips, kept_changes, x53
 from tests.test_gpu_gossip_burst import TESTNET
 from tests.test_gpu_gossip_store import TOOL
-from tests.test_sigverifyd_salvage_fake import case, run_client
 
 pytestmark = pytest.mark.gpu
 

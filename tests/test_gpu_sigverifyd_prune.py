@@ -17,7 +17,7 @@ from lightning_b200 import sigverifyd_wire as W
 from tests import sigverifyd_daemon, txsig
 from tests.test_gpu_gossip_burst import TESTNET
 from tests.test_gpu_gossip_store_prune import corrupted_x53, mutations
-from tests.test_sigverifyd_prune_fake import FIELDS, case, prune_frame, run_client
+from tests.sigverifyd_fake import FIELDS, case, prune_frame, run_client
 
 pytestmark = pytest.mark.gpu
 

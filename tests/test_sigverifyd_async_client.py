@@ -11,11 +11,10 @@ import sys
 
 import pytest
 
-from lightning_b200 import build
 from tests import sigverifyd_daemon
+from tests import sigverifyd_fake as sf
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-FAKE = os.path.join(ROOT, "tests", "host_emul", "fake_engine.c")
 
 # The client: python -c DRIVER <library> <mode> [args].  It builds seeded random inputs for every function that has a
 # _start, runs them as tickets and / or blocking calls as the mode says, and prints what it saw as JSON.
@@ -249,21 +248,11 @@ print(json.dumps(out))
 """
 
 
-def _gcc(args):
-    r = subprocess.run(["gcc"] + args, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-
-
 @pytest.fixture(scope="module")
 def bins(tmp_path_factory):
     d = tmp_path_factory.mktemp("async_client")
-    out = dict(daemon=str(d / "cln_sigverifyd"), lib=str(d / "libcln_dropin_fake.so"),
-               inproc=str(d / "libcln_dropin_inproc.so"))
-    _gcc(build.DAEMON_CFLAGS + [os.path.join(build.CSRC, "sigverifyd.c"), FAKE, "-o", out["daemon"]])
-    _gcc(build.DROPIN_CFLAGS + ["-shared", "-DFAKE_ENGINE_NO_CONTEXT", os.path.join(build.CSRC, "cln_dropin.c"), FAKE,
-                                "-o", out["lib"]])
-    _gcc(build.DROPIN_CFLAGS + ["-shared", os.path.join(build.CSRC, "cln_dropin.c"), FAKE, "-o", out["inproc"]])
-    return out
+    return dict(daemon=sf.daemon(d / "cln_sigverifyd"), lib=sf.dropin(d / "libcln_dropin_fake.so"),
+                inproc=sf.dropin(d / "libcln_dropin_inproc.so", client=False))
 
 
 def _env(**kw):
@@ -285,13 +274,8 @@ def _run(lib, mode, *args, env=None, ok=True):
 @pytest.fixture
 def fake(tmp_path, bins):
     """a daemon on the fake engine, and the engine's call log"""
-    log = tmp_path / "engine.log"
-    with sigverifyd_daemon.running(tmp_path, bins["daemon"], env=dict(os.environ, FAKE_ENGINE_LOG=str(log))) as sock:
-        yield sock, log
-
-
-def _calls(log):
-    return [tuple(line.split()) for line in log.read_text().splitlines()] if log.exists() else []
+    with sigverifyd_daemon.running(tmp_path, bins["daemon"], sf.env(tmp_path)) as sock:
+        yield sock, tmp_path / "engine.log"
 
 
 def test_mixed_tickets_match_blocking_calls(fake, bins):
@@ -318,14 +302,12 @@ def test_a_window_shares_engine_calls(tmp_path, bins, k):
         log = tmp_path / ("engine_%s.log" % how)
         outs[how] = _run(bins["lib"], "window", k, how, bins["daemon"], env=_env(FAKE_ENGINE_LOG=str(log)))
         assert outs[how]["daemon_rc"] == 0
-        logs[how] = [c[:3] for c in _calls(log)]
+        logs[how] = [c[:3] for c in sf.calls(log)]
     assert outs["tickets"]["answers"] == outs["blocking"]["answers"]
     assert outs["tickets"]["order"] == list(range(1, 3 * k + 1))
-    assert logs["tickets"] == [("sv_verify_host", "1", str(k)), ("sv_verify_bolt12_tagged_host", "0", str(k)),
-                               ("sv_verify_tx_host", "1", str(k))]
-    assert sorted(logs["blocking"]) == sorted([("sv_verify_host", "1", "1")] * k +
-                                              [("sv_verify_bolt12_tagged_host", "0", "1")] * k +
-                                              [("sv_verify_tx_host", "1", "1")] * k)
+    assert logs["tickets"] == [("sv_verify_host", 1, k), ("sv_verify_bolt12_tagged_host", 0, k), ("sv_verify_tx_host", 1, k)]
+    assert sorted(logs["blocking"]) == sorted([("sv_verify_host", 1, 1)] * k + [("sv_verify_bolt12_tagged_host", 0, 1)] * k +
+                                              [("sv_verify_tx_host", 1, 1)] * k)
 
 
 def test_blocking_calls_between_tickets(fake, bins):

@@ -16,14 +16,12 @@ import threading
 import numpy as np
 import pytest
 
-from lightning_b200 import build
 from lightning_b200 import sigverifyd_wire as W
 from tests import sigverifyd_daemon
-from tests.test_sigverifyd_fake_engine import (FAKE, TAGS, _calls, _gcc, _roundtrip, _start, bolt12_req, fill, fnv, patched,
-                                               short, verify_req)
+from tests import sigverifyd_fake as sf
+from tests.sigverifyd_fake import FAKE_BOLT11, TAGS, bolt12_req, calls, fill, fnv, patched, roundtrip, short, verify_req
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-FAKE_BOLT11 = os.path.join(ROOT, "tests", "host_emul", "fake_engine_bolt11.c")
 MAX_ITEMS = 1 << 20
 SMALL = dict(CALL_ITEMS=8, HASH_CALL_BYTES=200)  # per-call limits of the small-limits daemon
 
@@ -62,23 +60,17 @@ def bins(tmp_path_factory):
     """the daemon and the drop-in (client mode and in-process) on the fake engine with its BOLT11 check, a daemon with small
     call limits, and a daemon without the check"""
     d = tmp_path_factory.mktemp("fake_bolt11")
-    out = dict(daemon=str(d / "cln_sigverifyd"), bare=str(d / "cln_sigverifyd_bare"), small=str(d / "cln_sigverifyd_small"),
-               lib=str(d / "libcln_dropin_fake.so"), inproc=str(d / "libcln_dropin_inproc.so"))
-    daemon_src, dropin_src = os.path.join(build.CSRC, "sigverifyd.c"), os.path.join(build.CSRC, "cln_dropin.c")
-    _gcc(build.DAEMON_CFLAGS + [daemon_src, FAKE, FAKE_BOLT11, "-o", out["daemon"]])
-    _gcc(build.DAEMON_CFLAGS + [daemon_src, FAKE, "-o", out["bare"]])
-    _gcc(build.DAEMON_CFLAGS + ["-D%s=%d" % kv for kv in SMALL.items()] + [daemon_src, FAKE, FAKE_BOLT11, "-o", out["small"]])
-    _gcc(build.DROPIN_CFLAGS + ["-shared", "-DFAKE_ENGINE_NO_CONTEXT", dropin_src, FAKE, FAKE_BOLT11, "-o", out["lib"]])
-    _gcc(build.DROPIN_CFLAGS + ["-shared", dropin_src, FAKE, FAKE_BOLT11, "-o", out["inproc"]])
-    return out
+    return dict(daemon=sf.daemon(d / "cln_sigverifyd", FAKE_BOLT11), bare=sf.daemon(d / "cln_sigverifyd_bare"),
+                small=sf.daemon(d / "cln_sigverifyd_small", FAKE_BOLT11, limits=SMALL),
+                lib=sf.dropin(d / "libcln_dropin_fake.so", FAKE_BOLT11),
+                inproc=sf.dropin(d / "libcln_dropin_inproc.so", FAKE_BOLT11, client=False))
 
 
 @pytest.fixture
 def fake(tmp_path, bins):
     """a daemon on the fake engine with its BOLT11 check, and the engine's call log"""
-    ctx, log = _start(tmp_path, bins["daemon"])
-    with ctx as sock:
-        yield sock, log
+    with sigverifyd_daemon.running(tmp_path, bins["daemon"], sf.env(tmp_path)) as sock:
+        yield sock, tmp_path / "engine.log"
 
 
 def test_clients_get_every_reply_in_order(fake):
@@ -105,7 +97,7 @@ def test_clients_get_every_reply_in_order(fake):
             j = 0
             while j < len(reqs):
                 k = int(rng.integers(1, 5))
-                _roundtrip(c, reqs[j:j + k])
+                roundtrip(c, reqs[j:j + k])
                 j += k
             c.close()
         except Exception as ex:  # noqa: BLE001
@@ -118,7 +110,7 @@ def test_clients_get_every_reply_in_order(fake):
         t.join(timeout=120)
     assert not errors, errors
     assert sigverifyd_daemon.stats(sock)["requests"] == 240
-    assert sum(c[2] for c in _calls(log) if c[0] == "sv_verify_bolt11_host") == sum(invoices)
+    assert sum(c[2] for c in calls(log) if c[0] == "sv_verify_bolt11_host") == sum(invoices)
 
 
 def test_one_write_is_one_pass(fake):
@@ -129,9 +121,9 @@ def test_one_write_is_one_pass(fake):
     reqs = [sized_req(rng, 1, [30, 0, 7]), verify_req(rng, 2, 0, 2), sized_req(rng, 3, [100]),
             bolt12_req(rng, 4, *TAGS[0], [12], 0), sized_req(rng, 5, []), sized_req(rng, 6, [5, 5, 5, 5])]
     c = sigverifyd_daemon.connect(sock)
-    _roundtrip(c, reqs)
+    roundtrip(c, reqs)
     c.close()
-    assert _calls(log) == [("sv_verify_host", 0, 2, 0), ("sv_verify_bolt12_tagged_host", 0, 1, 12),
+    assert calls(log) == [("sv_verify_host", 0, 2, 0), ("sv_verify_bolt12_tagged_host", 0, 1, 12),
                            ("sv_verify_bolt11_host", 0, 8, 157)]
     st = sigverifyd_daemon.stats(sock)
     assert st["requests"] == 6 and st["launches"] == 3 and st["signatures"] == 2 + 1 + 8 and st["max_coalesced"] == 4, st
@@ -140,11 +132,11 @@ def test_one_write_is_one_pass(fake):
 def test_call_limits_split_at_request_boundaries(tmp_path, bins):
     """with small per-call limits (8 invoices, 200 bytes), a pass is cut into sv_verify_bolt11_host calls at request
     boundaries, by invoices and by bytes, a request above a limit alone; every reply is still the fake's"""
-    ctx, log = _start(tmp_path, bins["small"])
+    log = tmp_path / "engine.log"
     rng = np.random.default_rng(13)
-    with ctx as sock:
+    with sigverifyd_daemon.running(tmp_path, bins["small"], sf.env(tmp_path)) as sock:
         c = sigverifyd_daemon.connect(sock)
-        _roundtrip(c, [sized_req(rng, 1, [10, 10, 10]), sized_req(rng, 2, [10] * 4),  # 7 invoices, 70 bytes
+        roundtrip(c, [sized_req(rng, 1, [10, 10, 10]), sized_req(rng, 2, [10] * 4),  # 7 invoices, 70 bytes
                        sized_req(rng, 3, [50] * 3),                                  # 10 invoices > 8: a new call
                        sized_req(rng, 4, [60]),                                      # 150 + 60 bytes > 200: a new call
                        sized_req(rng, 5, []),
@@ -152,7 +144,7 @@ def test_call_limits_split_at_request_boundaries(tmp_path, bins):
                        sized_req(rng, 7, [250]),                                     # 250 bytes > 200: alone
                        sized_req(rng, 8, [3, 3])])
         c.close()
-    assert _calls(log) == [("sv_verify_bolt11_host", 0, 7, 70), ("sv_verify_bolt11_host", 0, 3, 150),
+    assert calls(log) == [("sv_verify_bolt11_host", 0, 7, 70), ("sv_verify_bolt11_host", 0, 3, 150),
                            ("sv_verify_bolt11_host", 0, 1, 60), ("sv_verify_bolt11_host", 0, 9, 9),
                            ("sv_verify_bolt11_host", 0, 1, 250), ("sv_verify_bolt11_host", 0, 2, 6)]
 
@@ -172,10 +164,10 @@ def test_malformed_requests_are_refused(fake):
     for b, rid in bad:
         c.sendall(b)
         assert W.read_msg(c) == ("sigverifyd_error", dict(req_id=rid, code=1))
-    assert _calls(log) == []
-    _roundtrip(c, [(frame, want)])
+    assert calls(log) == []
+    roundtrip(c, [(frame, want)])
     c.close()
-    assert _calls(log) == [("sv_verify_bolt11_host", 0, 2, 100)]
+    assert calls(log) == [("sv_verify_bolt11_host", 0, 2, 100)]
     assert sigverifyd_daemon.stats(sock)["requests"] == 1
 
 
@@ -183,14 +175,14 @@ def test_engine_without_bolt11_refuses(tmp_path, bins):
     """a daemon linked against an engine without sv_verify_bolt11_host answers a BOLT11 request with error 1 and keeps
     serving"""
     rng = np.random.default_rng(5)
-    ctx, log = _start(tmp_path, bins["bare"])
-    with ctx as sock:
+    log = tmp_path / "engine.log"
+    with sigverifyd_daemon.running(tmp_path, bins["bare"], sf.env(tmp_path)) as sock:
         c = sigverifyd_daemon.connect(sock)
         c.sendall(sized_req(rng, 11, [80])[0])
         assert W.read_msg(c) == ("sigverifyd_error", dict(req_id=11, code=1))
-        _roundtrip(c, [verify_req(rng, 12, 0, 2)])
+        roundtrip(c, [verify_req(rng, 12, 0, 2)])
         c.close()
-    assert [x[0] for x in _calls(log)] == ["sv_verify_host"]
+    assert [x[0] for x in calls(log)] == ["sv_verify_host"]
 
 
 # the drop-in: python -c CLIENT <library> <invoices.json> [window]; prints the answers of the blocking calls and, with a
@@ -261,8 +253,8 @@ def test_dropin_client_mode(tmp_path, bins):
     rng = np.random.default_rng(21)
     strings = _strings(rng, 300)
     want = [[st, node.hex()] for st, node in map(answer, strings)]
-    ctx, log = _start(tmp_path, bins["daemon"])
-    with ctx as sock:
+    log = tmp_path / "engine.log"
+    with sigverifyd_daemon.running(tmp_path, bins["daemon"], sf.env(tmp_path)) as sock:
         out = _client(tmp_path, bins["lib"], strings, window=64, env=_env(CLN_SIGVERIFYD_SOCKET=sock))
         st = sigverifyd_daemon.stats(sock)
     assert out["blocking"] == want and out["async"] == want
@@ -270,8 +262,8 @@ def test_dropin_client_mode(tmp_path, bins):
     assert out["order"] == list(range(1, 301))
     assert out["tickets"] == sorted(out["tickets"]) and len(set(out["tickets"])) == 300 and min(out["tickets"]) > 0
     assert st["requests"] == 600 and st["signatures"] == 600, st
-    calls = [c for c in _calls(log) if c[0] == "sv_verify_bolt11_host"]
-    assert sum(c[2] for c in calls) == 600 and len(calls) < 600  # the window shared engine calls
+    b11 = [c for c in calls(log) if c[0] == "sv_verify_bolt11_host"]
+    assert sum(c[2] for c in b11) == 600 and len(b11) < 600  # the window shared engine calls
 
 
 def test_dropin_reply_with_bad_status_aborts(tmp_path, bins):

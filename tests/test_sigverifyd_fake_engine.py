@@ -13,130 +13,15 @@ import threading
 import numpy as np
 import pytest
 
-from lightning_b200 import build
 from lightning_b200 import sigverifyd_wire as W
 from tests import sigverifyd_daemon, txsig
+from tests import sigverifyd_fake as sf
+from tests.sigverifyd_fake import (TAGS, TESTNET, bolt12_req, burst_req, calls, fill, fnv, gossip_req, key_req, le, patched,
+                                   rand, rev, roundtrip, sha_req, short, tx_hash, tx_req, verify_req)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-FAKE = os.path.join(ROOT, "tests", "host_emul", "fake_engine.c")
-KS = {0: 33, 1: 64, 2: 32}
 MAX_FRAME = 32 + (1 << 20) * 161
 SMALL = dict(CALL_ITEMS=8, HASH_CALL_BYTES=200, TX_CALL_BYTES=600)  # per-call limits of the small-limits daemon
-TESTNET = bytes.fromhex("43497fd7f826957108f4a30fd9cec3aeba79972084e90ead01ea330900000000")
-
-
-# ---- the fake engine's functions (fake_engine.c) -----------------------------------------------------------------------
-def fnv(data, h=0xcbf29ce484222325):
-    for b in data:
-        h = ((h ^ b) * 0x100000001b3) & 0xFFFFFFFFFFFFFFFF
-    return h
-
-
-def fill(h, n):
-    return bytes(fnv(bytes([k]), h) & 0xFF for k in range(n))
-
-
-def wire(status):
-    return bytes(s & 0xFF for s in status)
-
-
-def le(v, n):
-    return int(v).to_bytes(n, "little")
-
-
-def tx_hash(kind, key, sig, f, spans):
-    """f: version, locktime, sequence, sighash_type, prev_txid, prev_index, flags, input_amount, output_amount"""
-    return fnv(bytes([kind]) + key + sig + b"".join(le(f[k], 4) for k in ("version", "locktime", "sequence", "sighash_type")) +
-               f["prev_txid"] + le(f["prev_index"], 4) + le(f["flags"], 4) + le(f["input_amount"], 8) +
-               le(f["output_amount"], 8) + b"".join(le(len(s), 4) + s for s in spans))
-
-
-# ---- requests and the replies the fake dictates ---------------------------------------------------------------------
-def _rand(rng, n):
-    return rng.integers(0, 256, size=n, dtype=np.uint8).tobytes()
-
-
-def verify_req(rng, rid, kind, n):
-    h, k, s = _rand(rng, 32 * n), _rand(rng, KS[kind] * n), _rand(rng, 64 * n)
-    ks = KS[kind]
-    v = bytes(fnv(bytes([kind]) + h[32 * i:32 * i + 32] + k[ks * i:ks * i + ks] + s[64 * i:64 * i + 64]) % 3 for i in range(n))
-    return (W.encode("sigverifyd_verify", req_id=rid, kind=kind, n=n, hashes=h, keylen=ks * n, keys=k, sigs=s),
-            ("sigverifyd_verify_reply", dict(req_id=rid, n=n, verdicts=v)))
-
-
-def bolt12_req(rng, rid, mn, fn, sizes, want):
-    n = len(sizes)
-    streams = [_rand(rng, x) for x in sizes]
-    xo, sg = _rand(rng, 32 * n), _rand(rng, 64 * n)
-    hs = [fnv(mn + b"\0" + fn + b"\0" + streams[i] + xo[32 * i:32 * i + 32] + sg[64 * i:64 * i + 64]) for i in range(n)]
-    blob = b"".join(streams)
-    frame = W.encode("sigverifyd_bolt12", req_id=rid, mnlen=len(mn), messagename=mn, fnlen=len(fn), fieldname=fn, n=n,
-                     lens=sizes, bloblen=len(blob), blob=blob, xonly=xo, sigs=sg, want_sighash=want)
-    return frame, ("sigverifyd_bolt12_reply", dict(req_id=rid, n=n, status=wire(h % 3 - 1 for h in hs),
-                                                   nsighash=n if want else 0,
-                                                   sighashes=b"".join(fill(h, 32) for h in hs) if want else b""))
-
-
-def tx_req(rng, rid, kind, spans, want):
-    """spans: per transaction the lengths of (script, outputs, outpoints, sequences)"""
-    n = len(spans)
-    key, sigs = _rand(rng, KS[kind]), _rand(rng, 64 * n)
-    recs, data, hs = [], [], []
-    for i, sp in enumerate(spans):
-        f = dict(version=int(rng.integers(1, 3)), locktime=int(rng.integers(0, 2**32)), sequence=int(rng.integers(0, 2**32)),
-                 sighash_type=int(rng.choice([1, 3, 0x83])), prev_txid=_rand(rng, 32), prev_index=int(rng.integers(0, 9)),
-                 flags=1 | (2 if sp[2] or sp[3] else 0), input_amount=int(rng.integers(0, 2**62)),
-                 output_amount=int(rng.integers(0, 2**62)))
-        b = [_rand(rng, x) for x in sp]
-        recs.append(f)
-        data += b
-        hs.append(tx_hash(kind, key, sigs[64 * i:64 * i + 64], f, b))
-    kw = {k: [r[k] for r in recs] for k in txsig.U32_FIELDS}
-    blob = b"".join(data)
-    frame = W.encode("sigverifyd_tx", req_id=rid, kind=kind, keylen=len(key), key=key, n=n,
-                     prev_txid=b"".join(r["prev_txid"] for r in recs), input_amount=[r["input_amount"] for r in recs],
-                     output_amount=[r["output_amount"] for r in recs], script_len=[s[0] for s in spans],
-                     outputs_len=[s[1] for s in spans], prevouts_len=[s[2] for s in spans],
-                     sequences_len=[s[3] for s in spans], bloblen=len(blob), blob=blob, sigs=sigs, want_sighash=want, **kw)
-    return frame, ("sigverifyd_tx_reply", dict(req_id=rid, n=n, verdicts=bytes(h % 3 for h in hs), nsighash=n if want else 0,
-                                               sighashes=b"".join(fill(h, 32) for h in hs) if want else b""))
-
-
-def sha_req(rng, rid, sizes):
-    bufs = [_rand(rng, x) for x in sizes]
-    blob = b"".join(bufs)
-    return (W.encode("sigverifyd_sha256d", req_id=rid, n=len(bufs), lens=sizes, bloblen=len(blob), blob=blob),
-            ("sigverifyd_sha256d_reply", dict(req_id=rid, n=len(bufs), hashes=b"".join(fill(fnv(b), 32) for b in bufs))))
-
-
-def key_req(rng, rid, n):
-    keys = _rand(rng, 33 * n)
-    hs = [fnv(keys[33 * i:33 * i + 33]) for i in range(n)]
-    return (W.encode("sigverifyd_pubkey", req_id=rid, n=n, keys=keys),
-            ("sigverifyd_pubkey_reply", dict(req_id=rid, n=n, ok=bytes(h % 3 for h in hs),
-                                             xy=b"".join(fill(h, 64) for h in hs))))
-
-
-def gossip_req(rng, rid, n):
-    msgs = [_rand(rng, int(rng.integers(2, 300))) for _ in range(n)]
-    sg = _rand(rng, 33 * n)
-    st = [fnv(m + sg[33 * i:33 * i + 33]) % 6 - 1 for i, m in enumerate(msgs)]
-    blob = b"".join(msgs)
-    return (W.encode("sigverifyd_gossip", req_id=rid, n=n, lens=[len(m) for m in msgs], signers=sg, bloblen=len(blob),
-                     blob=blob), ("sigverifyd_gossip_reply", dict(req_id=rid, n=n, status=wire(st))))
-
-
-def burst_req(rng, rid, n):
-    msgs = [_rand(rng, int(rng.integers(2, 300))) for _ in range(n)]
-    kinds, sg = bytes(int(x) for x in rng.integers(0, 3, size=n)), _rand(rng, 33 * n)
-    st = [fnv(TESTNET + m + kinds[i:i + 1] + sg[33 * i:33 * i + 33]) % 10 - 4 for i, m in enumerate(msgs)]
-    blob = b"".join(msgs)
-    return (W.encode("sigverifyd_gossip_burst", req_id=rid, chain_hash=TESTNET, n=n, lens=[len(m) for m in msgs],
-                     signer_kind=kinds, signers=sg, bloblen=len(blob), blob=blob),
-            ("sigverifyd_gossip_burst_reply", dict(req_id=rid, n=n, status=wire(st))))
-
-
-TAGS = [(b"invoice", b"signature"), (b"invoice_request", b"signature"), (b"offer", b"signature")]
 
 
 def any_req(rng, rid):
@@ -162,63 +47,18 @@ def any_req(rng, rid):
     return W.encode("sigverifyd_stats", req_id=rid), None
 
 
-def patched(frame, at, value):
-    """frame with the bytes at offset `at` of its message replaced"""
-    body = bytearray(frame[4:])
-    body[at:at + len(value)] = value
-    return len(body).to_bytes(4, "big") + bytes(body)
-
-
-def short(frame):
-    """frame one byte short of its fields"""
-    body = frame[4:-1]
-    return len(body).to_bytes(4, "big") + body
-
-
 # ---- builds and daemons ---------------------------------------------------------------------------------------------
-def _gcc(args):
-    r = subprocess.run(["gcc"] + args, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-
-
 @pytest.fixture(scope="module")
 def bins(tmp_path_factory):
     d = tmp_path_factory.mktemp("fake_engine")
-    out = dict(daemon=str(d / "cln_sigverifyd"), lib=str(d / "libcln_dropin_fake.so"))
-    _gcc(build.DAEMON_CFLAGS + [os.path.join(build.CSRC, "sigverifyd.c"), FAKE, "-o", out["daemon"]])
-    _gcc(build.DROPIN_CFLAGS + ["-shared", "-DFAKE_ENGINE_NO_CONTEXT", os.path.join(build.CSRC, "cln_dropin.c"), FAKE,
-                                "-o", out["lib"]])
-    return out
-
-
-def _start(tmp_path, binary):
-    log = tmp_path / "engine.log"
-    return sigverifyd_daemon.running(tmp_path, binary, env=dict(os.environ, FAKE_ENGINE_LOG=str(log))), log
+    return dict(daemon=sf.daemon(d / "cln_sigverifyd"), lib=sf.dropin(d / "libcln_dropin_fake.so"))
 
 
 @pytest.fixture
 def fake(tmp_path, bins):
     """a daemon on the fake engine, and the engine's call log"""
-    ctx, log = _start(tmp_path, bins["daemon"])
-    with ctx as sock:
-        yield sock, log
-
-
-def _calls(log):
-    if not log.exists():
-        return []
-    return [(f, int(k), int(n), int(b)) for f, k, n, b in (line.split() for line in log.read_text().splitlines())]
-
-
-def _roundtrip(c, reqs):
-    """sends the frames in one write, reads one reply per frame and checks each against what the fake dictates"""
-    c.sendall(b"".join(f for f, _ in reqs))
-    for frame, want in reqs:
-        got = W.read_msg(c)
-        if want is None:  # a stats request: its counters are checked elsewhere
-            assert got[0] == "sigverifyd_stats_reply" and got[1]["req_id"] == W.decode(frame[4:])[1]["req_id"]
-        else:
-            assert got == want, (got[0], got[1].get("req_id"), want[0], want[1]["req_id"])
+    with sigverifyd_daemon.running(tmp_path, bins["daemon"], sf.env(tmp_path)) as sock:
+        yield sock, tmp_path / "engine.log"
 
 
 # ---- (a)-(e): the daemon ----------------------------------------------------------------------------------------------
@@ -236,7 +76,7 @@ def test_clients_get_every_reply_in_order(fake):
             j = 0
             while j < len(reqs):
                 k = int(rng.integers(1, 5))
-                _roundtrip(c, reqs[j:j + k])
+                roundtrip(c, reqs[j:j + k])
                 j += k
             c.close()
         except Exception as ex:  # noqa: BLE001
@@ -260,9 +100,9 @@ def test_one_write_is_one_pass(fake):
             verify_req(rng, 7, 0, 1), tx_req(rng, 8, 0, [(30, 0, 0, 0)], 0), bolt12_req(rng, 9, *TAGS[1], [12], 0),
             verify_req(rng, 10, 1, 4), sha_req(rng, 11, [5]), key_req(rng, 12, 3), tx_req(rng, 13, 1, [(7, 7, 0, 0)], 0)]
     c = sigverifyd_daemon.connect(sock)
-    _roundtrip(c, reqs)
+    roundtrip(c, reqs)
     c.close()
-    assert _calls(log) == [("sv_verify_host", 0, 3, 0), ("sv_verify_host", 1, 4, 0), ("sv_verify_host", 2, 3, 0),
+    assert calls(log) == [("sv_verify_host", 0, 3, 0), ("sv_verify_host", 1, 4, 0), ("sv_verify_host", 2, 3, 0),
                            ("sv_verify_bolt12_tagged_host", 0, 3, 52), ("sv_verify_tx_host", 0, 1, 30),
                            ("sv_verify_tx_host", 1, 3, 10 + 20 + 5 + 9 + 72 + 8 + 14), ("sv_sha256d_host", 0, 4, 72),
                            ("sv_pubkey_parse_host", 0, 5, 0)]
@@ -304,8 +144,8 @@ def test_refusals(fake):
     refused((2).to_bytes(4, "big") + (3003).to_bytes(2, "big"), rid=0)                     # a stats request without its id
     refused((10).to_bytes(4, "big") + (3050).to_bytes(2, "big") + (99).to_bytes(8, "big"), code=3, rid=0)
     good = [sha_req(rng, 40, [1]), burst_req(rng, 41, 1)]
-    _roundtrip(c, good)
-    assert not any(f == "sv_verify_host" for f, *_ in _calls(log))  # nothing refused reached the engine
+    roundtrip(c, good)
+    assert not any(f == "sv_verify_host" for f, *_ in calls(log))  # nothing refused reached the engine
     c.sendall((MAX_FRAME + 1).to_bytes(4, "big"))
     c.settimeout(20)
     try:
@@ -328,12 +168,12 @@ def test_stats_counters(fake):
     rng = np.random.default_rng(11)
     c = sigverifyd_daemon.connect(sock)
     # one pass: verify kind 0 (2 requests, 5 signatures) and kind 2 (1), tx kind 1 (2 requests, 3), sha256d (1), pubkey (1)
-    _roundtrip(c, [verify_req(rng, 1, 0, 3), verify_req(rng, 2, 0, 2), verify_req(rng, 3, 2, 1),
+    roundtrip(c, [verify_req(rng, 1, 0, 3), verify_req(rng, 2, 0, 2), verify_req(rng, 3, 2, 1),
                    tx_req(rng, 4, 1, [(4, 4, 0, 0)], 0), tx_req(rng, 5, 1, [(4, 4, 0, 0), (1, 1, 0, 0)], 1),
                    sha_req(rng, 6, [5, 6]), key_req(rng, 7, 4)])
-    _roundtrip(c, [gossip_req(rng, 8, 3)])                 # one launch of its own
-    _roundtrip(c, [burst_req(rng, 9, 2)])                  # likewise
-    _roundtrip(c, [verify_req(rng, 10, 1, 0)])             # an empty request still counts as a launch
+    roundtrip(c, [gossip_req(rng, 8, 3)])                 # one launch of its own
+    roundtrip(c, [burst_req(rng, 9, 2)])                  # likewise
+    roundtrip(c, [verify_req(rng, 10, 1, 0)])             # an empty request still counts as a launch
     c.sendall(short(key_req(rng, 11, 1)[0]))              # refused: not counted
     assert W.read_msg(c) == ("sigverifyd_error", dict(req_id=11, code=1))
     st = sigverifyd_daemon.stats(sock)
@@ -345,14 +185,12 @@ def test_stats_counters(fake):
 def test_call_limits_split_at_request_boundaries(tmp_path):
     """with small per-call limits (SMALL), a pass is cut into engine calls at request boundaries: sha256d by items and by
     bytes, pubkey by items, tx by span bytes, a request above a limit alone; every reply is still the fake's"""
-    d = str(tmp_path / "cln_sigverifyd_small")
-    _gcc(build.DAEMON_CFLAGS + ["-D%s=%d" % kv for kv in SMALL.items()] + [os.path.join(build.CSRC, "sigverifyd.c"), FAKE,
-                                                                           "-o", d])
-    ctx, log = _start(tmp_path, d)
+    d = sf.daemon(tmp_path / "cln_sigverifyd_small", limits=SMALL)
+    log = tmp_path / "engine.log"
     rng = np.random.default_rng(13)
-    with ctx as sock:
+    with sigverifyd_daemon.running(tmp_path, d, sf.env(tmp_path)) as sock:
         c = sigverifyd_daemon.connect(sock)
-        _roundtrip(c, [sha_req(rng, 1, [10, 10, 10]), sha_req(rng, 2, [10] * 4),    # 7 items, 70 bytes
+        roundtrip(c, [sha_req(rng, 1, [10, 10, 10]), sha_req(rng, 2, [10] * 4),    # 7 items, 70 bytes
                        sha_req(rng, 3, [50] * 3),                                   # 10 items > 8: a new call
                        sha_req(rng, 4, [60]),                                       # 150 + 60 bytes > 200: a new call
                        sha_req(rng, 5, []),
@@ -362,7 +200,7 @@ def test_call_limits_split_at_request_boundaries(tmp_path):
                        tx_req(rng, 11, 1, [(50, 50, 0, 0)], 0),                     # 650 > 600: a new call
                        tx_req(rng, 12, 1, [(300, 300, 72, 28)], 1)])                # 700 bytes alone
         c.close()
-    assert _calls(log) == [("sv_verify_tx_host", 1, 3, 550), ("sv_verify_tx_host", 1, 1, 100),
+    assert calls(log) == [("sv_verify_tx_host", 1, 3, 550), ("sv_verify_tx_host", 1, 1, 100),
                            ("sv_verify_tx_host", 1, 1, 700), ("sv_sha256d_host", 0, 7, 70), ("sv_sha256d_host", 0, 3, 150),
                            ("sv_sha256d_host", 0, 1, 60), ("sv_pubkey_parse_host", 0, 8, 0), ("sv_pubkey_parse_host", 0, 2, 0)]
 
@@ -469,11 +307,6 @@ print(json.dumps(out))
 """
 
 
-def _rev(b):
-    """libsecp256k1's opaque structs hold two 32-byte numbers as little-endian limbs"""
-    return b[31::-1] + b[:31:-1]
-
-
 def _ser_out(sat, s):
     return le(sat, 8) + (bytes([len(s)]) if len(s) < 0xFD else b"\xfd" + le(len(s), 2)) + s
 
@@ -488,43 +321,43 @@ def test_dropin_client_mode(tmp_path, bins):
     rng = np.random.default_rng(21)
     H = lambda b: b.hex()  # noqa: E731
     sc, want = dict(chain=H(TESTNET)), {}
-    ders = [_rand(rng, 33) for _ in range(12)] + [b"", _rand(rng, 32), _rand(rng, 34)]
+    ders = [rand(rng, 33) for _ in range(12)] + [b"", rand(rng, 32), rand(rng, 34)]
     sc["der"] = [H(d) for d in ders]
     want["der"] = []
     for d in ders:
         h = fnv(d) if len(d) == 33 else None
-        want["der"].append(H(_rev(fill(h, 64))) if h is not None and h % 3 else None)
-    data = [_rand(rng, x) for x in (0, 1, 55, 64, 300)]
+        want["der"].append(H(rev(fill(h, 64))) if h is not None and h % 3 else None)
+    data = [rand(rng, x) for x in (0, 1, 55, 64, 300)]
     sc["sha"], want["sha"] = [H(d) for d in data], [H(fill(fnv(d), 32)) for d in data]
 
     def verdict(kind, msg, key, sig):
         return fnv(bytes([kind]) + msg + key + sig) % 3 == 1
 
-    items = [(_rand(rng, 32), _rand(rng, 64), _rand(rng, 64)) for _ in range(24)]
+    items = [(rand(rng, 32), rand(rng, 64), rand(rng, 64)) for _ in range(24)]
     sc["signed"] = [(H(m), H(s), H(k)) for m, s, k in items]
-    want["signed"] = [verdict(1, m, _rev(k), _rev(s)) for m, s, k in items]
-    nid = [(m, s, _rand(rng, 33)) for m, s, _ in items]
+    want["signed"] = [verdict(1, m, rev(k), rev(s)) for m, s, k in items]
+    nid = [(m, s, rand(rng, 33)) for m, s, _ in items]
     sc["nodeid"] = [(H(m), H(s), H(k)) for m, s, k in nid]
-    want["nodeid"] = [verdict(0, m, k, _rev(s)) for m, s, k in nid]
+    want["nodeid"] = [verdict(0, m, k, rev(s)) for m, s, k in nid]
     sc["schnorr"] = [(H(m), H(s), H(k)) for m, s, k in items]
-    want["schnorr"] = [verdict(2, m, _rev(k)[:32], s) for m, s, k in items]
-    key = _rand(rng, 64)
+    want["schnorr"] = [verdict(2, m, rev(k)[:32], s) for m, s, k in items]
+    key = rand(rng, 64)
     sc["batch"], want["batch"] = [], []
     for n in (1, 9):
-        hs, ss = [_rand(rng, 32) for _ in range(n)], [_rand(rng, 64) for _ in range(n)]
+        hs, ss = [rand(rng, 32) for _ in range(n)], [rand(rng, 64) for _ in range(n)]
         sc["batch"].append((H(b"".join(hs)), H(b"".join(s + le(1, 4) for s in ss)), H(key), n))
-        want["batch"].append([verdict(1, h, _rev(key), _rev(s)) for h, s in zip(hs, ss)])
+        want["batch"].append([verdict(1, h, rev(key), rev(s)) for h, s in zip(hs, ss)])
     # check_tx_sig: transactions of 1-3 inputs and 1-4 outputs, every sighash type the gate passes or refuses
     sc["tx"], want["tx"] = [], []
     for it in range(30):
         nin, nout = int(rng.integers(1, 4)), int(rng.integers(1, 5))
-        ins = [(_rand(rng, 32), int(rng.integers(0, 5)), int(rng.integers(0, 2**32))) for _ in range(nin)]
-        outs = [(int(rng.integers(0, 2**40)), _rand(rng, int(rng.choice([0, 22, 34, 300])))) for _ in range(nout)]
-        inp, script = int(rng.integers(0, nin)), _rand(rng, int(rng.choice([1, 71, 300])))
+        ins = [(rand(rng, 32), int(rng.integers(0, 5)), int(rng.integers(0, 2**32))) for _ in range(nin)]
+        outs = [(int(rng.integers(0, 2**40)), rand(rng, int(rng.choice([0, 22, 34, 300])))) for _ in range(nout)]
+        inp, script = int(rng.integers(0, nin)), rand(rng, int(rng.choice([1, 71, 300])))
         sht, witness = int(rng.choice([1, 1, 0x83, 0x83, 2, 3])), bool(rng.random() < 0.8)
         c = dict(version=2, locktime=int(rng.integers(0, 2**31)), ins=[(H(t), i, s) for t, i, s in ins],
                  outs=[(sat, H(s)) for sat, s in outs], input=inp, script=H(script), witness=witness,
-                 amount=int(rng.integers(0, 2**45)), key=H(_rand(rng, 64)), sig=H(_rand(rng, 64) + le(sht, 4)))
+                 amount=int(rng.integers(0, 2**45)), key=H(rand(rng, 64)), sig=H(rand(rng, 64) + le(sht, 4)))
         sc["tx"].append(c)
         if sht != 1 and not (witness and sht == 0x83):
             want["tx"].append(False)
@@ -539,49 +372,48 @@ def test_dropin_client_mode(tmp_path, bins):
         f = dict(version=2, locktime=c["locktime"], sequence=ins[inp][2], sighash_type=sht, prev_txid=ins[inp][0],
                  prev_index=ins[inp][1], flags=flags | (2 if nin > 1 else 0), input_amount=c["amount"], output_amount=0)
         sig = bytes.fromhex(c["sig"])[:64]
-        want["tx"].append(tx_hash(1, _rev(bytes.fromhex(c["key"])), _rev(sig), f, [script, o, pv, sq]) % 3 == 1)
+        want["tx"].append(tx_hash(1, rev(bytes.fromhex(c["key"])), rev(sig), f, [script, o, pv, sq]) % 3 == 1)
     # check_tx_sigs_bip143_batch on sv_tx records (tests/txsig.py), the sighash type of each signature gated
     txs, blob = txsig.make_multi_txs(rng, 12)
     shts = [int(x) for x in rng.choice([1, 0x83, 2, 3], size=12)]
-    sigs = [_rand(rng, 64) for _ in range(12)]
+    sigs = [rand(rng, 64) for _ in range(12)]
     sc["bip143"] = [(H(bytes(txs)), H(blob), H(key), H(b"".join(s + le(t, 4) for s, t in zip(sigs, shts))), 12)]
     want["bip143"] = [[]]
     for t, s, sht in zip(txs, sigs, shts):
         f = {k: getattr(t, k) for k in txsig.U32_FIELDS + ["input_amount", "output_amount"]}
         f["prev_txid"], f["sighash_type"] = bytes(t.prev_txid), sht
-        ok = tx_hash(1, _rev(key), _rev(s), f, list(txsig.spans(t, blob))) % 3 == 1
+        ok = tx_hash(1, rev(key), rev(s), f, list(txsig.spans(t, blob))) % 3 == 1
         want["bip143"][0].append(ok and sht in (1, 0x83))
     # bolt12_check_signature: the fields serialised as one TLV stream, sent under the call's tag
     sc["bolt12"], want["bolt12"] = [], []
     for it in range(12):
-        fields = [(int(t), _rand(rng, int(rng.choice([0, 3, 40, 300])))) for t in sorted(rng.choice(70000, 4, replace=False))]
+        fields = [(int(t), rand(rng, int(rng.choice([0, 3, 40, 300])))) for t in sorted(rng.choice(70000, 4, replace=False))]
         mn, fn = TAGS[it % 3]
-        k, s = _rand(rng, 64), _rand(rng, 64)
+        k, s = rand(rng, 64), rand(rng, 64)
         sc["bolt12"].append(([(t, H(v)) for t, v in fields], mn.decode(), fn.decode(), H(k), H(s)))
         stream = b"".join(_bigsize(t) + _bigsize(len(v)) + v for t, v in fields)
-        want["bolt12"].append(fnv(mn + b"\0" + fn + b"\0" + stream + _rev(k)[:32] + s) % 3 - 1 == 1)
+        want["bolt12"].append(fnv(mn + b"\0" + fn + b"\0" + stream + rev(k)[:32] + s) % 3 - 1 == 1)
     # the typed gossip entry points (a message of another type is -1 whatever the daemon says) and bursts
     sc["gossip"], want["gossip"] = [], []
     for fn, typ in (("sigcheck_channel_announcement_batch", 256), ("sigcheck_node_announcement_batch", 257),
                     ("sigcheck_channel_update_batch", 258)):
-        msgs = [(t if rng.random() < 0.8 else 259).to_bytes(2, "big") + _rand(rng, int(rng.integers(0, 200)))
+        msgs = [(t if rng.random() < 0.8 else 259).to_bytes(2, "big") + rand(rng, int(rng.integers(0, 200)))
                 for t in [typ] * 15] + [b"\x01"]
-        signers = _rand(rng, 33 * len(msgs)) if typ == 258 else bytes(33 * len(msgs))
+        signers = rand(rng, 33 * len(msgs)) if typ == 258 else bytes(33 * len(msgs))
         sc["gossip"].append((fn, [H(m) for m in msgs], H(signers)))
         want["gossip"].append([fnv(m + signers[33 * i:33 * i + 33]) % 6 - 1 if m[:2] == typ.to_bytes(2, "big") else -1
                                for i, m in enumerate(msgs)])
     sc["burst"], want["burst"] = [], []
     for with_kinds in (False, True):
-        msgs = [_rand(rng, int(rng.integers(2, 200))) for _ in range(20)]
+        msgs = [rand(rng, int(rng.integers(2, 200))) for _ in range(20)]
         kinds = bytes(int(x) for x in rng.integers(0, 3, size=20)) if with_kinds else bytes(20)
-        signers = _rand(rng, 33 * 20) if with_kinds else bytes(33 * 20)
+        signers = rand(rng, 33 * 20) if with_kinds else bytes(33 * 20)
         sc["burst"].append(([H(m) for m in msgs], H(kinds) if with_kinds else None, H(signers) if with_kinds else None))
         want["burst"].append([fnv(TESTNET + m + kinds[i:i + 1] + signers[33 * i:33 * i + 33]) % 10 - 4
                               for i, m in enumerate(msgs)])
     path = tmp_path / "scenario.json"
     path.write_text(json.dumps(sc))
-    ctx, log = _start(tmp_path, bins["daemon"])
-    with ctx as sock:
+    with sigverifyd_daemon.running(tmp_path, bins["daemon"], sf.env(tmp_path)) as sock:
         env = dict(os.environ, PYTHONPATH=ROOT + os.pathsep + os.environ.get("PYTHONPATH", ""), CLN_SIGVERIFYD_SOCKET=sock)
         r = subprocess.run([sys.executable, "-c", CLIENT, str(path), bins["lib"]], env=env, cwd=str(tmp_path),
                            capture_output=True, text=True, timeout=300)

@@ -1,9 +1,8 @@
-"""CPU: the sigverifyd_fee_grind message (onchaind's HTLC fee grind through the verifier subdaemon).  The generated C
-and Python codecs agree; the daemon, built against the fake engine (tests/host_emul/fake_engine.c), routes each grind to
+"""CPU: the sigverifyd_fee_grind message (onchaind's HTLC fee grind through the verifier subdaemon).  The Python codec
+reads both messages back; the daemon, built against the fake engine (tests/host_emul/fake_engine.c), routes each grind to
 one sv_grind_tx_fee_host call with the request's own bytes, answers in request order among other traffic, and refuses
 malformed requests; the drop-in's check_tx_sig_grind_fee in client mode sends the record check_tx_sig builds.  The fake's
 grind is tests/host_emul/fake_engine_grind.c, linked beside the fake engine; a daemon linked without it refuses grinds."""
-import ctypes
 import json
 import os
 import subprocess
@@ -12,36 +11,27 @@ import sys
 import numpy as np
 import pytest
 
-from lightning_b200 import build
 from lightning_b200 import sigverifyd_wire as W
 from tests import sigverifyd_daemon
-from tests.test_sigverifyd_fake_engine import (FAKE, _calls, _gcc, _rand, _rev, _roundtrip, _start, fnv, le, patched, short,
-                                               tx_req, verify_req)
+from tests import sigverifyd_fake as sf
+from tests.sigverifyd_fake import FAKE_GRIND, KS, calls, fnv, le, patched, rand, rev, roundtrip, short, tx_req, verify_req
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-KS = {0: 33, 1: 64}
-FAKE_GRIND = os.path.join(ROOT, "tests", "host_emul", "fake_engine_grind.c")
 
 
 @pytest.fixture(scope="module")
 def bins(tmp_path_factory):
     """the daemon and the client-mode drop-in library on the fake engine with its grind, and a daemon without the grind"""
     d = tmp_path_factory.mktemp("fake_grind")
-    out = dict(daemon=str(d / "cln_sigverifyd"), lib=str(d / "libcln_dropin_fake.so"), bare=str(d / "cln_sigverifyd_bare"))
-    daemon_src = os.path.join(build.CSRC, "sigverifyd.c")
-    _gcc(build.DAEMON_CFLAGS + [daemon_src, FAKE, FAKE_GRIND, "-o", out["daemon"]])
-    _gcc(build.DAEMON_CFLAGS + [daemon_src, FAKE, "-o", out["bare"]])
-    _gcc(build.DROPIN_CFLAGS + ["-shared", "-DFAKE_ENGINE_NO_CONTEXT", os.path.join(build.CSRC, "cln_dropin.c"), FAKE,
-                                FAKE_GRIND, "-o", out["lib"]])
-    return out
+    return dict(daemon=sf.daemon(d / "cln_sigverifyd", FAKE_GRIND), lib=sf.dropin(d / "libcln_dropin_fake.so", FAKE_GRIND),
+                bare=sf.daemon(d / "cln_sigverifyd_bare"))
 
 
 @pytest.fixture
 def fake(tmp_path, bins):
     """a daemon on the fake engine with its grind, and the engine's call log"""
-    ctx, log = _start(tmp_path, bins["daemon"])
-    with ctx as sock:
-        yield sock, log
+    with sigverifyd_daemon.running(tmp_path, bins["daemon"], sf.env(tmp_path)) as sock:
+        yield sock, tmp_path / "engine.log"
 
 
 def grind_answer(kind, key, sig, f, script, out_script, weight, lo, hi):
@@ -57,9 +47,9 @@ def grind_answer(kind, key, sig, f, script, out_script, weight, lo, hi):
 
 def grind_req(rng, rid, kind, script_len=140, out_len=34, weight=663, lo=253, hi=125000):
     f = dict(version=2, locktime=int(rng.integers(0, 2**31)), sequence=int(rng.integers(0, 2)),
-             sighash_type=int(rng.choice([1, 0x83])), prev_index=int(rng.integers(0, 600)), prev_txid=_rand(rng, 32),
+             sighash_type=int(rng.choice([1, 0x83])), prev_index=int(rng.integers(0, 600)), prev_txid=rand(rng, 32),
              input_amount=int(rng.integers(0, 2**40)))
-    key, sig, script, out_script = _rand(rng, KS[kind]), _rand(rng, 64), _rand(rng, script_len), _rand(rng, out_len)
+    key, sig, script, out_script = rand(rng, KS[kind]), rand(rng, 64), rand(rng, script_len), rand(rng, out_len)
     frame = W.encode("sigverifyd_fee_grind", req_id=rid, kind=kind, keylen=len(key), key=key, script_len=len(script),
                      script=script, out_script_len=len(out_script), out_script=out_script, sig=sig, weight=weight,
                      min_feerate=lo, max_feerate=hi, **f)
@@ -87,10 +77,10 @@ def test_daemon_routes_each_grind_to_one_engine_call(fake):
     reqs = [grind_req(rng, 1, 0), tx_req(rng, 2, 1, [(10, 20, 0, 0)], 0), grind_req(rng, 3, 1, 71, 22, 703, 0, 0xFFFFFFFF),
             verify_req(rng, 4, 0, 2), grind_req(rng, 5, 0, 0, 0, 0, 9, 8), grind_req(rng, 6, 1, 300, 34, 1, 10, 10)]
     c = sigverifyd_daemon.connect(sock)
-    _roundtrip(c, reqs)
+    roundtrip(c, reqs)
     c.close()
-    calls = [x for x in _calls(log) if x[0] == "sv_grind_tx_fee_host"]
-    assert calls == [("sv_grind_tx_fee_host", 0, 1, 174), ("sv_grind_tx_fee_host", 0, 1, 0),
+    grinds = [x for x in calls(log) if x[0] == "sv_grind_tx_fee_host"]
+    assert grinds == [("sv_grind_tx_fee_host", 0, 1, 174), ("sv_grind_tx_fee_host", 0, 1, 0),
                      ("sv_grind_tx_fee_host", 1, 1, 93), ("sv_grind_tx_fee_host", 1, 1, 334)]
     assert sum(r[1][1]["found"] for r in reqs[0::2] if r[1][0] == "sigverifyd_fee_grind_reply") >= 1
 
@@ -109,23 +99,23 @@ def test_malformed_grinds_are_refused(fake):
         c.sendall(b)
         got = W.read_msg(c)
         assert got[0] == "sigverifyd_error" and got[1]["code"] == 1 and got[1]["req_id"] in (9, 0), got
-    _roundtrip(c, [(frame, want)])
+    roundtrip(c, [(frame, want)])
     c.close()
-    assert [x[0] for x in _calls(log)] == ["sv_grind_tx_fee_host"]
+    assert [x[0] for x in calls(log)] == ["sv_grind_tx_fee_host"]
 
 
 def test_engine_without_grind_refuses_grinds(tmp_path, bins):
     """a daemon linked against an engine without sv_grind_tx_fee_host answers a grind with error 1 and keeps serving"""
     rng = np.random.default_rng(5)
-    ctx, log = _start(tmp_path, bins["bare"])
-    with ctx as sock:
+    log = tmp_path / "engine.log"
+    with sigverifyd_daemon.running(tmp_path, bins["bare"], sf.env(tmp_path)) as sock:
         c = sigverifyd_daemon.connect(sock)
         frame, _ = grind_req(rng, 11, 1)
         c.sendall(frame)
         assert W.read_msg(c) == ("sigverifyd_error", dict(req_id=11, code=1))
-        _roundtrip(c, [verify_req(rng, 12, 0, 2)])
+        roundtrip(c, [verify_req(rng, 12, 0, 2)])
         c.close()
-    assert [x[0] for x in _calls(log)] == ["sv_verify_host"]
+    assert [x[0] for x in calls(log)] == ["sv_verify_host"]
 
 
 CLIENT = r"""
@@ -173,11 +163,11 @@ def test_dropin_client_mode(tmp_path, bins):
     cases, want = [], []
     for i in range(16):
         sht = int(rng.choice([1, 0x83, 2, 3, 0x81]))
-        c = dict(txid=_rand(rng, 32).hex(), index=int(rng.integers(0, 9)), sequence=int(rng.integers(0, 2)),
+        c = dict(txid=rand(rng, 32).hex(), index=int(rng.integers(0, 9)), sequence=int(rng.integers(0, 2)),
                  locktime=int(rng.integers(0, 2**31)), out_amount=int(rng.integers(0, 2**40)),
-                 out_script=_rand(rng, int(rng.choice([0, 22, 34]))).hex(), amount=int(rng.integers(0, 2**40)),
-                 wscript=_rand(rng, int(rng.choice([1, 140]))).hex(), key=_rand(rng, 64).hex(),
-                 sig=(_rand(rng, 64) + le(sht, 4)).hex(), weight=int(rng.choice([0, 663, 703])),
+                 out_script=rand(rng, int(rng.choice([0, 22, 34]))).hex(), amount=int(rng.integers(0, 2**40)),
+                 wscript=rand(rng, int(rng.choice([1, 140]))).hex(), key=rand(rng, 64).hex(),
+                 sig=(rand(rng, 64) + le(sht, 4)).hex(), weight=int(rng.choice([0, 663, 703])),
                  lo=int(rng.integers(0, 1000)), hi=int(rng.integers(0, 200000)))
         cases.append(c)
         if sht not in (1, 0x83):
@@ -185,13 +175,12 @@ def test_dropin_client_mode(tmp_path, bins):
             continue
         f = dict(version=2, locktime=c["locktime"], sequence=c["sequence"], sighash_type=sht, prev_txid=bytes.fromhex(c["txid"]),
                  prev_index=c["index"], input_amount=c["amount"])
-        found, rate, fee = grind_answer(1, _rev(bytes.fromhex(c["key"])), _rev(bytes.fromhex(c["sig"])[:64]), f,
+        found, rate, fee = grind_answer(1, rev(bytes.fromhex(c["key"])), rev(bytes.fromhex(c["sig"])[:64]), f,
                                         bytes.fromhex(c["wscript"]), bytes.fromhex(c["out_script"]), c["weight"], c["lo"], c["hi"])
         want.append([rate, fee] if found else None)
     path = tmp_path / "grind.json"
     path.write_text(json.dumps(cases))
-    ctx, log = _start(tmp_path, bins["daemon"])
-    with ctx as sock:
+    with sigverifyd_daemon.running(tmp_path, bins["daemon"], sf.env(tmp_path)) as sock:
         env = dict(os.environ, PYTHONPATH=ROOT + os.pathsep + os.environ.get("PYTHONPATH", ""), CLN_SIGVERIFYD_SOCKET=sock)
         r = subprocess.run([sys.executable, "-c", CLIENT, str(path), bins["lib"]], env=env, cwd=str(tmp_path),
                            capture_output=True, text=True, timeout=300)

@@ -1,8 +1,7 @@
 """CPU: repairing a gossip_store FILE in place — sv_repair_gossip_store_fd and sv_gossip_prune_cut
 (lightning_b200/csrc/gossip_store_fd.c), the verifier subdaemon's sigverifyd_gossip_store_repair (the store's fd passed over
 the socket with SCM_RIGHTS) and the drop-in's gossip_store_repair in both modes — built with gcc against the fake prune
-(tests/host_emul/fake_engine_prune.c) whose walk stops where gossmap's does on a torn store; the builds, the client process
-and the fake's Python statement are tests/test_sigverifyd_prune_fake.py's.  Checked: the cut against a Python statement of
+(tests/host_emul/fake_engine_prune.c) whose walk stops where gossmap's does on a torn store.  Checked: the cut against a Python statement of
 the tail rule on every stop kind; the file ends as the fake's pruned store cut there, with the fake's summary and new_len,
 in-process, through a daemon on a socket and through `--fd N`; a client-mode process never creates a context; every
 refused file or frame is answered without the daemon exiting, leaves the file as it was and the daemon with no descriptor
@@ -17,49 +16,21 @@ import subprocess
 import time
 
 import numpy as np
+import pytest
 
 from lightning_b200 import sigverifyd_wire as W
 from lightning_b200.engine import SvGossipPruneSummary
+from tests import sigverifyd_codec as codec
+from tests import sigverifyd_daemon
+from tests import sigverifyd_fake as sf
 from tests.gossip_store import BAD_CRC, EOF, INCOMPLETE, NO_AMOUNT, PARTIAL, ST_ENDED, TRUNCATED
-from tests.test_sigverifyd_fake_engine import verify_req
-from tests.test_sigverifyd_prune_fake import (FIELDS, MAX_PRUNE_STORE, PRUNE, TESTNET, _begun, _env, _trace, _wait,
-                                              back_to, bins, case, fake_prune, make_store, nfds, prune_frame, run_client,
-                                              serve)
+from tests.sigverifyd_fake import (FIELDS, MAX_PRUNE_STORE, PRUNE, TESTNET, back_to, begun, case, cut_rule, fake_prune,
+                                   make_store, nfds, prune_frame, run_client, tail_rule, trace, verify_req, wait_trace)
 
 
-def tail_rule(stop, end_offset, length):
-    """where a repair ends a store of `length` bytes whose prune stopped at `stop` / `end_offset`, from the summary alone
-    (the first three rules of sv_repair_gossip_store_fd in include/cln_sigverify.h)"""
-    if stop in (INCOMPLETE, PARTIAL, NO_AMOUNT):
-        return min(end_offset, length)
-    if stop == EOF and end_offset < length:
-        return end_offset
-    return length
-
-
-def room_back_off(pruned, cut):
-    """the last rule: while the first live channel_announcement of pruned[:cut] has fewer than 22 bytes after it before
-    cut (no room for its amount record), the store ends at it"""
-    while True:
-        off, at = 1, cut
-        while off + 14 <= cut:
-            flags, mlen = struct.unpack(">HH", pruned[off:off + 4])
-            typ = struct.unpack(">H", pruned[off + 12:off + 14])[0]
-            if off + 12 + mlen > cut:
-                break
-            if not flags & 0x8000 and typ == 256 and off + 12 + mlen + 22 > cut:
-                at = off
-                break
-            off += 12 + mlen
-        if at == cut:
-            return cut
-        cut = at
-
-
-def cut_rule(pruned, s):
-    """sv_gossip_prune_cut: the tail rule, then the back-off when it cuts"""
-    cut = tail_rule(s["stop"], s["end_offset"], len(pruned))
-    return room_back_off(pruned, cut) if cut < len(pruned) else cut
+@pytest.fixture(scope="module")
+def bins(tmp_path_factory):
+    return sf.store_bins(tmp_path_factory.mktemp("repair_fake"))
 
 
 # ---- stores and what the fake makes of them (fake_engine_prune.c) ----------------------------------------------------
@@ -166,11 +137,11 @@ def test_file_repaired_every_way(tmp_path, bins):
     cases = lambda how: [c for k in names for c in (case(d[how] / k, op="repair"),
                                                     case(d[how] / k, want[k][2], op="repair"))]
     got = {"inproc": run_client(tmp_path, bins["inproc"], "inproc", cases("inproc"))}
-    with serve(tmp_path, bins["daemon"], _env(tmp_path)) as (proc, sock):
+    with sigverifyd_daemon.running(tmp_path, bins["daemon"], sf.env(tmp_path)) as sock:
         got["sock"] = run_client(tmp_path, bins["client"], "sock:" + sock, cases("sock"))
-        assert proc.poll() is None
+        assert sock.proc.poll() is None
     parent, child = socket.socketpair()
-    dm = subprocess.Popen([bins["daemon"], "--fd", str(child.fileno()), "0"], pass_fds=(child.fileno(),), env=_env(tmp_path),
+    dm = subprocess.Popen([bins["daemon"], "--fd", str(child.fileno()), "0"], pass_fds=(child.fileno(),), env=sf.env(tmp_path),
                           stderr=subprocess.PIPE)
     child.close()
     try:
@@ -227,20 +198,19 @@ def test_refused_files(tmp_path, bins):
              case("", 10, None, kind="closed", op="repair"), case(short, 0, op="repair"), case(good, op="repair")]
     want_err = [errno.EBADF, errno.EINVAL, errno.EINVAL, errno.EINVAL, errno.EFBIG, errno.EBADF, errno.EINVAL]
     before = {f: f.read_bytes() for f in (ro, short, v1)}
-    with serve(tmp_path, bins["daemon"], _env(tmp_path)) as (proc, sock):
+    with sigverifyd_daemon.running(tmp_path, bins["daemon"], sf.env(tmp_path)) as sock:
         time.sleep(0.2)
-        base = nfds(proc)
+        base = nfds(sock.proc)
         got = run_client(tmp_path, bins["client"], "sock:" + sock, cases)
-        assert proc.poll() is None
-        assert back_to(proc, base) == base
+        assert sock.proc.poll() is None
+        assert back_to(sock.proc, base) == base
     assert [g[:2] for g in got[:-1]] == [[False, e] for e in want_err]
     out, s, cut = fake_repair(store)
     assert got[-1] == [True, 0, s, cut] and good.read_bytes() == out and cut < len(store)
     for f, b in before.items():
         assert f.read_bytes() == b, f
     assert os.path.getsize(big) == MAX_PRUNE_STORE + 4096
-    calls = [line.split() for line in (tmp_path / "engine.log").read_text().splitlines()]
-    assert [int(c[3]) for c in calls if c[0] == PRUNE] == [len(store)]
+    assert [c[3] for c in sf.calls(tmp_path / "engine.log") if c[0] == PRUNE] == [len(store)]
     good.write_bytes(store)
     local = run_client(tmp_path, bins["inproc"], "inproc", cases[:4] + cases[5:])
     assert [g[:2] for g in local[:-1]] == [[False, e] for e in want_err[:4] + want_err[5:]]
@@ -256,9 +226,9 @@ def test_refused_frames(tmp_path, bins):
     f = tmp_path / "gossip_store"
     store = torn_stores()["incomplete"]
     f.write_bytes(store)
-    with serve(tmp_path, bins["daemon"], _env(tmp_path)) as (proc, sock):
+    with sigverifyd_daemon.running(tmp_path, bins["daemon"], sf.env(tmp_path)) as sock:
         time.sleep(0.2)
-        base = nfds(proc)
+        base = nfds(sock.proc)
         c = socket.socket(socket.AF_UNIX, socket.SOCK_STREAM)
         c.settimeout(30)
         c.connect(sock)
@@ -278,7 +248,7 @@ def test_refused_frames(tmp_path, bins):
         assert name == "sigverifyd_gossip_store_repair_reply" and m["req_id"] == 3 and m["err"] == 0
         assert {k: m[k] for k in FIELDS} == s and m["new_len"] == cut
         c.close()
-        assert back_to(proc, base) == base
+        assert back_to(sock.proc, base) == base
     assert f.read_bytes() == out
 
 
@@ -292,19 +262,19 @@ def test_repair_beside_channel_checks_never_beside_a_prune(tmp_path, bins):
         f.write_bytes(s)
     fds = [os.open(f, os.O_RDWR) for f in files]
     try:
-        with serve(tmp_path, bins["daemon"], _env(tmp_path, 600)) as (proc, sock):
+        with sigverifyd_daemon.running(tmp_path, bins["daemon"], sf.env(tmp_path, {PRUNE: 600})) as sock:
             a, b, v = (socket.socket(socket.AF_UNIX, socket.SOCK_STREAM) for _ in range(3))
             for c in (a, b, v):
                 c.settimeout(30)
                 c.connect(sock)
             socket.send_fds(a, [repair_frame(1, len(stores[0]))], [fds[0]])
-            _wait(_begun(tmp_path, PRUNE))
+            wait_trace(tmp_path, begun(PRUNE))
             socket.send_fds(b, [prune_frame(2, len(stores[1]))], [fds[1]])
             for k in range(3):
                 f, want = verify_req(rng, 10 + k, 0, 3)
                 v.sendall(f)
                 assert W.read_msg(v) == want
-            assert not any(e[:2] == ("end", PRUNE) for e in _trace(tmp_path))
+            assert not any(e[:2] == ("end", PRUNE) for e in trace(tmp_path))
             name, m = W.read_msg(a)
             assert name == "sigverifyd_gossip_store_repair_reply" and m["err"] == 0 and m["new_len"] == fake_repair(stores[0])[2]
             name, m = W.read_msg(b)
@@ -314,48 +284,29 @@ def test_repair_beside_channel_checks_never_beside_a_prune(tmp_path, bins):
     finally:
         for fd in fds:
             os.close(fd)
-    assert [e[0] for e in _trace(tmp_path) if e[1] == PRUNE] == ["begin", "end", "begin", "end"]
+    assert [e[0] for e in trace(tmp_path) if e[1] == PRUNE] == ["begin", "end", "begin", "end"]
     assert files[0].read_bytes() == fake_repair(stores[0])[0]
     assert files[1].read_bytes() == fake_prune(stores[1])[0]
 
 
 # ---- the codec -------------------------------------------------------------------------------------------------------
-def test_codec_round_trip(bins):
+@pytest.fixture(scope="module")
+def shim(tmp_path_factory):
+    return codec.build_shim(tmp_path_factory.mktemp("wire"))
+
+
+def test_codec_round_trip(shim):
     """the C codec (sigverifyd_wiregen.h) and the Python one (sigverifyd_wire.py) give the same bytes for both messages and
-    read each other's; a short or long message, or another type, is refused"""
-    shim = ctypes.CDLL(bins["shim"])
-    vp, sz = ctypes.c_void_p, ctypes.c_size_t
-    shim.shim_towire_repair.restype = sz
-    shim.shim_towire_repair.argtypes = [vp, sz, ctypes.c_uint64, ctypes.c_uint8, vp, ctypes.c_uint64]
-    shim.shim_fromwire_repair.argtypes = [vp, sz, vp, vp]
-    shim.shim_towire_repair_reply.restype = sz
-    shim.shim_towire_repair_reply.argtypes = [vp, sz, vp]
-    shim.shim_fromwire_repair_reply.argtypes = [vp, sz, vp]
+    read each other's; a short or long message, or another type, is refused (tests/sigverifyd_codec.py)"""
     rng = np.random.default_rng(8)
     for _ in range(50):
         rid, has, ln = int(rng.integers(0, 2**63)), int(rng.integers(0, 2)), int(rng.integers(0, 2**64, dtype=np.uint64))
         chain = rng.integers(0, 256, size=32, dtype=np.uint8).tobytes()
-        body = W.encode("sigverifyd_gossip_store_repair", req_id=rid, has_chain=has, chain_hash=chain, len=ln)[4:]
-        assert len(body) == 2 + 8 + 1 + 32 + 8 and body[:2] == (3011).to_bytes(2, "big")
-        out = (ctypes.c_uint8 * 64)()
-        n = shim.shim_towire_repair(out, 64, rid, has, (ctypes.c_uint8 * 32).from_buffer_copy(chain), ln)
-        assert bytes(out[:n]) == body
-        u, co = (ctypes.c_uint64 * 3)(), ctypes.c_size_t()
-        assert shim.shim_fromwire_repair(body, len(body), u, ctypes.byref(co)) == 1
-        assert list(u) == [rid, has, ln] and body[co.value:co.value + 32] == chain
-        assert W.decode(body) == ("sigverifyd_gossip_store_repair", dict(req_id=rid, has_chain=has, chain_hash=chain, len=ln))
-        for bad in (body[:-1], body + b"\0", (3010).to_bytes(2, "big") + body[2:]):
-            assert shim.shim_fromwire_repair(bad, len(bad), u, ctypes.byref(co)) == 0
+        req = dict(req_id=rid, has_chain=has, chain_hash=chain, len=ln)
         vals = [rid, int(rng.integers(0, 2**32)), int(rng.integers(0, 2**32)), int(rng.integers(0, 2**32))] + [
             int(x) for x in rng.integers(0, 2**64, size=13, dtype=np.uint64)]
-        names = ["req_id", "err"] + FIELDS + ["new_len"]
-        rb = W.encode("sigverifyd_gossip_store_repair_reply", **dict(zip(names, vals)))[4:]
-        assert len(rb) == 2 + 8 + 3 * 4 + 13 * 8 and rb[:2] == (3111).to_bytes(2, "big")
-        out = (ctypes.c_uint8 * 200)()
-        n = shim.shim_towire_repair_reply(out, 200, (ctypes.c_uint64 * 17)(*vals))
-        assert bytes(out[:n]) == rb
-        v = (ctypes.c_uint64 * 17)()
-        assert shim.shim_fromwire_repair_reply(rb, len(rb), v) == 1 and list(v) == vals
-        assert W.decode(rb) == ("sigverifyd_gossip_store_repair_reply", dict(zip(names, vals)))
-        for bad in (rb[:-1], rb + b"\0", (3110).to_bytes(2, "big") + rb[2:]):
-            assert shim.shim_fromwire_repair_reply(bad, len(bad), v) == 0
+        rep = dict(zip(["req_id", "err"] + FIELDS + ["new_len"], vals))
+        for name, m in (("sigverifyd_gossip_store_repair", req), ("sigverifyd_gossip_store_repair_reply", rep)):
+            codec.agree(shim, name, m)
+            codec.refused(shim, name, m)
+            codec.wrong_type_refused(shim, name, m)

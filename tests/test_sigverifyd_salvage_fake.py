@@ -8,104 +8,28 @@ in-process, through a daemon on a socket and through `--fd N`; a second call men
 creates a context; every refused file or frame is answered without the daemon exiting and leaves the file as it was; a
 salvage runs on the gossip worker beside channel checks and never beside a prune; the reply's codec."""
 import errno
-import json
 import os
 import socket
 import subprocess
-import sys
 import time
 
 import numpy as np
 import pytest
 
-from lightning_b200 import build
 from lightning_b200 import sigverifyd_wire as W
 from tests import gossip_store_salvage as sv
-from tests.test_gossip_store_host import load_fixture
-from tests.test_gossip_store_salvage_host import damage_classes, with_uuid
-from tests.test_sigverifyd_fake_engine import verify_req
-from tests.test_sigverifyd_prune_fake import (FIELDS, HE, MAX_PRUNE_STORE, PRUNE, ROOT, STORE_FD, TESTNET, _begun, _env,
-                                              _trace, _wait, back_to, fake_prune, make_store, nfds, prune_frame, serve)
-from tests.test_sigverifyd_repair_fake import cut_rule
-
-SALVAGE_FD = os.path.join(build.CSRC, "gossip_salvage_fd.c")
-
-
-def _run(args):
-    r = subprocess.run(args, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
+from tests import sigverifyd_daemon
+from tests import sigverifyd_fake as sf
+from tests.gossip_store import load_fixture
+from tests.gossip_store_salvage import damage_classes, with_uuid
+from tests.sigverifyd_fake import (FIELDS, MAX_PRUNE_STORE, PRUNE, TESTNET, back_to, begun, cut_rule, fake_prune, make_store,
+                                   nfds, prune_frame, run_client, trace, verify_req, wait_trace)
+from tests.sigverifyd_fake import salvage_case as case
 
 
 @pytest.fixture(scope="module")
 def bins(tmp_path_factory):
-    d = tmp_path_factory.mktemp("salvage_fake")
-    salv_o = str(d / "fake_engine_salvage.o")
-    _run(["g++", "-O2", "-std=c++17", "-fPIC", "-Wall", "-Wno-unused-function", "-c",
-          os.path.join(HE, "fake_engine_salvage.cpp"), "-o", salv_o])
-    out = dict(daemon=str(d / "cln_sigverifyd"), inproc=str(d / "libdropin_inproc.so"), client=str(d / "libdropin_client.so"))
-    engine = [os.path.join(HE, "fake_engine_prune.c"), STORE_FD, SALVAGE_FD, salv_o, "-lstdc++"]
-    _run(["gcc"] + build.DAEMON_CFLAGS + [os.path.join(build.CSRC, "sigverifyd.c"), os.path.join(HE, "fake_engine_timed.c")] +
-         engine + ["-o", out["daemon"]])
-    dropin = ["gcc"] + build.DROPIN_CFLAGS + ["-shared", os.path.join(build.CSRC, "cln_dropin.c"),
-                                              os.path.join(HE, "fake_engine.c")] + engine
-    _run(dropin + ["-o", out["inproc"]])
-    _run(dropin + ["-DFAKE_ENGINE_NO_CONTEXT", "-o", out["client"]])  # its sv_create aborts
-    return out
-
-
-CLIENT = r"""
-import ctypes, json, os, sys
-from lightning_b200.engine import SvGossipPruneSummary, SvGossipSalvageSummary
-lib = ctypes.CDLL(sys.argv[1], use_errno=True)
-lib.gossip_store_salvage.restype = ctypes.c_bool
-lib.gossip_store_salvage.argtypes = [ctypes.c_int, ctypes.c_uint64, ctypes.c_void_p, ctypes.POINTER(SvGossipPruneSummary),
-                                     ctypes.POINTER(SvGossipSalvageSummary), ctypes.POINTER(ctypes.c_uint64)]
-lib.cln_sigverify_connect.argtypes = [ctypes.c_char_p]
-mode = sys.argv[2]
-if mode.startswith("sock:"):
-    assert lib.cln_sigverify_connect(mode[5:].encode()) == 0
-elif mode.startswith("fd:"):
-    assert lib.cln_sigverify_connect_fd(int(mode[3:])) == 0
-out = []
-for c in json.load(open(sys.argv[3])):
-    if c["kind"] == "pipe":
-        fd, w = os.pipe()
-        os.write(w, bytes(64))
-    elif c["kind"] == "closed":
-        fd = os.open(os.devnull, os.O_RDONLY)
-        os.close(fd)
-    else:
-        fd = os.open(c["path"], os.O_RDWR if c["kind"] == "rw" else os.O_RDONLY)
-    s, v, n = SvGossipPruneSummary(), SvGossipSalvageSummary(), ctypes.c_uint64(12345)
-    chain = bytes.fromhex(c["chain"]) if c["chain"] else None
-    ok = lib.gossip_store_salvage(fd, c["len"], chain, ctypes.byref(s), ctypes.byref(v), ctypes.byref(n))
-    e = ctypes.get_errno()
-    if c["kind"] != "closed":
-        os.close(fd)
-    if c["kind"] == "pipe":
-        os.close(w)
-    out.append([ok, 0 if ok else e, {f: getattr(s, f) for f, _ in s._fields_} if ok else None,
-                {f: getattr(v, f) for f, _ in v._fields_} if ok else None, n.value if ok else None])
-print(json.dumps(out))
-"""
-
-
-def run_client(tmp_path, lib, mode, cases, pass_fds=(), check=True):
-    """each case's [ok, errno, repair summary, salvage summary, new_len] from a process of its own"""
-    path = tmp_path / ("cases%d.json" % time.monotonic_ns())
-    path.write_text(json.dumps(cases))
-    env = dict(os.environ, PYTHONPATH=ROOT + os.pathsep + os.environ.get("PYTHONPATH", ""))
-    r = subprocess.run([sys.executable, "-c", CLIENT, lib, mode, str(path)], env=env, capture_output=True, text=True,
-                       timeout=300, pass_fds=pass_fds)
-    if check:
-        assert r.returncode == 0, r.stderr[-3000:]
-        return json.loads(r.stdout)
-    return r
-
-
-def case(path, length=None, chain=TESTNET, kind="rw"):
-    return dict(kind=kind, path=str(path), len=os.path.getsize(path) if length is None else length,
-                chain=chain.hex() if chain else None)
+    return sf.store_bins(tmp_path_factory.mktemp("salvage_fake"), salvage=True)
 
 
 def salvage_frame(rid, length, chain=TESTNET):
@@ -150,11 +74,11 @@ def test_file_salvaged_every_way(tmp_path, bins):
             (d[how] / k).write_bytes(st[k])
     cases = lambda how: [c for k in names for c in (case(d[how] / k), case(d[how] / k, want[k][3]))]
     got = {"inproc": run_client(tmp_path, bins["inproc"], "inproc", cases("inproc"))}
-    with serve(tmp_path, bins["daemon"], _env(tmp_path)) as (proc, sock):
+    with sigverifyd_daemon.running(tmp_path, bins["daemon"], sf.env(tmp_path)) as sock:
         got["sock"] = run_client(tmp_path, bins["client"], "sock:" + sock, cases("sock"))
-        assert proc.poll() is None
+        assert sock.proc.poll() is None
     parent, child = socket.socketpair()
-    dm = subprocess.Popen([bins["daemon"], "--fd", str(child.fileno()), "0"], pass_fds=(child.fileno(),), env=_env(tmp_path),
+    dm = subprocess.Popen([bins["daemon"], "--fd", str(child.fileno()), "0"], pass_fds=(child.fileno(),), env=sf.env(tmp_path),
                           stderr=subprocess.PIPE)
     child.close()
     try:
@@ -199,12 +123,12 @@ def test_refused_files(tmp_path, bins):
              case("", 10, None, kind="closed"), case(short, 0), case(good)]
     want_err = [errno.EBADF, errno.EINVAL, errno.EINVAL, errno.EINVAL, errno.EFBIG, errno.EBADF, errno.EINVAL]
     before = {f: f.read_bytes() for f in (ro, short, v1)}
-    with serve(tmp_path, bins["daemon"], _env(tmp_path)) as (proc, sock):
+    with sigverifyd_daemon.running(tmp_path, bins["daemon"], sf.env(tmp_path)) as sock:
         time.sleep(0.2)
-        base = nfds(proc)
+        base = nfds(sock.proc)
         got = run_client(tmp_path, bins["client"], "sock:" + sock, cases)
-        assert proc.poll() is None
-        assert back_to(proc, base) == base
+        assert sock.proc.poll() is None
+        assert back_to(sock.proc, base) == base
     assert [g[:2] for g in got[:-1]] == [[False, e] for e in want_err]
     out, s, v, cut = fake_salvage(store)
     assert got[-1] == [True, 0, s, v, cut] and good.read_bytes() == out
@@ -227,9 +151,9 @@ def test_frames(tmp_path, bins):
     f = tmp_path / "gossip_store"
     store = stores()["zeroed_100k"]
     f.write_bytes(store)
-    with serve(tmp_path, bins["daemon"], _env(tmp_path)) as (proc, sock):
+    with sigverifyd_daemon.running(tmp_path, bins["daemon"], sf.env(tmp_path)) as sock:
         time.sleep(0.2)
-        base = nfds(proc)
+        base = nfds(sock.proc)
         c = socket.socket(socket.AF_UNIX, socket.SOCK_STREAM)
         c.settimeout(60)
         c.connect(sock)
@@ -249,7 +173,7 @@ def test_frames(tmp_path, bins):
         assert name == "sigverifyd_gossip_store_salvage_reply" and m["req_id"] == 3 and m["err"] == 0
         assert {k: m[k] for k in FIELDS} == s and {k: m[k] for k in sv.FIELDS} == v and m["new_len"] == cut
         c.close()
-        assert back_to(proc, base) == base
+        assert back_to(sock.proc, base) == base
     assert f.read_bytes() == out
     body = W.encode("sigverifyd_gossip_store_salvage", req_id=7, has_chain=1, chain_hash=TESTNET, len=99)[4:]
     assert len(body) == 2 + 8 + 1 + 32 + 8 and body[:2] == (3012).to_bytes(2, "big")
@@ -265,19 +189,19 @@ def test_salvage_beside_channel_checks_never_beside_a_prune(tmp_path, bins):
         f.write_bytes(s)
     fds = [os.open(f, os.O_RDWR) for f in files]
     try:
-        with serve(tmp_path, bins["daemon"], _env(tmp_path, 600)) as (proc, sock):
+        with sigverifyd_daemon.running(tmp_path, bins["daemon"], sf.env(tmp_path, {PRUNE: 600})) as sock:
             a, b, vv = (socket.socket(socket.AF_UNIX, socket.SOCK_STREAM) for _ in range(3))
             for c in (a, b, vv):
                 c.settimeout(60)
                 c.connect(sock)
             socket.send_fds(a, [salvage_frame(1, len(st[0]))], [fds[0]])
-            _wait(_begun(tmp_path, PRUNE))
+            wait_trace(tmp_path, begun(PRUNE))
             socket.send_fds(b, [prune_frame(2, len(st[1]))], [fds[1]])
             for k in range(3):
                 f, want = verify_req(rng, 10 + k, 0, 3)
                 vv.sendall(f)
                 assert W.read_msg(vv) == want
-            assert not any(e[:2] == ("end", PRUNE) for e in _trace(tmp_path))
+            assert not any(e[:2] == ("end", PRUNE) for e in trace(tmp_path))
             name, m = W.read_msg(a)
             assert name == "sigverifyd_gossip_store_salvage_reply" and m["err"] == 0 and m["restored"] == 1
             name, m = W.read_msg(b)
@@ -287,6 +211,6 @@ def test_salvage_beside_channel_checks_never_beside_a_prune(tmp_path, bins):
     finally:
         for fd in fds:
             os.close(fd)
-    assert [e[0] for e in _trace(tmp_path) if e[1] == PRUNE] == ["begin", "end", "begin", "end"]
+    assert [e[0] for e in trace(tmp_path) if e[1] == PRUNE] == ["begin", "end", "begin", "end"]
     assert files[0].read_bytes() == fake_salvage(st[0])[0]
     assert files[1].read_bytes() == fake_prune(st[1])[0]

@@ -1,72 +1,48 @@
 """CPU: the verifier subdaemon's wire codec.  The C side (lightning_b200/csrc/sigverifyd_wiregen.h) and the Python side
-(lightning_b200/sigverifyd_wire.py) are both generated from sigverifyd_wire.csv by tools/gen_wire.py; they must agree byte
-for byte, and the C parser must refuse truncated, over-long and wrongly-typed messages (CLN's fromwire_* contract)."""
-import ctypes
+(lightning_b200/sigverifyd_wire.py) are both generated from sigverifyd_wire.csv by tools/gen_wire.py; the committed files
+must be what the generator makes of the CSV, and the two sides must agree byte for byte and refuse truncated, over-long
+and wrongly-typed messages (CLN's fromwire_* contract, checked by tests/sigverifyd_codec.py)."""
+import importlib.util
 import os
-import subprocess
 
 import numpy as np
 import pytest
+
+from tests import sigverifyd_codec as codec
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
-def shim():
-    subprocess.check_call(["python", os.path.join(ROOT, "tools", "gen_wire.py")], stdout=subprocess.DEVNULL)
-    so = os.path.join(ROOT, "tests", "host_emul", "libwireshim.so")
-    subprocess.check_call(["gcc", "-O2", "-shared", "-fPIC", "-Wall", "-Wextra", "-Werror", "-o", so,
-                           os.path.join(ROOT, "tests", "host_emul", "wire_shim.c")])
-    lib = ctypes.CDLL(so)
-    for f in (lib.shim_towire_verify, lib.shim_towire_verify_reply, lib.shim_towire_stats_reply):
-        f.restype = ctypes.c_size_t
-    return lib
+def shim(tmp_path_factory):
+    return codec.build_shim(tmp_path_factory.mktemp("wire"))
 
 
 def test_generated_header_is_current():
-    """the committed generated files match what the generator produces from the committed CSV"""
-    hdr = open(os.path.join(ROOT, "lightning_b200", "csrc", "sigverifyd_wiregen.h")).read()
-    py = open(os.path.join(ROOT, "lightning_b200", "sigverifyd_wire.py")).read()
-    subprocess.check_call(["python", os.path.join(ROOT, "tools", "gen_wire.py")], stdout=subprocess.DEVNULL)
-    assert hdr == open(os.path.join(ROOT, "lightning_b200", "csrc", "sigverifyd_wiregen.h")).read()
-    assert py == open(os.path.join(ROOT, "lightning_b200", "sigverifyd_wire.py")).read()
+    """the committed generated files are what tools/gen_wire.py makes of the committed CSV (nothing is written)"""
+    spec = importlib.util.spec_from_file_location("gen_wire", os.path.join(ROOT, "tools", "gen_wire.py"))
+    gen = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(gen)
+    msgs = gen.parse(gen.CSV)
+    assert open(codec.WIREGEN).read() == gen.gen_c(msgs)
+    assert open(os.path.join(ROOT, "lightning_b200", "sigverifyd_wire.py")).read() == gen.gen_py(msgs)
 
 
 def test_c_and_python_codecs_agree(shim):
-    from lightning_b200 import sigverifyd_wire as W
     rng = np.random.default_rng(1)
     for n, kind, ks in ((0, 0, 33), (1, 0, 33), (3, 1, 64), (483, 2, 32)):
         h, k, s = (rng.integers(0, 256, size=n * w, dtype=np.uint8).tobytes() for w in (32, ks, 64))
-        frame = W.encode("sigverifyd_verify", req_id=0x1122334455667788, kind=kind, n=n, hashes=h, keylen=n * ks, keys=k, sigs=s)
-        body = frame[4:]
-        assert int.from_bytes(frame[:4], "big") == len(body) and body[:2] == (3001).to_bytes(2, "big")
-        out = ctypes.create_string_buffer(len(body) + 16)
-        ln = shim.shim_towire_verify(out, len(out), ctypes.c_uint64(0x1122334455667788), kind, n, h, n * ks, k, s)
-        assert ln == len(body) and out.raw[:ln] == body
-        rid = ctypes.c_uint64()
-        f3 = (ctypes.c_uint32 * 3)()
-        offs = (ctypes.c_size_t * 3)()
-        assert shim.shim_fromwire_verify(body, len(body), ctypes.byref(rid), f3, offs) == 1
-        assert rid.value == 0x1122334455667788 and list(f3) == [kind, n, n * ks]
-        assert body[offs[0]:offs[0] + 32 * n] == h and body[offs[1]:offs[1] + ks * n] == k and body[offs[2]:offs[2] + 64 * n] == s
-        name, vals = W.decode(body)
-        assert name == "sigverifyd_verify" and vals["hashes"] == h and vals["keys"] == k and vals["sigs"] == s and vals["n"] == n
-        # fromwire refuses: truncated, one byte too long, wrong type, a count that overruns the message
-        for bad in (body[:-1], body + b"\0", (3002).to_bytes(2, "big") + body[2:], body[:11] + (n + 1).to_bytes(4, "big") + body[15:]):
-            assert shim.shim_fromwire_verify(bad, len(bad), ctypes.byref(rid), f3, offs) == 0
-    v = bytes([1, 0, 1, 1, 0])
-    out = ctypes.create_string_buffer(64)
-    ln = shim.shim_towire_verify_reply(out, 64, ctypes.c_uint64(7), 5, v)
-    assert W.decode(out.raw[:ln]) == ("sigverifyd_verify_reply", dict(req_id=7, n=5, verdicts=v))
-    assert shim.shim_towire_verify_reply(out, 10, ctypes.c_uint64(7), 5, v) == 0  # does not fit: nothing written
-    ln = shim.shim_towire_stats_reply(out, 64, ctypes.c_uint64(9), ctypes.c_uint64(10), ctypes.c_uint64(3), ctypes.c_uint64(2**40), 4)
-    assert W.decode(out.raw[:ln])[1] == dict(req_id=9, requests=10, launches=3, signatures=2**40, max_coalesced=4)
+        m = dict(req_id=0x1122334455667788, kind=kind, n=n, hashes=h, keylen=n * ks, keys=k, sigs=s)
+        codec.agree(shim, "sigverifyd_verify", m)
+        codec.refused(shim, "sigverifyd_verify", m)
+        codec.wrong_type_refused(shim, "sigverifyd_verify", m)
+    for name, m in (("sigverifyd_verify_reply", dict(req_id=7, n=5, verdicts=bytes([1, 0, 1, 1, 0]))),
+                    ("sigverifyd_stats_reply", dict(req_id=9, requests=10, launches=3, signatures=2**40, max_coalesced=4))):
+        codec.agree(shim, name, m)
+        codec.refused(shim, name, m)
     lens = [300, 5, 140]
     blob = rng.integers(0, 256, size=sum(lens), dtype=np.uint8).tobytes()
     sg = rng.integers(0, 256, size=33 * 3, dtype=np.uint8).tobytes()
-    frame = W.encode("sigverifyd_gossip", req_id=1, n=3, lens=lens, signers=sg, bloblen=len(blob), blob=blob)
-    body = frame[4:]
-    rid, f2, offs = ctypes.c_uint64(), (ctypes.c_uint32 * 2)(), (ctypes.c_size_t * 3)()
-    assert shim.shim_fromwire_gossip(body, len(body), ctypes.byref(rid), f2, offs) == 1
-    assert list(f2) == [3, len(blob)] and body[offs[2]:] == blob and body[offs[1]:offs[1] + 99] == sg
-    assert [int.from_bytes(body[offs[0] + 4 * i:offs[0] + 4 * i + 4], "big") for i in range(3)] == lens
+    m = dict(req_id=1, n=3, lens=lens, signers=sg, bloblen=len(blob), blob=blob)
+    codec.agree(shim, "sigverifyd_gossip", m)
+    codec.refused(shim, "sigverifyd_gossip", m)
