@@ -112,7 +112,7 @@ def build_host_emul(force=False):
     src = [os.path.join(ROOT, "tests", "host_emul", f) for f in ("emul.cpp", "bolt12_emul.cpp", "gossip_store_emul.cpp",
                                                              "gossip_funding_emul.cpp", "fee_grind_emul.cpp",
                                                              "gossip_salvage_emul.cpp", "bolt11_emul.cpp")]
-    srcs = _sources(CSRC, (".cuh",)) + src
+    srcs = _sources(CSRC, (".cuh",)) + src + [os.path.join(ROOT, "tests", "host_emul", "ge_trace.h")]
     if not force and _newer(EMUL, srcs):
         return EMUL
     cmd = HOST_EMUL_CXX + ["-o", EMUL] + src

@@ -70,6 +70,27 @@ def invoices(fx):
     return [blob[o:o + n] for o, n in zip(fx["off"].tolist(), fx["len"].tolist())]
 
 
+def signature(s):
+    """(r, s, recovery id) of an invoice from its last 104 data words"""
+    data = s.decode().lower().rsplit("1", 1)[1][:-6]
+    v = 0
+    for c in data[-104:]:
+        v = (v << 5) | CHARSET.index(c)
+    return v >> 264, (v >> 8) & (2**256 - 1), v & 255
+
+
+def rec_scalars(fx, i):
+    """(u1, u2, d) of the recovery of a rec_* item (make_bolt11.py): u1 = -e / r, u2 = +-s / r and d, the discrete log of
+    E = lift_x(r), from the nonce k of R = k G stored as rec_k (d = k when R.y, the recovery id's bit 0, is even)"""
+    from tests.ecc import N
+    r, s, recid = signature(invoices(fx)[i])
+    e = int.from_bytes(fx["hash"][i].tobytes(), "big") % N
+    k = int.from_bytes(fx["rec_k"][i].tobytes(), "big")
+    assert k, i
+    rinv = pow(r, -1, N)
+    return -e * rinv % N, (-s if recid & 1 else s) * rinv % N, (N - k if recid & 1 else k)
+
+
 def oracle():
     """The reference's BOLT11 decoder, recorded on the module's `cln` tape (tests/oracle_replay.py)."""
     o = oracle_replay.Oracle("cln")

@@ -19,6 +19,16 @@ The corpus (seeded, so a re-run gives the same file):
   flip          one 5-bit word of one invoice changed in every region (hrp, timestamp, tag, length, data, signature),
                 checksum recomputed, and one raw character flipped in every position (checksum not recomputed)
   trunc         every truncation of one invoice: raw prefixes, and word prefixes with the checksum recomputed
+  rec_window    invoices without `n` whose recovery doubles at half 1 of ladder window 0 (group_schedule.window_candidates)
+  rec_comb      the same for the comb: at its first, middle, second-to-last and last non-zero row, doubling and cancelling
+  rec_infinity  s = e / k: s R = e G, so Q = infinity and the recovery fails
+The rec_* signatures are built from each invoice's own signing hash e, which covers the hrp and the data words but not the
+signature: R = k G (R.x < n), r = R.x, recovery id R.y & 1, so the recovery's x-only point E = lift_x(r) has the discrete
+log d = k or n - k, u1 = -e / r is fixed, and s = +-u2 r sets u2 to any value (group_schedule's `main` schedule, as
+k_main<SV_KIND_SCHNORR> runs it).  Not covered: recovery ids 2 / 3 at these additions (R is then a curve point picked by
+its x in [n, p), with no known discrete log, so u2 d cannot be steered) and u1 = 0 (e = 0 mod n needs a SHA-256
+preimage).  Their bytes come from SHA-256, so the rng stream of the items before them is unchanged; rec_k holds each
+one's k (zero elsewhere), and the key Python computes, Q = (u1 + u2 d) G, must equal CLN's.
 Each item records bolt11_decode's result (bit 0) and bolt11_decode_nosig's (bit 1), the receiver_id, the signing hash and
 both failure messages.  recover_*: (signature, recovery id, message) triples with secp256k1_ecdsa_recover's answer,
 including Q = infinity (s R = e G) and the refusals before any point arithmetic.
@@ -34,6 +44,8 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 from tests import bolt11, ecc  # noqa: E402
+from tests import group_fixture as F  # noqa: E402
+from tests import group_schedule as S  # noqa: E402
 
 P, N = ecc.P, ecc.N
 CHARSET = bolt11.CHARSET
@@ -102,7 +114,10 @@ def sqrt_p(a):
 class Gen:
     def __init__(self, rng):
         self.rng = rng
+        self.stream = None  # once set, rb() hashes this prefix and a counter instead of drawing from rng
+        self.nb = 0
         self.items = []  # (bytes, label)
+        self.rec = {}    # item index -> (k, key33 or None): the recovery groups' nonce and the key Python computes
         self.nk = 0
 
     def key(self):
@@ -111,7 +126,13 @@ class Gen:
         return sk, ecc.pubkey_create(sk)[0]
 
     def rb(self, n):
-        return bytes(self.rng.integers(0, 256, n, dtype=np.uint8))
+        if self.stream is None:
+            return bytes(self.rng.integers(0, 256, n, dtype=np.uint8))
+        self.nb += 1
+        out = b""
+        while len(out) < n:
+            out += hashlib.sha256(self.stream + b" %d %d" % (self.nb, len(out))).digest()
+        return out[:n]
 
     def fields(self, with_n=None, desc=b"coffee", hints=0, extra=()):
         f = field("p", to_words(self.rb(32))) + field("s", to_words(self.rb(32))) + field("d", to_words(desc))
@@ -245,7 +266,55 @@ def build(rng):
         g.add(s_ok[:k], "trunc")
     for k in range(len(allw)):
         g.add(encode(hrp, allw[:k]), "trunc")
+    # recovery at the exceptional additions of its ladder and comb, and at Q = infinity: bytes from SHA-256, not from rng
+    g.stream = b"make_bolt11 rec"
+    for i in range(6):
+        for u2, _, _ in S.window_candidates(0):
+            rec_invoice(g, "rec_window", i, lambda u1, d, u2=u2: u2)
+    for i in range(4):
+        for row in (0, 1, 2, 3):  # first, middle, second-to-last and last non-zero comb digit of u1
+            for sign in (1, -1):
+                rec_invoice(g, "rec_comb", i, lambda u1, d, row=row, sign=sign: (
+                    F._row_target(u1, comb_rows(u1)[row], sign) * pow(d, -1, N)))
+    for i in range(6):
+        rec_invoice(g, "rec_infinity", i, lambda u1, d: -u1 * pow(d, -1, N))  # u2 d = -u1: s = e / k
     return g
+
+
+def comb_rows(u1):
+    rows = [j for j, v in enumerate(S.prepare_u1(u1)) if v]
+    return rows[0], rows[len(rows) // 2], rows[-2], rows[-1]
+
+
+def rec_invoice(g, label, i, u2_of):
+    """a signed-style invoice (no `n`) whose signature makes the recovery run u1 = -e / r and u2 = u2_of(u1, d), d the
+    discrete log of E = lift_x(r): R = k G with k from SHA-256 (skipping R.x >= n), r = R.x, recid = R.y & 1, so d = k or
+    n - k, and s = +-u2 r.  Records k and Q = (u1 + u2 d) G, compressed (None at infinity)."""
+    hrp, w = "lnbc", g.body(g.fields(None))
+    e = int.from_bytes(bolt11.signing_hash(hrp, w), "big") % N
+    for ctr in range(100):
+        k = int.from_bytes(hashlib.sha256(b"make_bolt11 rec_k %s %d %d %d" % (label.encode(), i, len(g.items), ctr))
+                           .digest(), "big") % N
+        if not k:
+            continue
+        x, y = ecc.base_mult(k)
+        if x >= N:
+            continue
+        recid, d = y & 1, (N - k if y & 1 else k)
+        u1 = -e * pow(x, -1, N) % N
+        u2 = u2_of(u1, d) % N
+        s = (-u2 if recid else u2) * x % N
+        if s:
+            break
+    else:
+        raise AssertionError((label, i))
+    q = (u1 + u2 * d) % N
+    key = None
+    if q:
+        qx, qy = ecc.base_mult(q)
+        key = bytes([2 + (qy & 1)]) + b32(qx)
+    g.rec[len(g.items)] = (k, key)
+    g.add(encode(hrp, w + to_words(b32(x) + b32(s) + bytes([recid]))), label)
 
 
 def recover_vectors(rng):
@@ -286,6 +355,11 @@ def main():
         ret[i] = lib.cln_bolt11_check(s, ctypes.c_size_t(len(s)), node[i].ctypes.data, h[i].ctypes.data, f, nf)
         fail.append(f.value.decode("utf-8", "replace"))
         nfail.append(nf.value.decode("utf-8", "replace"))
+    rec_k = np.zeros((n, 32), np.uint8)
+    for i, (k, key) in g.rec.items():  # CLN's answer and the Python arithmetic must agree
+        rec_k[i] = np.frombuffer(b32(k), np.uint8)
+        assert (ret[i] & 1, node[i].tobytes()) == ((1, key) if key else (0, bytes(33))), (i, g.items[i][1])
+        assert key or fail[i] == "signature recovery failed", (i, fail[i])
     rv = recover_vectors(rng)
     rsig = np.frombuffer(b"".join(v[0] for v in rv), np.uint8).reshape(-1, 64)
     rrec = np.array([v[1] for v in rv], np.int32)
@@ -298,7 +372,7 @@ def main():
     np.savez_compressed(
         bolt11.FIXTURE, blob=np.frombuffer(bytes(blob), np.uint8), off=np.array(off, np.uint64), len=np.array(ln, np.uint32),
         ret=ret, node=node, hash=h, fail=np.array(fail), nosig_fail=np.array(nfail), labels=np.array(labels),
-        label=np.array([labels.index(lab) for _, lab in g.items], np.uint8),
+        label=np.array([labels.index(lab) for _, lab in g.items], np.uint8), rec_k=rec_k,
         recover_sig=rsig, recover_recid=rrec, recover_msg=rmsg, recover_ok=rok, recover_key=rkey)
     st = bolt11.expected_status(ret, np.array(fail), np.array(labels)[[labels.index(lab) for _, lab in g.items]])
     print(f"{n} invoices, blob {len(blob)} bytes; expected status 1/0/-1/unchecked: {(st == 1).sum()}/{(st == 0).sum()}/"

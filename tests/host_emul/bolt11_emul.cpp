@@ -5,10 +5,11 @@
 // verify_curve_side: the rules every verification route shares) or the recovery (b11_recover_prep, the x-only key decode
 // and ecmult_uniform that k_main<SV_KIND_SCHNORR> runs, schnorr_park, b11_recover_final_batch).  What this cannot check is
 // the packing of the two groups and the launches themselves; tests/test_gpu_bolt11.py does that on the device.  The comb
-// table is the one emul.cpp builds (read through emul_gtable_get).
+// table is the one emul.cpp builds (read through emul_gtable_get).  The group law logs its branches into emul.cpp's log.
 #include <cstring>
 #include <vector>
 #include "../../lightning_b200/csrc/common.cuh"
+#include "ge_trace.h"
 #include "../../lightning_b200/csrc/bolt11.cuh"
 
 extern "C" void emul_gtable_get(u32 e, u32* xy16);  // emul.cpp
@@ -27,8 +28,8 @@ static const ge_mem* b11_gtable() {
     return g_b11_table.data();
 }
 
-// the recovery alone: status 1 with the compressed key, 0 (key zeros) where secp256k1_ecdsa_recover fails
-static int b11_recover_host(const u8* sig64, u8 recid, const u8* msg32, u8* out33) {
+// the recovery up to the parked result, as k_b11_rec_prep and k_main<SV_KIND_SCHNORR> leave it
+static void b11_recover_park(sv_jac* j, const u8* sig64, u8 recid, const u8* msg32) {
     sv_work w;
     u8 x32[32];
     b11_recover_prep(w, x32, sig64, recid, msg32);
@@ -38,8 +39,13 @@ static int b11_recover_host(const u8* sig64, u8 recid, const u8* msg32, u8* out3
     qtab_entry tab[8];
     gej R;
     ecmult_uniform(R, &w, E, b11_gtable(), tab);
+    schnorr_park(j, R, ok);
+}
+
+// the recovery alone: status 1 with the compressed key, 0 (key zeros) where secp256k1_ecdsa_recover fails
+static int b11_recover_host(const u8* sig64, u8 recid, const u8* msg32, u8* out33) {
     sv_jac j;
-    schnorr_park(&j, R, ok);
+    b11_recover_park(&j, sig64, recid, msg32);
     int st;
     b11_recover_final_batch(&st, out33, &j, 1);
     return st;
@@ -73,6 +79,16 @@ int emul_bolt11(const u8* s, u32 span, u8* hash32, u8* node33, int* have_n) {
 
 int emul_bolt11_recover(const u8* sig64, int recid, const u8* msg32, u8* out33) {
     return b11_recover_host(sig64, (u8)recid, msg32, out33);
+}
+
+// cnt (1 .. SV_FINAL_BATCH) recoveries parked side by side and finished by one b11_recover_final_batch, as one thread of
+// k_b11_rec_final finishes them; -1 for any other cnt
+int emul_bolt11_recover_batch(const u8* sig64, const int* recid, const u8* msg32, int cnt, int* status, u8* key33) {
+    if (cnt < 1 || cnt > SV_FINAL_BATCH) return -1;
+    sv_jac j[SV_FINAL_BATCH];
+    for (int i = 0; i < cnt; i++) b11_recover_park(&j[i], sig64 + 64 * i, (u8)recid[i], msg32 + 32 * i);
+    b11_recover_final_batch(status, key33, j, cnt);
+    return 0;
 }
 
 }  // extern "C"

@@ -14,11 +14,13 @@
 #include <cstring>
 #include <vector>
 #include "../../lightning_b200/csrc/common.cuh"
-// branch log of the group law (ge.cuh SV_GE_TRACE): one byte per addition, SV_GE_MIXED / SV_GE_FULL | SV_GE_ADD_*, kept
-// per thread and only while a caller of emul_trace_* has switched it on (the second lane of a pair runs on a thread of its
-// own and is not logged: both lanes take the same branches)
-static thread_local std::vector<unsigned char>* g_trace = nullptr;
-#define SV_GE_TRACE(ev) do { if (g_trace) g_trace->push_back((unsigned char)(ev)); } while (0)
+// branch log of the group law (ge_trace.h): the second lane of a pair runs on a thread of its own and is not logged, both
+// lanes take the same branches
+#include "ge_trace.h"
+std::vector<unsigned char>*& emul_trace_log() {
+    static thread_local std::vector<unsigned char>* log = nullptr;
+    return log;
+}
 struct fe;
 // host stand-in for the warp shuffle between the two lanes of a pair (verify.cuh pair_swap): the lanes are two threads
 // that meet at a mailbox; a sense-reversing barrier on atomics orders the exchange
@@ -204,10 +206,10 @@ void emul_selftest_group(int op, const u32* in, size_t n, u32* out) {
 static std::vector<unsigned char> g_trace_buf;
 void emul_trace_begin(void) {
     g_trace_buf.clear();
-    g_trace = &g_trace_buf;
+    emul_trace_log() = &g_trace_buf;
 }
 size_t emul_trace_end(u8* out, size_t cap) {
-    g_trace = nullptr;
+    emul_trace_log() = nullptr;
     size_t n = g_trace_buf.size();
     if (out) memcpy(out, g_trace_buf.data(), n < cap ? n : cap);
     return n;

@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 
 from tests import bolt11
+from tests import group_schedule as S
 
 P8 = ctypes.POINTER(ctypes.c_uint8)
 
@@ -64,6 +65,18 @@ def test_fixture_coverage(fx):
     hs = lab == "high_s"
     assert (e[hs] == 1).sum() > 0 and (e[hs] == 0).sum() > 0
     assert max(fx["len"][lab == "long"]) > 2000
+    # recovery at its exceptional additions: the ladder's window-0 doubling, every comb case and Q = infinity
+    assert (lab == "rec_window").sum() >= 4 and np.all(e[lab == "rec_window"] == 1)
+    assert (lab == "rec_infinity").sum() >= 4 and np.all(e[lab == "rec_infinity"] == 0)
+    cases = collections.Counter()
+    for i in np.nonzero(lab == "rec_comb")[0]:
+        comb = [br for _, step, br in S.schedule("main", *bolt11.rec_scalars(fx, i)).steps if step == "comb"]
+        hit = [br for br in comb if br in (S.DOUBLE, S.INFINITY)]
+        assert len(hit) == 1, (i, comb)
+        case = (S.BRANCH[hit[0]], comb[-1] == hit[0])  # (branch, at the last row)
+        cases[case] += 1
+        assert e[i] == (0 if case == ("infinity", True) else 1), (i, case)
+    assert min(cases[(br, last)] for br in ("double", "infinity") for last in (False, True)) >= 4, cases
     # invoices refused for a field value the engine does not check stay in the corpus, counted by message
     unchecked = collections.Counter(f for f, x in zip(fx["fail"], e) if x == bolt11.UNCHECKED)
     assert sum(unchecked.values()) > 0
@@ -95,15 +108,60 @@ def test_host_build_takes_the_n_path(fx, emul):
     np.testing.assert_array_equal(have_n.astype(bool), want)
 
 
+def _recover_batch(emul, fx, idx):
+    """the recovery vectors idx parked side by side and finished by one b11_recover_final_batch -> (status, keys)"""
+    n = len(idx)
+    st = np.zeros(n, np.int32)
+    keys = np.zeros((n, 33), np.uint8)
+    sig = np.ascontiguousarray(fx["recover_sig"][idx])
+    rc = np.ascontiguousarray(fx["recover_recid"][idx], np.int32)
+    msg = np.ascontiguousarray(fx["recover_msg"][idx])
+    assert emul.emul_bolt11_recover_batch(sig.ctypes.data_as(P8), rc.ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
+                                          msg.ctypes.data_as(P8), n, st.ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
+                                          keys.ctypes.data_as(P8)) == 0
+    return st, keys
+
+
+def _final_batches(ok):
+    """groups of recovery vectors for one batched final each.  The last 16 vectors (make_bolt11.py: 8 at Q = infinity,
+    then the 8 refusal candidates) each sit in every slot of a group of 16 among ordinary vectors; then a short tail
+    group, a group with nothing usable, and groups where only slot 0 or only slot 15 is usable."""
+    n = len(ok)
+    ordinary, special = np.arange(n - 16), np.arange(n - 16, n)
+    unusable, usable = np.nonzero(ok == 0)[0], np.nonzero(ok == 1)[0]
+    groups, seen = [], set()
+    for rot in range(16):
+        for j, v in enumerate(special):
+            slot = (j + rot) % 16
+            g = np.insert(ordinary[(15 * (16 * rot + j) + np.arange(15)) % len(ordinary)], slot, v)
+            seen.add((int(v), slot))
+            groups.append(g)
+    assert len(seen) == 16 * 16
+    groups.append(np.array([ordinary[0], special[0], ordinary[1], special[8], special[15], ordinary[2], special[3]]))
+    groups.append(unusable)
+    filler = np.resize(unusable, 15)
+    groups += [np.concatenate([usable[:1], filler]), np.concatenate([filler, usable[-1:]])]
+    return groups
+
+
 def test_recovery_matches_libsecp(fx, emul, cln11):
-    """the recovery alone against secp256k1_ecdsa_recover: key, refusals and Q = infinity"""
+    """the recovery alone against secp256k1_ecdsa_recover: key, refusals and Q = infinity, one at a time and in batched
+    finals (one inversion over up to 16 parked results, where an unusable one must not disturb its neighbours)"""
     emul.emul_bolt11_recover.restype = ctypes.c_int
     emul.emul_bolt11_recover.argtypes = [ctypes.c_char_p, ctypes.c_int, ctypes.c_char_p, P8]
+    emul.emul_bolt11_recover_batch.restype = ctypes.c_int
     out = np.zeros(33, np.uint8)
-    for i in range(len(fx["recover_ok"])):
+    n = len(fx["recover_ok"])
+    want_ok, want_key = np.zeros(n, np.int32), np.zeros((n, 33), np.uint8)
+    for i in range(n):
         sig, rc, msg = fx["recover_sig"][i].tobytes(), int(fx["recover_recid"][i]), fx["recover_msg"][i].tobytes()
         ok, key = bolt11.ref_recover(cln11, sig, rc, msg)
         assert (ok, key) == (fx["recover_ok"][i], fx["recover_key"][i].tobytes()), i
         got = emul.emul_bolt11_recover(sig, rc, msg, out.ctypes.data_as(P8))
         assert (got, out.tobytes()) == (ok, key), i
-    assert fx["recover_ok"].sum() > 0 and (fx["recover_ok"] == 0).sum() >= 8
+        want_ok[i], want_key[i] = ok, np.frombuffer(key, np.uint8)
+    assert want_ok.sum() > 0 and (want_ok[n - 16:n - 8] == 0).all() and (want_ok == 0).sum() >= 14
+    for g in _final_batches(want_ok):
+        st, keys = _recover_batch(emul, fx, g)
+        bad = np.nonzero((st != want_ok[g]) | (keys != want_key[g]).any(axis=1))[0]
+        assert bad.size == 0, (g.tolist(), bad.tolist())

@@ -36,23 +36,37 @@ def _run(engine, fx, idx):
     return engine.verify_bolt11_spans(fx["blob"], fx["off"][idx], fx["len"][idx])
 
 
+@pytest.fixture(scope="module")
+def default_answers(engine, fx):
+    """status and receiver_id of every item under the default settings"""
+    st, node, _ = _run(engine, fx, np.arange(len(fx["ret"])))
+    return st, node
+
+
 @pytest.mark.parametrize("small_max", [None, 0], ids=["small_batch_kernel", "throughput_kernels"])
 @pytest.mark.parametrize("nosqrt", [1, 0], ids=["nosqrt", "plain"])
-def test_fixture_every_item(engine, fx, small_max, nosqrt):
+def test_fixture_every_item(engine, fx, default_answers, small_max, nosqrt):
+    """every item under each setting; no answer, CLN's or one it leaves unchecked, depends on the setting (recovery runs
+    the same kernels under all of them)"""
     default = engine.small_max()
     try:
         if small_max is not None:
             engine.set_small_max(small_max)
         engine.set_nosqrt(nosqrt)
         idx = np.arange(len(fx["ret"]))
-        _check(fx, idx, *_run(engine, fx, idx))
+        st, node, h = _run(engine, fx, idx)
+        _check(fx, idx, st, node, h)
+        np.testing.assert_array_equal(st, default_answers[0])
+        np.testing.assert_array_equal(node, default_answers[1])
     finally:
         engine.set_small_max(default)
         engine.set_nosqrt(1)
 
 
 def test_batch_sizes(engine, fx):
-    """1, 31, 33, 8,192 and 40,000 invoices, and 9,000 `n` invoices: above the small-batch limit on their own"""
+    """1, 31, 33, 8,192 and 40,000 invoices, 9,000 `n` invoices: above the small-batch limit on their own, and one wave of
+    k_main plus one recovered invoices, with Q = infinity and window-0 doublings at the edges of the final's groups and of
+    the wave (the grid-stride loop's second pass)"""
     rng = np.random.default_rng(11)
     n_items = len(fx["ret"])
     for size in (1, 31, 33, 8192, 40000):
@@ -61,6 +75,15 @@ def test_batch_sizes(engine, fx):
     with_n = np.nonzero(fx["label_name"] == "signed_n")[0]
     assert engine.small_max() < 9000
     idx = np.concatenate([with_n[rng.integers(0, len(with_n), 9000)], rng.integers(0, n_items, 1000)])
+    _check(fx, idx, *_run(engine, fx, idx))
+    info = engine.info()
+    wave = info["main_grid"] * info["main_block"]
+    lab = fx["label_name"]
+    signed = np.nonzero(lab == "signed")[0]
+    inf, win = np.nonzero(lab == "rec_infinity")[0], np.nonzero(lab == "rec_window")[0]
+    idx = signed[rng.integers(0, len(signed), wave + 1)]
+    for k, pos in enumerate((0, 15, 16, wave - 1, wave)):  # wave: the last item, alone in the second pass
+        idx[pos] = inf[k] if k % 2 == 0 else win[k]
     _check(fx, idx, *_run(engine, fx, idx))
 
 
@@ -78,19 +101,30 @@ def test_strings_and_bytes(engine, fx):
 
 
 def _special(fx):
-    """a -1, a 0, an `n` item and a recovery-id-3 item"""
+    """a -1, a 0, an `n` item, a recovery-id-3 item, and two recovered invoices whose recovery fails after the ladder: Q at
+    infinity and R.x off the curve"""
     lab, e = fx["label_name"], fx["expected"]
     # make_bolt11.py builds the recid23 items in pairs, recovery id 2 then 3
     pick = [np.nonzero(lab == "charset")[0][0], np.nonzero(lab == "recid_high")[0][0],
-            np.nonzero(lab == "signed_n")[0][0], np.nonzero(lab == "recid23")[0][1]]
-    assert [e[i] for i in pick] == [-1, 0, 1, 1]
+            np.nonzero(lab == "signed_n")[0][0], np.nonzero(lab == "recid23")[0][1],
+            np.nonzero(lab == "rec_infinity")[0][0], np.nonzero(lab == "off_curve")[0][0]]
+    assert [e[i] for i in pick] == [-1, 0, 1, 1, 0, 0]
     return pick
 
 
 @pytest.mark.parametrize("small_max", [None, 0], ids=["small_batch_kernel", "throughput_kernels"])
 def test_isolation(engine, fx, small_max):
-    """a -1, a 0, an `n` item and a recovery-id-3 item at every offset of a batch change no other item's answer"""
-    base = np.nonzero(np.isin(fx["label_name"], ["signed", "signed_n", "high_s"]))[0][:47]
+    """a -1, a 0, an `n` item, a recovery-id-3 item, Q = infinity and R.x off the curve at every offset of a batch change
+    no other item's answer"""
+    lab, e = fx["label_name"], fx["expected"]
+    base = np.nonzero(np.isin(lab, ["signed", "signed_n", "high_s"]))[0][:47]
+    # the recovered invoices of the base (no `n`; high-S ones recover, with `n` they are refused): a recovered special
+    # item's index among the recovered ones is how many precede it, and k_b11_rec_final finishes them 16 to a thread, so
+    # over all offsets it must take every slot of a group and also land in the short last group
+    rec = (lab[base] == "signed") | ((lab[base] == "high_s") & (e[base] == 1))
+    at = {int(rec[:pos].sum()) for pos in range(len(base) + 1)}
+    total = int(rec.sum()) + 1
+    assert {a % 16 for a in at} == set(range(16)) and total % 16 and max(at) >= total // 16 * 16, (at, total)
     default = engine.small_max()
     try:
         if small_max is not None:

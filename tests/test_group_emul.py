@@ -13,7 +13,7 @@ from collections import Counter, defaultdict
 import numpy as np
 import pytest
 
-from tests import adversarial
+from tests import adversarial, bolt11
 from tests import group_cases as C
 from tests import group_fixture as F
 from tests import group_schedule as S
@@ -155,8 +155,29 @@ def model_name(route):
     return {"small_pair": "small", "samekey": "main"}.get(route, route)
 
 
+def recovery_items():
+    """(invoice, u1, u2, d) of the BOLT11 invoices built to steer the key recovery (make_bolt11.py rec_*)"""
+    fx = bolt11.load_fixture()
+    invs = bolt11.invoices(fx)
+    for i in np.nonzero(np.char.startswith(fx["label_name"], "rec_"))[0]:
+        yield (invs[i],) + bolt11.rec_scalars(fx, i)
+
+
+def trace_recovery(emul, inv):
+    """branch log of one invoice through bolt11.cuh's host build (parse, hash, and the recovery's `main` schedule)"""
+    h, node = np.zeros(32, np.uint8), np.zeros(33, np.uint8)
+    have_n = ctypes.c_int()
+    buf = np.zeros(4096, np.uint8)
+    emul.emul_trace_begin()
+    emul.emul_bolt11(inv, ctypes.c_uint32(len(inv)), ptr(h), ptr(node), ctypes.byref(have_n))
+    n = emul.emul_trace_end(ptr(buf), ctypes.c_size_t(buf.size))
+    assert n <= buf.size and have_n.value == 0
+    return [int(v) for v in buf[:n]]
+
+
 def test_schedule_model_matches_host_branch_log(eng, emul):
-    """every item through every schedule the host build has: the model's predicted branch sequence == the log"""
+    """every item through every schedule the host build has, and the BOLT11 recoveries through theirs: the model's
+    predicted branch sequence == the log"""
     rs = routes(emul)
     checked = Counter()
     try:
@@ -173,6 +194,9 @@ def test_schedule_model_matches_host_branch_log(eng, emul):
                 checked[route] += 1
     finally:
         emul.emul_set_ecdsa33_exact(0)
+    for inv, u1, u2, d in recovery_items():
+        assert trace_recovery(emul, inv) == S.schedule("main", u1, u2, d).codes(), (inv, hex(u1), hex(u2), hex(d))
+        checked["recovery"] += 1
     assert min(checked.values()) >= 40, checked
 
 
@@ -213,6 +237,10 @@ def coverage():
         for name in S.SCHEDULES:
             for c in S.classes(S.schedule(name, u1, u2, d, rpn), name):
                 cov[f"{fam}.{name}"][c] += 1
+    # BOLT11 key recovery: the `main` schedule of k_main<SV_KIND_SCHNORR>, with u2 as free as in ECDSA
+    for _, u1, u2, d in recovery_items():
+        for c in S.classes(S.schedule("main", u1, u2, d), "main"):
+            cov["recovery.main"][c] += 1
     return cov
 
 
@@ -221,6 +249,8 @@ def test_every_reachable_step_class_is_hit():
     for name, reach in S.REACH.items():
         missing = [c for c in reach if not cov[f"ecdsa.{name}"][c]]
         assert not missing, (name, missing)
+    missing = [c for c in S.REACH["main"] if not cov["recovery.main"][c]]
+    assert not missing, ("recovery.main", missing)
     # BIP-340: the classes that tie u1 to u2*d
     assert cov["bip340.main"][("comb", "double")] and cov["bip340.main"][("comb", "infinity")]
     for c in (("join2", "double"), ("join2", "infinity"), ("join2", "b_inf")):
